@@ -1,4 +1,4 @@
-"""code2vec_b200: B200-native (sm_100a) backend for code2vec's path-attention hot path.
+"""code2vec_b200: H100-native (sm_90a) backend for code2vec's path-attention hot path.
 
 Layout: ``csrc/`` CUDA kernels + the C ABI (include/c2v_b200.h) -> ``libc2v_b200.so``;
 ``engine.py`` ctypes binding + storage; the host-side mirror of the reference's model / config /

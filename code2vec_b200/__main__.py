@@ -1,4 +1,4 @@
-"""`python -m code2vec_b200 ...`: the reference's command line (code2vec.py:16-38) on the B200 backends.
+"""`python -m code2vec_b200 ...`: the reference's command line (code2vec.py:16-38) on the engine's backends.
 
 Same flags (`Config.arguments_parser`, reference config.py:11-44) and the same order of actions:
 train, export word2vec files, evaluate (or release), predict.  `--predict` differs in one respect: the

@@ -134,7 +134,7 @@ class Code2VecModel(Code2VecModelBase):
         self.log("b200 backend arithmetic: train = %s, evaluate/predict = %s (C2V_MATH=fp32|tf32|3xtf32 forces one for both)" % (
             {0: "fp32 FFMA", 1: "tf32 tensor cores", 2: "3xTF32 tensor cores (fp32-equivalent)"}[self._math_train],
             {0: "fp32 FFMA", 1: "tf32 tensor cores", 2: "3xTF32 tensor cores (fp32-equivalent)"}[self._math_eval]))
-        # C2V_HINT_NEXT=1: pass each next batch to the engine (c2v_hint_next_batch); no measured gain on one GPU
+        # C2V_HINT_NEXT=1: pass each next batch to the engine (c2v_hint_next_batch); off by default
         self._hint_next = os.environ.get("C2V_HINT_NEXT", "0") == "1"
         if self.config.is_training:
             self.trainer = Trainer(self.engine, keep_prob=self.config.DROPOUT_KEEP_RATE, seed=int(time.time()) & 0x7FFFFFFF,

@@ -1,4 +1,4 @@
-"""Builds libc2v_b200.so (the C-ABI shared library) in-tree with nvcc for sm_100a.
+"""Builds libc2v_b200.so (the C-ABI shared library) in-tree with nvcc for sm_90a (H100).
 
 The library is the product's only compute path; there is no CPU fallback.  `python -m
 code2vec_b200.build` (or __graft_entry__.build()) cross-compiles without a GPU.
@@ -18,7 +18,7 @@ OBJ_DIR = os.path.join(PKG_DIR, "csrc", "_obj")
 
 SOURCES = ["engine.cu"]
 NVCC_FLAGS = [
-    "-gencode", "arch=compute_100a,code=sm_100a", "-O3", "-lineinfo", "-std=c++17",
+    "-gencode", "arch=compute_90a,code=sm_90a", "-O3", "-lineinfo", "-std=c++17",
     "-Xcompiler", "-fPIC", "--expt-relaxed-constexpr",
 ]
 
@@ -43,7 +43,9 @@ def _newest_source_mtime() -> float:
 
 
 def needs_build() -> bool:
-    return (not os.path.exists(LIB_PATH)) or os.path.getmtime(LIB_PATH) < _newest_source_mtime()
+    # this file counts as a source: it holds NVCC_FLAGS (the target architecture among them)
+    newest = max(_newest_source_mtime(), os.path.getmtime(os.path.abspath(__file__)))
+    return (not os.path.exists(LIB_PATH)) or os.path.getmtime(LIB_PATH) < newest
 
 
 def build(force: bool = False, verbose: bool = False) -> str:

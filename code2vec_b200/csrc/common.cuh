@@ -1,4 +1,4 @@
-// Shared device helpers for the path-attention engine (sm_100a only).
+// Shared device helpers for the path-attention engine (sm_90a only).
 #pragma once
 #include <cuda_runtime.h>
 #include <stdint.h>

@@ -16,8 +16,6 @@
 #include "kernels.cuh"
 #include "sgemm.cuh"
 #include "umma_gemm.cuh"
-#include "umma_gemm2.cuh"
-#include "ctx_fused.cuh"
 
 using namespace c2v;
 
@@ -83,7 +81,7 @@ Workspace carve(const c2v_dims& d) {
   if ((size_t)kSplitDw * X * D > part) part = (size_t)kSplitDw * X * D;
   w.part = take(part * 4);
   w.da_part = take(B * D * 4);
-  w.lse_part = take(B * 2 * (((size_t)d.target_vocab + 255) / 256) * 8);   // (max, sum exp) per (row, 128-col half tile)
+  w.lse_part = take(B * (size_t)umma::lse_slots(d.target_vocab) * 8);   // (max, sum exp) per (row, partial slot)
   w.dl = take(B * (size_t)(kMaxSampled + 1) * 4);     // sampled softmax: dL/dlogits [B, 1+S]
   w.st_src = take(N * 4);
   w.st_pth = take(N * 4);
@@ -182,8 +180,7 @@ struct c2v_engine {
   bool bkt_zeroed = false;   // the bucket counters have been cleared once (bucket_scan_kernel leaves them cleared)
   int recompute = 0;         // option "recompute_logits" (tensor-core modes, single-GPU step): the logits GEMM runs twice -- once for the
                              // log-sum-exp only, once writing dL/dlogits from its epilogue -- instead of writing logits and rewriting them.
-                             // Measured: logits 0.42 + xent 0.36 -> 0.69 + 0.02 ms in tf32 (the LSE-only pass is epilogue-bound too), but
-                             // 6.3 -> 7.1 ms in 3xTF32 (a third 3x GEMM and a second table split): off by default
+                             // In 3xTF32 it costs a third 3x GEMM and a second table split: off by default
   int exp_slab = 1;          // option "exp_slab" (tensor-core modes, single-GPU full-softmax step; default on): the logits epilogue writes
                              // U = exp(s - true logit) and the softmax's normalisation is deferred into per-row factors applied by the
                              // dv / dY GEMMs, so no pass re-reads the slab to turn logits into dL/dlogits (DESIGN.md section 4.9).  Rows
@@ -191,18 +188,17 @@ struct c2v_engine {
   bool slab_flag_zeroed = false;
   bool slab_exp_live = false;         // c2v_target_forward left U (not logits) in the slab: c2v_target_backward finishes that schedule
   int gather_occ[2] = {0, 0};         // resident CTAs per SM of gather_ctx_kernel<false / true>, queried once
-  int adam_epi_prefetch = 0; // option "adam_epilogue_prefetch" (measured slower, off): the dY epilogue's Adam update prefetches its (theta, m, v)
+  int adam_epi_prefetch = 0; // option "adam_epilogue_prefetch" (off by default): the dY epilogue's Adam update prefetches its (theta, m, v)
                              // lines into L2 one tile ahead
   const float* row_scale = nullptr;   // while the step's dv GEMM runs: the per-example factor its split-K reduction applies
-  int fuse_sg = 0;           // option "fuse_softmax_grad": dv / dY compute dL/dlogits from the logits slab on the fly (tf32 mode).
-                             // Correct, and it removes the 2.1 GB softmax-gradient pass (0.36 -> 0.02 ms), but with 32-bit operands the two
-                             // GEMMs are already shared-memory-bandwidth bound and the in-place rewrite of the A stage costs more than
-                             // it saves on B200 (dv 0.34 -> 0.63 ms, dY 0.69 -> 1.02 ms): off by default
+  int fuse_sg = 0;           // option "fuse_softmax_grad": dv / dY compute dL/dlogits from the logits slab on the fly (tf32 mode):
+                             // the GEMM's loaders transform each A element on its way into shared memory, which removes the 2.1 GB
+                             // softmax-gradient pass but takes the A operand off TMA; off by default
   bool sg_live = false;      // ws.S holds LOGITS and sg describes how dv / dY turn them into dL/dlogits
   umma::SoftmaxGradArgs sg{};
-  int fuse_gather = 0;       // option "fuse_gather": gather -> projection -> tanh as one kernel on the tf32 path (ctx_fused.cuh);
-                             // bit-identical to the two-kernel path, but measured slower on B200 so far (0.31 vs 0.27 ms forward) -> off
-  int cta_pair = 2;          // tcgen05 GEMMs as CTA pairs (cta_group::2, UMMA 256 x BN): 0 never, 1 always, 2 auto
+  int fuse_gather = 0;       // option "fuse_gather": gather -> projection -> tanh as one kernel on the tf32 path (umma::launch_ctx_fused);
+                             // bit-identical to the two-kernel path; off by default
+  int cta_pair = 2;          // option "cta_pair": accepted and validated, no effect (the sm_90a GEMM has no CTA-pair form)
   int num_sms;
   cudaEvent_t ev_tgt_ready = nullptr;   // recorded after dY (caller-owned)
   int dy_late = 1;                      // where dY = P^T.v runs: 0 after dv, 1 inside context_backward, 2 on side2 after dv
@@ -218,7 +214,7 @@ struct c2v_engine {
   cudaEvent_t ev_fork2 = nullptr, ev_join2 = nullptr;
   bool dy_in_flight = false;            // a dY launched on side2 has not been joined yet
   // target-table Adam folded into the dY epilogue (c2v_arm_target_adam)
-  bool tgt_armed = false;               // the next tcgen05 dY product applies the update instead of storing dY
+  bool tgt_armed = false;               // the next tensor-core dY product applies the update instead of storing dY
   float tgt_lr = 0.f, tgt_b1 = 0.f, tgt_b2 = 0.f, tgt_eps = 0.f;
   int64_t tgt_t = 0;
   int64_t armed_t = 0;                  // step whose hyper-parameters c2v_arm_target_adam declared (0 = none)
@@ -289,21 +285,14 @@ struct PhaseTimer {
 inline int rest_ok(const c2v_engine* e) {
   return (e->rest_shortcut && e->hp_b1 > 0.f && e->hp_b1 <= 0.95f && e->hp_b2 >= 0.99f && e->hp_b2 < 1.f && e->hp_eps > 0.f) ? 1 : 0;
 }
-inline bool is_tc(const c2v_engine* e) { return e->math_mode != C2V_MATH_FP32; }          // tcgen05 GEMMs
+inline bool is_tc(const c2v_engine* e) { return e->math_mode != C2V_MATH_FP32; }          // tensor-core (wgmma) GEMMs
 inline bool is_3x(const c2v_engine* e) { return e->math_mode == C2V_MATH_3XTF32; }        // ... as 3xTF32
 
-// tcgen05 GEMM launchers: single-CTA (UMMA 128 x BN) or CTA-pair (UMMA 256 x BN).  Option "cta_pair":
-// 0 = never, 1 = always, 2 = auto (default): pairs wherever they measured faster on B200 -- every GEMM
-// except the two whose work items are few and long (dW: 3x2 tiles x split-K; dY: 1024-deep K), where the
-// halved item count costs more than the halved B traffic saves (profiles/r01_bench_*).
-#define C2V_PAIR(site_default) (e->cta_pair == 1 || (e->cta_pair == 2 && (site_default)))
-#define C2V_UMMA_192(...) (C2V_PAIR(true) ? umma::launch2<192, 6>(__VA_ARGS__) : umma::launch<192, 4>(__VA_ARGS__))
-#define C2V_UMMA_192_SINGLE(...) (C2V_PAIR(false) ? umma::launch2<192, 6>(__VA_ARGS__) : umma::launch<192, 4>(__VA_ARGS__))
-#define C2V_UMMA_256(...) (C2V_PAIR(true) ? umma::launch2<256, 6>(__VA_ARGS__) : umma::launch<256, 4>(__VA_ARGS__))
-// the same with the operand majors fixed at compile time (the fused-epilogue GEMMs each have one layout, so only
-// that instantiation is built): AMN / BMN = operand is M- resp. N-contiguous in memory
-#define C2V_UMMA_FIXED(BN, AMN, BMN, pair_default, EPI, ...)                                   \
-  (C2V_PAIR(pair_default) ? umma::launch2_cfg<BN, 6, AMN, BMN, EPI>(__VA_ARGS__) : umma::launch_cfg<BN, 4, AMN, BMN, EPI>(__VA_ARGS__))
+// tensor-core GEMM launchers (umma_gemm.cuh): runtime dispatch over the operand majors, or the majors fixed at compile
+// time (the fused-epilogue GEMMs each have one layout, so only that instantiation is built): AMN / BMN = operand is
+// M- resp. N-contiguous in memory
+#define C2V_UMMA(...) umma::launch(__VA_ARGS__)
+#define C2V_UMMA_FIXED(AMN, BMN, EPI, ...) umma::launch_cfg<AMN, BMN, EPI>(__VA_ARGS__)
 
 template <class T> T* wsp(c2v_engine* e, size_t off) { return reinterpret_cast<T*>(e->wbase + off); }
 
@@ -550,7 +539,7 @@ bool plan_buckets(c2v_engine* e, BucketPlan* bp, bool force = false) {
   if (e->table_world <= 1) return false;
   const c2v_dims& d = e->dims;
   // sort_peer_access: 0 never, 1 (default) when the tables are large enough for random peer accesses to thrash the TLB
-  // (measured: a loss at 1.1 GB of tables, 1.8-3.4x faster at 5 GB), 2 always; the inbox exchange always needs the order
+  // (the 2 GB threshold below), 2 always; the inbox exchange always needs the order
   const double table_bytes = ((double)d.token_vocab + d.path_vocab) * d.embed_dim * 4.0;
   if (!force && (e->sort_peer == 0 || (e->sort_peer == 1 && table_bytes < 2.0e9))) return false;
   const int W = e->table_world;
@@ -600,11 +589,11 @@ int run_ctx_fwd(c2v_engine* e, cudaStream_t st, const ContextSource& cs, const D
   { int rc0 = prepare_rows(e, st, cs); if (rc0) return rc0; }
   if (is_tc(e) && !is_3x(e) && e->fuse_gather && e->dims.embed_dim % 32 == 0 && cs.rows % 4 == 0 &&
       (((uintptr_t)cs.src | (uintptr_t)cs.pth | (uintptr_t)cs.tgt) % 16) == 0) {
-    // gather -> dropout -> projection -> tanh in one kernel (ctx_fused.cuh); X' is written out only when a backward
+    // gather -> dropout -> projection -> tanh in one kernel (umma::launch_ctx_fused); X' is written out only when a backward
     // pass will need it (dW = X'^T . dU)
     PhaseTimer pt(e, PH_CTX_FWD, st);
     umma::EpiTanhStore ep{H, (size_t)D};
-    C2V_LAUNCH(e, C2V_CUDA(e, (umma::launch_ctx_fused<192, 4>(st, cs.rows, D, e->theta.W, (size_t)D, cs, dp,
+    C2V_LAUNCH(e, C2V_CUDA(e, (umma::launch_ctx_fused(st, cs.rows, D, e->theta.W, (size_t)D, cs, dp,
                                                               keep_x ? wsp<float>(e, e->ws.Xg) : nullptr, ep, e->num_sms))));
     return C2V_OK;
   }
@@ -638,10 +627,10 @@ int run_ctx_fwd(c2v_engine* e, cudaStream_t st, const ContextSource& cs, const D
     umma::Operand opB{x3 ? wsp<float>(e, e->ws.W_hi) : e->theta.W, (size_t)D, true, x3 ? wsp<float>(e, e->ws.W_lo) : nullptr};
     if (x3) {
       umma::EpiTanhStorePrecise ep{H, (size_t)D};
-      C2V_LAUNCH(e, C2V_CUDA(e, (C2V_UMMA_FIXED(192, false, true, true, umma::EpiTanhStorePrecise, st, cs.rows, D, K, 1, opA, opB, ep, e->num_sms))));
+      C2V_LAUNCH(e, C2V_CUDA(e, (C2V_UMMA_FIXED(false, true, umma::EpiTanhStorePrecise, st, cs.rows, D, K, 1, opA, opB, ep, e->num_sms))));
     } else {
       umma::EpiTanhStore ep{H, (size_t)D};
-      C2V_LAUNCH(e, C2V_CUDA(e, (C2V_UMMA_FIXED(192, false, true, true, umma::EpiTanhStore, st, cs.rows, D, K, 1, opA, opB, ep, e->num_sms))));
+      C2V_LAUNCH(e, C2V_CUDA(e, (C2V_UMMA_FIXED(false, true, umma::EpiTanhStore, st, cs.rows, D, K, 1, opA, opB, ep, e->num_sms))));
     }
     return C2V_OK;
   }
@@ -654,7 +643,7 @@ int run_ctx_fwd(c2v_engine* e, cudaStream_t st, const ContextSource& cs, const D
 }
 
 // S[B, Y] = v . Ytab^T   (tensorflow_model.py:226,297)
-// with_lse (tf32 path only): also emit per-(row, 256-column tile) log-sum-exp partials into ws.lse_part.
+// with_lse (tf32 path only): also emit per-(row, partial slot) log-sum-exp partials (umma::lse_slots) into ws.lse_part.
 // grad != nullptr: the pass writes dL/dlogits (EpiSoftmaxGrad); lse_only: nothing but the log-sum-exp partials.
 struct LogitsGrad { const float* lse; const int32_t* target; int row0; float inv_batch; };
 // exp_offset != nullptr: the pass writes U = exp(logit - exp_offset[row]) and (max U, sum U) partials (EpiExpSum).
@@ -679,40 +668,40 @@ int run_logits(c2v_engine* e, cudaStream_t st, const float* v, int B, float* S, 
       opB.base = wsp<float>(e, e->ws.tgt_hi); opB.lo = wsp<float>(e, e->ws.tgt_lo);
     }
     PhaseTimer pt(e, PH_LOGITS, st);
-    const int slots = 2 * ((Y + 255) / 256);
+    const int slots = umma::lse_slots(Y);
     if (exp_offset && x3) {
       umma::EpiExpSumT<true, true> ep{S, wsp<float>(e, e->ws.S_lo), e->ws.ldS, exp_offset, wsp<float2>(e, e->ws.lse_part), slots};
-      C2V_LAUNCH(e, C2V_CUDA(e, (C2V_UMMA_FIXED(256, false, false, true, decltype(ep), st, B, Y, D, 1, opA, opB, ep, e->num_sms))));
+      C2V_LAUNCH(e, C2V_CUDA(e, (C2V_UMMA_FIXED(false, false, decltype(ep), st, B, Y, D, 1, opA, opB, ep, e->num_sms))));
     } else if (exp_offset) {
       umma::EpiExpSumT<false, false> ep{S, nullptr, e->ws.ldS, exp_offset, wsp<float2>(e, e->ws.lse_part), slots};
-      C2V_LAUNCH(e, C2V_CUDA(e, (C2V_UMMA_FIXED(256, false, false, true, decltype(ep), st, B, Y, D, 1, opA, opB, ep, e->num_sms))));
+      C2V_LAUNCH(e, C2V_CUDA(e, (C2V_UMMA_FIXED(false, false, decltype(ep), st, B, Y, D, 1, opA, opB, ep, e->num_sms))));
     } else if (gate && x3) {
       umma::EpiStoreLseGatedT<true> ep{{S, e->ws.ldS, wsp<float2>(e, e->ws.lse_part), slots}, gate};
-      C2V_LAUNCH(e, C2V_CUDA(e, (C2V_UMMA_FIXED(256, false, false, true, decltype(ep), st, B, Y, D, 1, opA, opB, ep, e->num_sms))));
+      C2V_LAUNCH(e, C2V_CUDA(e, (C2V_UMMA_FIXED(false, false, decltype(ep), st, B, Y, D, 1, opA, opB, ep, e->num_sms))));
     } else if (gate) {
       umma::EpiStoreLseGatedT<false> ep{{S, e->ws.ldS, wsp<float2>(e, e->ws.lse_part), slots}, gate};
-      C2V_LAUNCH(e, C2V_CUDA(e, (C2V_UMMA_FIXED(256, false, false, true, decltype(ep), st, B, Y, D, 1, opA, opB, ep, e->num_sms))));
+      C2V_LAUNCH(e, C2V_CUDA(e, (C2V_UMMA_FIXED(false, false, decltype(ep), st, B, Y, D, 1, opA, opB, ep, e->num_sms))));
     } else if (grad && x3) {
       umma::EpiSoftmaxGradT<true, true> ep{S, wsp<float>(e, e->ws.S_lo), e->ws.ldS, grad->lse, grad->target, grad->row0, grad->inv_batch, B};
-      C2V_LAUNCH(e, C2V_CUDA(e, (C2V_UMMA_FIXED(256, false, false, true, decltype(ep), st, B, Y, D, 1, opA, opB, ep, e->num_sms))));
+      C2V_LAUNCH(e, C2V_CUDA(e, (C2V_UMMA_FIXED(false, false, decltype(ep), st, B, Y, D, 1, opA, opB, ep, e->num_sms))));
     } else if (grad) {
       umma::EpiSoftmaxGradT<false, false> ep{S, nullptr, e->ws.ldS, grad->lse, grad->target, grad->row0, grad->inv_batch, B};
-      C2V_LAUNCH(e, C2V_CUDA(e, (C2V_UMMA_FIXED(256, false, false, true, decltype(ep), st, B, Y, D, 1, opA, opB, ep, e->num_sms))));
+      C2V_LAUNCH(e, C2V_CUDA(e, (C2V_UMMA_FIXED(false, false, decltype(ep), st, B, Y, D, 1, opA, opB, ep, e->num_sms))));
     } else if (lse_only && x3) {
       umma::EpiLseOnlyT<true> ep{{S, e->ws.ldS, wsp<float2>(e, e->ws.lse_part), slots}};
-      C2V_LAUNCH(e, C2V_CUDA(e, (C2V_UMMA_FIXED(256, false, false, true, decltype(ep), st, B, Y, D, 1, opA, opB, ep, e->num_sms))));
+      C2V_LAUNCH(e, C2V_CUDA(e, (C2V_UMMA_FIXED(false, false, decltype(ep), st, B, Y, D, 1, opA, opB, ep, e->num_sms))));
     } else if (lse_only) {
       umma::EpiLseOnlyT<false> ep{{S, e->ws.ldS, wsp<float2>(e, e->ws.lse_part), slots}};
-      C2V_LAUNCH(e, C2V_CUDA(e, (C2V_UMMA_FIXED(256, false, false, true, decltype(ep), st, B, Y, D, 1, opA, opB, ep, e->num_sms))));
+      C2V_LAUNCH(e, C2V_CUDA(e, (C2V_UMMA_FIXED(false, false, decltype(ep), st, B, Y, D, 1, opA, opB, ep, e->num_sms))));
     } else if (with_lse && x3) {
-      umma::EpiStoreLsePrecise ep{S, e->ws.ldS, wsp<float2>(e, e->ws.lse_part), 2 * ((Y + 255) / 256)};
-      C2V_LAUNCH(e, C2V_CUDA(e, (C2V_UMMA_FIXED(256, false, false, true, umma::EpiStoreLsePrecise, st, B, Y, D, 1, opA, opB, ep, e->num_sms))));
+      umma::EpiStoreLsePrecise ep{S, e->ws.ldS, wsp<float2>(e, e->ws.lse_part), umma::lse_slots(Y)};
+      C2V_LAUNCH(e, C2V_CUDA(e, (C2V_UMMA_FIXED(false, false, umma::EpiStoreLsePrecise, st, B, Y, D, 1, opA, opB, ep, e->num_sms))));
     } else if (with_lse) {
-      umma::EpiStoreLse ep{S, e->ws.ldS, wsp<float2>(e, e->ws.lse_part), 2 * ((Y + 255) / 256)};
-      C2V_LAUNCH(e, C2V_CUDA(e, (C2V_UMMA_FIXED(256, false, false, true, umma::EpiStoreLse, st, B, Y, D, 1, opA, opB, ep, e->num_sms))));
+      umma::EpiStoreLse ep{S, e->ws.ldS, wsp<float2>(e, e->ws.lse_part), umma::lse_slots(Y)};
+      C2V_LAUNCH(e, C2V_CUDA(e, (C2V_UMMA_FIXED(false, false, umma::EpiStoreLse, st, B, Y, D, 1, opA, opB, ep, e->num_sms))));
     } else {
       umma::EpiStore ep{S, e->ws.ldS, 0};
-      C2V_LAUNCH(e, C2V_CUDA(e, (C2V_UMMA_256(st, B, Y, D, 1, opA, opB, ep, e->num_sms))));
+      C2V_LAUNCH(e, C2V_CUDA(e, (C2V_UMMA(st, B, Y, D, 1, opA, opB, ep, e->num_sms))));
     }
     return C2V_OK;
   }
@@ -784,7 +773,7 @@ int context_backward(c2v_engine* e, cudaStream_t st, const ContextSource& cs, co
       umma::Operand opA{H, (size_t)D, false, H_lo};
       umma::Operand opB{x3 ? wsp<float>(e, e->ws.W_hi) : e->theta.W, (size_t)D, false, x3 ? wsp<float>(e, e->ws.W_lo) : nullptr};
       umma::EpiStore ep{dXg, (size_t)K3, 0};
-      C2V_LAUNCH(e, C2V_CUDA(e, (C2V_UMMA_192(st, N, K3, D, 1, opA, opB, ep, e->num_sms))));
+      C2V_LAUNCH(e, C2V_CUDA(e, (C2V_UMMA(st, N, K3, D, 1, opA, opB, ep, e->num_sms))));
     }
     if (e->lazy) {
       if (e->lazy_grads_pending)
@@ -833,7 +822,7 @@ int context_backward(c2v_engine* e, cudaStream_t st, const ContextSource& cs, co
       umma::Operand opB{H, (size_t)D, true, H_lo};
       const int ks = umma::effective_splits(N, kSplitDw);
       umma::EpiStore ep{part, (size_t)D, (size_t)K3 * D};
-      C2V_LAUNCH(e, C2V_CUDA(e, (C2V_UMMA_192_SINGLE(st, K3, D, N, kSplitDw, opA, opB, ep, e->num_sms))));
+      C2V_LAUNCH(e, C2V_CUDA(e, (C2V_UMMA(st, K3, D, N, kSplitDw, opA, opB, ep, e->num_sms))));
       rc = launch_colsum(e, st, part, (size_t)K3 * D, ks, K3 * D, e->grad.W);
       if (rc) return rc;
     }
@@ -893,17 +882,17 @@ int run_dv(c2v_engine* e, cudaStream_t st, int B, float* dv) {
       opB.base = wsp<float>(e, e->ws.tgt_hi); opB.lo = wsp<float>(e, e->ws.tgt_lo);
     }
     // enough split-K slices to fill the SMs about twice; few when the batch already gives many tiles
-    const int tiles = ((B + 127) / 128) * ((D + 191) / 192);
+    const int tiles = ((B + umma::BM - 1) / umma::BM) * ((D + umma::BN - 1) / umma::BN);
     int want = (2 * e->num_sms + tiles - 1) / tiles;
     if (want > kSplitDv) want = kSplitDv;
     const int ks = umma::effective_splits(Y, want);
     umma::EpiStore ep{part, (size_t)D, (size_t)B * D};
-    if (e->sg_live) {       // A = the logits slab, rewritten to dL/dlogits tile by tile in shared memory
-      umma::AXSoftmaxGradK<4> ax{e->sg};
-      C2V_LAUNCH(e, C2V_CUDA(e, (umma::launch_cfg<192, 4, false, true, umma::EpiStore, umma::AXSoftmaxGradK<4>>(st, B, D, Y, want, opA, opB, ep,
+    if (e->sg_live) {       // A = the logits slab, turned into dL/dlogits by the GEMM's loaders
+      umma::AXSoftmaxGrad<true> ax{e->sg};
+      C2V_LAUNCH(e, C2V_CUDA(e, (umma::launch_cfg<false, true, umma::EpiStore, umma::AXSoftmaxGrad<true>>(st, B, D, Y, want, opA, opB, ep,
                                                                                                             e->num_sms, ax))));
     } else {
-      C2V_LAUNCH(e, C2V_CUDA(e, (C2V_UMMA_192(st, B, D, Y, want, opA, opB, ep, e->num_sms))));
+      C2V_LAUNCH(e, C2V_CUDA(e, (C2V_UMMA(st, B, D, Y, want, opA, opB, ep, e->num_sms))));
     }
     return launch_colsum(e, st, part, (size_t)B * D, ks, B * D, dv, e->row_scale, D);
   }
@@ -939,11 +928,11 @@ int run_dy(c2v_engine* e, cudaStream_t st, const float* v, int B) {
         umma::EpiAdam ep{e->theta.tgt, e->am.tgt, e->av.tgt, (size_t)D, (float)lr_t, e->tgt_b1, e->tgt_b2, e->tgt_eps,
                          1.f - e->tgt_b1, 1.f - e->tgt_b2, e->adam_epi_prefetch};
         if (e->sg_live) {
-          umma::AXSoftmaxGradMN<2> ax{e->sg};
-          C2V_LAUNCH(e, C2V_CUDA(e, (umma::launch_cfg<192, 4, true, true, umma::EpiAdam, umma::AXSoftmaxGradMN<2>>(st, Y, D, B, 1, opA, opB, ep,
+          umma::AXSoftmaxGrad<false> ax{e->sg};
+          C2V_LAUNCH(e, C2V_CUDA(e, (umma::launch_cfg<true, true, umma::EpiAdam, umma::AXSoftmaxGrad<false>>(st, Y, D, B, 1, opA, opB, ep,
                                                                                                                e->num_sms, ax))));
         } else {
-          C2V_LAUNCH(e, C2V_CUDA(e, (C2V_UMMA_FIXED(192, true, true, false, umma::EpiAdam, st, Y, D, B, 1, opA, opB, ep, e->num_sms))));
+          C2V_LAUNCH(e, C2V_CUDA(e, (C2V_UMMA_FIXED(true, true, umma::EpiAdam, st, Y, D, B, 1, opA, opB, ep, e->num_sms))));
         }
         e->tgt_armed = false;
         e->tgt_fused_t = e->tgt_t;
@@ -951,11 +940,11 @@ int run_dy(c2v_engine* e, cudaStream_t st, const float* v, int B) {
       } else {
         umma::EpiStore ep{e->grad.tgt, (size_t)D, 0};
         if (e->sg_live) {
-          umma::AXSoftmaxGradMN<2> ax{e->sg};
-          C2V_LAUNCH(e, C2V_CUDA(e, (umma::launch_cfg<192, 4, true, true, umma::EpiStore, umma::AXSoftmaxGradMN<2>>(st, Y, D, B, 1, opA, opB, ep,
+          umma::AXSoftmaxGrad<false> ax{e->sg};
+          C2V_LAUNCH(e, C2V_CUDA(e, (umma::launch_cfg<true, true, umma::EpiStore, umma::AXSoftmaxGrad<false>>(st, Y, D, B, 1, opA, opB, ep,
                                                                                                                 e->num_sms, ax))));
         } else {
-          C2V_LAUNCH(e, C2V_CUDA(e, (C2V_UMMA_192_SINGLE(st, Y, D, B, 1, opA, opB, ep, e->num_sms))));
+          C2V_LAUNCH(e, C2V_CUDA(e, (C2V_UMMA(st, Y, D, B, 1, opA, opB, ep, e->num_sms))));
         }
       }
     } else {
@@ -1021,7 +1010,7 @@ int train_step_impl(c2v_engine* e, cudaStream_t st, const int32_t* src, const in
     {
       PhaseTimer pt(e, PH_XENT, st);
       C2V_LAUNCH(e, (true_logit_kernel<<<(B + 7) / 8, 256, 0, st>>>(v, e->theta.tgt, target, 0, Y, e->dims.code_dim, B, tl)));
-      C2V_LAUNCH(e, (xent_combine_kernel<<<B, 256, 0, st>>>(wsp<float2>(e, e->ws.lse_part), 2 * ((Y + 255) / 256), S, e->ws.ldS, target,
+      C2V_LAUNCH(e, (xent_combine_kernel<<<B, 256, 0, st>>>(wsp<float2>(e, e->ws.lse_part), umma::lse_slots(Y), S, e->ws.ldS, target,
                                                             loss_b, lse, tl)));
       C2V_LAUNCH(e, (loss_reduce_kernel<<<1, 256, 0, st>>>(loss_b, B, invB, loss_out)));
     }
@@ -1035,7 +1024,7 @@ int train_step_impl(c2v_engine* e, cudaStream_t st, const int32_t* src, const in
     // deferred normalisation: U = exp(s - true logit) from the logits epilogue, one patched element and one factor per row;
     // the gated kernels after the combine are the two-pass schedule, run by the device only when a row left the fp32 window
     const int D = e->dims.code_dim;
-    const int n_tiles = 2 * ((Y + 255) / 256);
+    const int n_tiles = umma::lse_slots(Y);
     float* tl = wsp<float>(e, e->ws.true_logit);
     float* rscale = wsp<float>(e, e->ws.rscale);
     float* vs = wsp<float>(e, e->ws.v_scaled);
@@ -1078,7 +1067,7 @@ int train_step_impl(c2v_engine* e, cudaStream_t st, const int32_t* src, const in
   {
     PhaseTimer pt(e, PH_XENT, st);
     if (fused_lse) {
-      const int n_tiles = 2 * ((Y + 255) / 256);       // partial slots per row
+      const int n_tiles = umma::lse_slots(Y);       // partial slots per row
       C2V_LAUNCH(e, (xent_combine_kernel<<<B, 256, 0, st>>>(wsp<float2>(e, e->ws.lse_part), n_tiles, S, e->ws.ldS, target,
                                                             loss_b, lse)));
       const int chunks = (int)((e->ws.ldS / 4 + 256 * 8 - 1) / (256 * 8));
@@ -1214,7 +1203,7 @@ int adam_impl(c2v_engine* e, cudaStream_t st, float lr, float b1, float b2, floa
     if (i == 2 && (skip_tgt || e->tgt_lazy)) continue;     // lazy target rows: deferred like the embedding rows
     const size_t n4 = n[i] / 4;
     size_t blocks = (n4 + 255) / 256;
-    if (blocks > 148 * 16) blocks = 148 * 16;
+    if (blocks > (size_t)e->num_sms * 16) blocks = (size_t)e->num_sms * 16;
     if (blocks < 1) blocks = 1;
     const int zero = (i < 2) ? 1 : 0;   // embedding gradient tables are cleared for the next scatter-add
     PhaseTimer pt(e, PH_ADAM, st);
@@ -1252,8 +1241,8 @@ int c2v_create(const c2v_dims* dims, int device, c2v_engine** out) {
   cudaDeviceProp prop;
   c = cudaGetDeviceProperties(&prop, device);
   if (c != cudaSuccess) return fail(nullptr, C2V_ERR_CUDA, cudaGetErrorString(c));
-  if (prop.major != 10)
-    return fail(nullptr, C2V_ERR_UNSUPPORTED, "this library is built for sm_100a (B200) only");
+  if (prop.major != 9 || prop.minor != 0)
+    return fail(nullptr, C2V_ERR_UNSUPPORTED, "this library is built for sm_90a (H100) only");
   c2v_engine* e = new c2v_engine();
   e->dims = *dims;
   e->device = device;
@@ -1520,7 +1509,7 @@ int c2v_loss(c2v_engine* e, const float* code_vec, const int32_t* target, int32_
   {
     PhaseTimer pt(e, PH_XENT, st);
     if (fused)      // the logits epilogue already folded each tile into (max, sum exp) partials
-      C2V_LAUNCH(e, (xent_combine_kernel<<<B, 256, 0, st>>>(wsp<float2>(e, e->ws.lse_part), 2 * ((Y + 255) / 256), S, e->ws.ldS, target,
+      C2V_LAUNCH(e, (xent_combine_kernel<<<B, 256, 0, st>>>(wsp<float2>(e, e->ws.lse_part), umma::lse_slots(Y), S, e->ws.ldS, target,
                                                             wsp<float>(e, e->ws.loss_b), wsp<float>(e, e->ws.lse))));
     else
       C2V_LAUNCH(e, (xent_kernel<<<B, kXentThreads, 0, st>>>(S, e->ws.ldS, target, Y, invB, wsp<float>(e, e->ws.loss_b),
@@ -1713,7 +1702,7 @@ int c2v_target_forward(c2v_engine* e, const float* code_all, int32_t Bt, const i
   float* S = wsp<float>(e, e->ws.S);
   const int Y = e->dims.target_vocab;
   const bool fused = (is_tc(e)) && (reinterpret_cast<uintptr_t>(code_all) % 16 == 0);
-  const int n_tiles = 2 * ((Y + 255) / 256);
+  const int n_tiles = umma::lse_slots(Y);
   e->slab_exp_live = false;
   if (fused && e->exp_slab && !e->fuse_sg && e->has_grad) {
     // deferred normalisation over a row-sharded table: (c_b, sum U) stand in for (row max, sum exp) in the cross-rank combine
@@ -1978,9 +1967,8 @@ int c2v_selftest_gemm3(c2v_engine* e, int32_t a_mn, int32_t b_mn, int32_t bn, in
   umma::Operand opB{Bm, ldb, b_mn != 0, B_lo};
   if (!umma::operand_ok(opA) || !umma::operand_ok(opB)) return fail(e, C2V_ERR_INVALID, "operand not TMA-compatible");
   umma::EpiStore ep{C, ldc, (size_t)M * ldc};
-  if (bn == 256) C2V_LAUNCH(e, C2V_CUDA(e, (C2V_UMMA_256(st, M, N, K, splits, opA, opB, ep, e->num_sms))));
-  else if (bn == 192) C2V_LAUNCH(e, C2V_CUDA(e, (C2V_UMMA_192(st, M, N, K, splits, opA, opB, ep, e->num_sms))));
-  else return fail(e, C2V_ERR_INVALID, "bn must be 192 or 256");
+  if (bn != 192 && bn != 256) return fail(e, C2V_ERR_INVALID, "bn must be 192 or 256");
+  C2V_LAUNCH(e, C2V_CUDA(e, (C2V_UMMA(st, M, N, K, splits, opA, opB, ep, e->num_sms))));
   return umma::effective_splits(K, splits);
 }
 

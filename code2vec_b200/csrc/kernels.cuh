@@ -8,7 +8,7 @@
 namespace c2v {
 
 // one CTA per example: 128 threads and <= 64 registers make 8 CTAs resident per SM, so a 1024-example batch is ONE wave on
-// 148 SMs (1184 slots) -- with 256 threads it was 1.7 waves, the second one 73 % full
+// the H100's 132 SMs (1056 slots)
 constexpr int kAttnThreads = 128;
 constexpr int kAttnWarps = kAttnThreads / 32;
 
@@ -134,8 +134,10 @@ attn_fwd_kernel(const float* __restrict__ H, const float* __restrict__ a, const 
 // forward pass already produced -- so H is read ONCE and overwritten in the same pass (a warp per context: the dot
 // product, dz and du all come from the row the warp holds in registers).
 // ---------------------------------------------------------------------------------------------
+// NV <= 3 (D <= 384): 8 resident CTAs per SM (64 registers) hold a 1024-example batch in one wave on 132 SMs; 7 would
+// leave a second wave, which costs more than the few spilled registers
 template <int NV, bool SPLIT>
-__global__ void __launch_bounds__(kAttnThreads, NV <= 3 ? 7 : 4)      // 7 x 148 SMs still holds a 1024-example batch in one wave
+__global__ void __launch_bounds__(kAttnThreads, NV <= 3 ? 8 : 4)
 attn_bwd_kernel(float* __restrict__ H, const float* __restrict__ alpha, const float* __restrict__ dv,
                 const float* __restrict__ v, const float* __restrict__ a, int C, int D, float* __restrict__ da_part,
                 float* __restrict__ H_lo) {
@@ -923,8 +925,8 @@ scatter_dx_kernel(const __grid_constant__ ContextSource cs, const __grid_constan
 // Row-sharded tables (peer memory over NVLink): locality-sorted gather / scatter-add.
 //
 // With the tables of BASELINE configs[4] (3M x 256 and 2M x 256 floats: 5 GB of parameters and 5 GB of gradient
-// shards mapped from the peers) random row accesses to peer memory ran at 70-90 GB/s against ~600 GB/s for the
-// java14m tables: every access touches a different 2 MB page of a mapping far larger than the GPU's TLB reach.
+// shards mapped from the peers) random row accesses to peer memory are TLB-bound: every access touches a different
+// 2 MB page of a mapping far larger than the GPU's TLB reach.
 // The context entries (n, segment) of a batch are therefore bucketed by (owner rank, 2 MB page of the owner's shard)
 // with a counting sort -- bucket_count / bucket_scan / bucket_fill -- and the gather and the scatter-add walk the
 // entries in bucket order: each remote page is visited once, by neighbouring warps, instead of once per access.

@@ -1,19 +1,19 @@
-// tcgen05 (5th-gen tensor core) GEMM for sm_100a:  C[M,N] = A[M,K] . B[K,N],  fp32 storage,
-// kind::tf32 operands (10-bit mantissa), fp32 accumulation in TMEM  (C2V_MATH_TF32).
+// Hopper (sm_90a) tensor-core GEMM:  C[M,N] = A[M,K] . B[K,N],  fp32 storage, tf32 operands (10-bit
+// mantissa), fp32 accumulation in registers  (C2V_MATH_TF32; C2V_MATH_3XTF32 issues three products).
 //
-// Persistent, warp-specialised, one CTA per SM:
-//   warp 0      : TMA producer   -- cp.async.bulk.tensor (128-byte swizzle) into a 4-stage smem ring
-//   warp 1      : MMA issuer     -- one elected lane issues tcgen05.mma.cta_group::1.kind::tf32
-//                                   (UMMA 128 x BN x 8), tcgen05.commit frees smem stages / publishes
-//                                   the accumulator; also owns the TMEM allocation
-//   warps 2..9  : epilogue       -- tcgen05.ld (32x32b) of their TMEM lane quadrant (two warps per
-//                                   quadrant, half of the columns each), fused epilogue functor
-//                                   (store / tanh / log-sum-exp partials / split-K slice)
-// The accumulator is double-buffered in TMEM (2 x BN columns) so the epilogue of tile i overlaps
-// the MMAs of tile i+1.  Operands may be K-major (K contiguous) or MN-major (M resp. N
-// contiguous) in global memory; both are staged as 128-byte swizzled rows and described to the
-// tensor core through shared-memory matrix descriptors.  Out-of-range rows / K-tail are
-// zero-filled by TMA, so any M, N, K work; split-K over blockIdx-independent work items.
+// Persistent, warp-specialised, one CTA of three warpgroups per SM:
+//   warpgroup 0     : producer -- fills a 4-stage shared-memory ring.  K-major operands arrive by TMA
+//                     (cp.async.bulk.tensor, 128-byte swizzle, issued by one thread); MN-major operands are
+//                     loaded by all 128 threads and transposed on the way into shared memory, because
+//                     wgmma takes 32-bit (tf32) operands K-major only.  An A-operand policy (AX*) may
+//                     instead compute the A tile (softmax gradient of a logits tile, embedding gather).
+//   warpgroups 1, 2 : consumers -- each owns 64 rows of the 128-row tile and issues
+//                     wgmma.mma_async m64n128k8 (tf32) into a 64-register accumulator per thread;
+//                     then the fused epilogue (store / tanh / log-sum-exp partials / split-K slice / Adam).
+// Every stage is published by an mbarrier (TMA transaction bytes + one arrival per producer thread) and
+// released by one arrival per consumer warp once the wgmma group that read it has retired.
+// Out-of-range rows / K-tail are zero-filled (by TMA or by the loaders), so any M, N, K work; split-K
+// over blockIdx-independent work items.
 #pragma once
 #include <cuda.h>
 #include <cuda_runtime.h>
@@ -24,12 +24,12 @@
 namespace c2v {
 namespace umma {
 
-constexpr int BM = 128;          // UMMA_M (cta_group::1)
+constexpr int BM = 128;          // rows of a tile: two consumer warpgroups x wgmma M = 64
+constexpr int BN = 128;          // columns of a tile: wgmma N
 constexpr int BK = 32;           // fp32 elements per stage along K = one 128-byte swizzle row
-constexpr int UMMA_K = 8;        // K per tcgen05.mma for 32-bit operands (32 bytes)
-constexpr int kEpiWarps = 8;     // two warps per TMEM lane quadrant, each draining half of the tile's columns
-constexpr int kThreads = 32 * (2 + kEpiWarps);
-constexpr int kEpiWarp0 = 2;
+constexpr int WG_K = 8;          // K per wgmma for 32-bit operands (32 bytes)
+constexpr int STAGES = 4;
+constexpr int kThreads = 3 * 128;
 
 // fast transcendental forms for the tensor-core path (operands are already tf32-rounded):
 // exp via ex2.approx (rel. error 2^-22), tanh(x) = 1 - 2 / (exp(2x) + 1) (abs. error ~1e-7).
@@ -46,8 +46,8 @@ __device__ __forceinline__ uint32_t smem_u32(const void* p) { return (uint32_t)_
 __device__ __forceinline__ void mbar_init(uint64_t* bar, uint32_t count) {
   asm volatile("mbarrier.init.shared::cta.b64 [%0], %1;" ::"r"(smem_u32(bar)), "r"(count));
 }
-__device__ __forceinline__ void mbar_expect_tx(uint64_t* bar, uint32_t bytes) {
-  asm volatile("mbarrier.arrive.expect_tx.shared::cta.b64 _, [%0], %1;" ::"r"(smem_u32(bar)), "r"(bytes) : "memory");
+__device__ __forceinline__ void mbar_expect_tx(uint64_t* bar, uint32_t bytes) {      // no arrival
+  asm volatile("mbarrier.expect_tx.relaxed.cta.shared::cta.b64 [%0], %1;" ::"r"(smem_u32(bar)), "r"(bytes) : "memory");
 }
 __device__ __forceinline__ void mbar_arrive(uint64_t* bar) {
   asm volatile("mbarrier.arrive.shared::cta.b64 _, [%0];" ::"r"(smem_u32(bar)) : "memory");
@@ -69,6 +69,8 @@ __device__ __forceinline__ void mbar_wait(uint64_t* bar, uint32_t parity) {
     if (clock64() - t0 > 20000000000LL) __trap();     // ~10 s at 2 GHz
   }
 }
+__device__ __forceinline__ void fence_proxy_async_smem() { asm volatile("fence.proxy.async.shared::cta;" ::: "memory"); }
+__device__ __forceinline__ void wg_bar_sync(int id) { asm volatile("bar.sync %0, 128;" ::"r"(id) : "memory"); }
 
 // ---- TMA ----------------------------------------------------------------------------------------
 __device__ __forceinline__ void tma_load_2d(void* smem_dst, const CUtensorMap* map, uint64_t* bar, int c0, int c1) {
@@ -77,82 +79,42 @@ __device__ __forceinline__ void tma_load_2d(void* smem_dst, const CUtensorMap* m
       ::"r"(smem_u32(smem_dst)), "l"(map), "r"(smem_u32(bar)), "r"(c0), "r"(c1) : "memory");
 }
 
-// ---- tcgen05 ------------------------------------------------------------------------------------
-__device__ __forceinline__ void tmem_alloc(uint32_t* smem_result, uint32_t ncols) {
-  asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(smem_result)), "r"(ncols) : "memory");
-  asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
+// ---- wgmma --------------------------------------------------------------------------------------
+// Shared-memory matrix descriptor of a K-major SWIZZLE_128B tile (rows of 128 B, 16-byte chunk c of row r at
+// (c ^ (r & 7)) * 16, 8-row groups 1024 B apart): start address >> 4 in [0,14), leading byte offset (unused
+// for swizzled K-major layouts, 1) in [16,30), stride byte offset 1024 >> 4 in [32,46), swizzle mode 1 =
+// 128B in [62,64).  The tile base is 1024-byte aligned; one wgmma consumes 32 B of each row, so the K step
+// is +32 B on the start address.
+__device__ __forceinline__ uint64_t gmma_desc(uint32_t saddr) {
+  return (uint64_t)((saddr >> 4) & 0x3FFF) | (1ull << 16) | ((uint64_t)(1024 >> 4) << 32) | (1ull << 62);
 }
-__device__ __forceinline__ void tmem_dealloc(uint32_t taddr, uint32_t ncols) {
-  asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(taddr), "r"(ncols) : "memory");
-}
-__device__ __forceinline__ void tc_fence_before() { asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory"); }
-__device__ __forceinline__ void tc_fence_after() { asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory"); }
-__device__ __forceinline__ void tc_commit(uint64_t* bar) {
-  asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];" ::"r"(smem_u32(bar)) : "memory");
-}
-__device__ __forceinline__ void mma_tf32(uint32_t tmem_d, uint64_t adesc, uint64_t bdesc, uint32_t idesc, uint32_t accumulate) {
+__device__ __forceinline__ void wg_fence() { asm volatile("wgmma.fence.sync.aligned;" ::: "memory"); }
+__device__ __forceinline__ void wg_commit() { asm volatile("wgmma.commit_group.sync.aligned;" ::: "memory"); }
+template <int N>
+__device__ __forceinline__ void wg_wait() { asm volatile("wgmma.wait_group.sync.aligned %0;" ::"n"(N) : "memory"); }
+// D[64 x 128] (+)= A[64 x 8] . B[8 x 128]; thread (warp w, lane l) holds rows 16w + l/4 (+8), columns 8j + 2(l%4) (+1)
+// in d[4j + 2i + c] (row + 8i, column + c)
+__device__ __forceinline__ void wgmma_tf32(float (&d)[64], uint64_t da, uint64_t db, uint32_t accumulate) {
   asm volatile(
       "{\n\t.reg .pred p;\n\t"
-      "setp.ne.b32 p, %4, 0;\n\t"
-      "tcgen05.mma.cta_group::1.kind::tf32 [%0], %1, %2, %3, p;\n\t}"
-      ::"r"(tmem_d), "l"(adesc), "l"(bdesc), "r"(idesc), "r"(accumulate) : "memory");
-}
-// 32 lanes x 32 consecutive 32-bit columns: thread i gets row (lane_base + i), columns [c, c+32)
-__device__ __forceinline__ void tmem_ld32(uint32_t taddr, uint32_t (&r)[32]) {
-  asm volatile(
-      "tcgen05.ld.sync.aligned.32x32b.x32.b32 "
-      "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, "
-      "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, [%32];"
-      : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7]), "=r"(r[8]),
-        "=r"(r[9]), "=r"(r[10]), "=r"(r[11]), "=r"(r[12]), "=r"(r[13]), "=r"(r[14]), "=r"(r[15]), "=r"(r[16]),
-        "=r"(r[17]), "=r"(r[18]), "=r"(r[19]), "=r"(r[20]), "=r"(r[21]), "=r"(r[22]), "=r"(r[23]), "=r"(r[24]),
-        "=r"(r[25]), "=r"(r[26]), "=r"(r[27]), "=r"(r[28]), "=r"(r[29]), "=r"(r[30]), "=r"(r[31])
-      : "r"(taddr));
-}
-// 64 consecutive columns in one round trip: r0 = columns [c, c+32), r1 = [c+32, c+64)
-__device__ __forceinline__ void tmem_ld64(uint32_t taddr, uint32_t (&a)[32], uint32_t (&b)[32]) {
-  asm volatile(
-      "tcgen05.ld.sync.aligned.32x32b.x64.b32 "
-      "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, "
-      "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, "
-      "%32, %33, %34, %35, %36, %37, %38, %39, %40, %41, %42, %43, %44, %45, %46, %47, "
-      "%48, %49, %50, %51, %52, %53, %54, %55, %56, %57, %58, %59, %60, %61, %62, %63}, [%64];"
-      : "=r"(a[0]), "=r"(a[1]), "=r"(a[2]), "=r"(a[3]), "=r"(a[4]), "=r"(a[5]), "=r"(a[6]), "=r"(a[7]), "=r"(a[8]),
-        "=r"(a[9]), "=r"(a[10]), "=r"(a[11]), "=r"(a[12]), "=r"(a[13]), "=r"(a[14]), "=r"(a[15]), "=r"(a[16]),
-        "=r"(a[17]), "=r"(a[18]), "=r"(a[19]), "=r"(a[20]), "=r"(a[21]), "=r"(a[22]), "=r"(a[23]), "=r"(a[24]),
-        "=r"(a[25]), "=r"(a[26]), "=r"(a[27]), "=r"(a[28]), "=r"(a[29]), "=r"(a[30]), "=r"(a[31]),
-        "=r"(b[0]), "=r"(b[1]), "=r"(b[2]), "=r"(b[3]), "=r"(b[4]), "=r"(b[5]), "=r"(b[6]), "=r"(b[7]), "=r"(b[8]),
-        "=r"(b[9]), "=r"(b[10]), "=r"(b[11]), "=r"(b[12]), "=r"(b[13]), "=r"(b[14]), "=r"(b[15]), "=r"(b[16]),
-        "=r"(b[17]), "=r"(b[18]), "=r"(b[19]), "=r"(b[20]), "=r"(b[21]), "=r"(b[22]), "=r"(b[23]), "=r"(b[24]),
-        "=r"(b[25]), "=r"(b[26]), "=r"(b[27]), "=r"(b[28]), "=r"(b[29]), "=r"(b[30]), "=r"(b[31])
-      : "r"(taddr));
-}
-__device__ __forceinline__ void tmem_ld_wait() { asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory"); }
-
-// ---- descriptors ----------------------------------------------------------------------------------
-// Shared-memory matrix descriptor (cute::UMMA::SmemDescriptor bit layout): start address >> 4 in
-// [0,14), leading byte offset >> 4 in [16,30), stride byte offset >> 4 in [32,46), version = 1 in
-// [46,48), layout type in [61,64): SWIZZLE_128B = 2 (16-byte chunks swizzled over 8 rows; K-major
-// operands) or SWIZZLE_128B_BASE32B = 1 (32-byte chunks swizzled over 4 rows) -- the only layout the
-// tensor core accepts for MN-major 32-bit (tf32) operands; TMA writes it with
-// CU_TENSOR_MAP_SWIZZLE_128B_ATOM_32B.
-constexpr uint32_t kLayoutSw128 = 2, kLayoutSw128Base32 = 1;
-__host__ __device__ constexpr uint64_t make_smem_desc_hi(uint32_t sbo_bytes, uint32_t layout_type) {
-  return (uint64_t)((sbo_bytes >> 4) & 0x3FFF) | (1ull << 14) | ((uint64_t)layout_type << 29);     // upper 32 bits
-}
-__device__ __forceinline__ uint64_t make_smem_desc(uint32_t smem_addr, uint32_t lbo_bytes, uint32_t sbo_bytes,
-                                                   uint32_t layout_type) {
-  const uint32_t lo = ((smem_addr >> 4) & 0x3FFF) | (((lbo_bytes >> 4) & 0x3FFF) << 16);
-  return ((uint64_t)make_smem_desc_hi(sbo_bytes, layout_type) << 32) | lo;
-}
-// Instruction descriptor (cute::UMMA::InstrDescriptor): D = F32, A = B = TF32, majors, N >> 3, M >> 4.
-__host__ __device__ constexpr uint32_t make_idesc_tf32(int M, int N, bool a_mn, bool b_mn) {
-  return (1u << 4) | (2u << 7) | (2u << 10) | ((a_mn ? 1u : 0u) << 15) | ((b_mn ? 1u : 0u) << 16) |
-         ((uint32_t)(N >> 3) << 17) | ((uint32_t)(M >> 4) << 24);
+      "setp.ne.b32 p, %66, 0;\n\t"
+      "wgmma.mma_async.sync.aligned.m64n128k8.f32.tf32.tf32 "
+      "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, "
+      "%24, %25, %26, %27, %28, %29, %30, %31, %32, %33, %34, %35, %36, %37, %38, %39, %40, %41, %42, %43, %44, %45, "
+      "%46, %47, %48, %49, %50, %51, %52, %53, %54, %55, %56, %57, %58, %59, %60, %61, %62, %63}, %64, %65, p, 1, 1;\n\t}"
+      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]),
+        "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]),
+        "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]),
+        "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31]), "+f"(d[32]),
+        "+f"(d[33]), "+f"(d[34]), "+f"(d[35]), "+f"(d[36]), "+f"(d[37]), "+f"(d[38]), "+f"(d[39]), "+f"(d[40]),
+        "+f"(d[41]), "+f"(d[42]), "+f"(d[43]), "+f"(d[44]), "+f"(d[45]), "+f"(d[46]), "+f"(d[47]), "+f"(d[48]),
+        "+f"(d[49]), "+f"(d[50]), "+f"(d[51]), "+f"(d[52]), "+f"(d[53]), "+f"(d[54]), "+f"(d[55]), "+f"(d[56]),
+        "+f"(d[57]), "+f"(d[58]), "+f"(d[59]), "+f"(d[60]), "+f"(d[61]), "+f"(d[62]), "+f"(d[63])
+      : "l"(da), "l"(db), "r"(accumulate));
 }
 
 // ---- epilogues ---------------------------------------------------------------------------------------
-// Each epilogue warp owns 32 accumulator rows (its TMEM lane quadrant) and a range of columns.  A
+// In the epilogue each thread holds one accumulator row's 32 consecutive columns at a time.  A
 // functor supplies:  State / begin / end  -- per-(row, tile) state and its publication;
 //                    observe(m, n0, 32 raw accumulators, nvalid, state) -- row-wise math (log-sum-exp);
 //                    map(x)    -- the element-wise transform applied on the way out (identity, tanh);
@@ -160,11 +122,10 @@ __host__ __device__ constexpr uint32_t make_idesc_tf32(int M, int N, bool a_mn, 
 //                    Pre / prefetch / store4 / store1(base, offset, value) -- what "storing" an element
 //                    means (a plain write, or the optimizer update of the parameter the element is
 //                    the gradient of; prefetch issues that update's loads ahead of the arithmetic).
-// The store itself is done by drain_accumulator: TMEM -> registers (thread = row) -> a 4 KB
-// XOR-swizzled shared-memory transpose per warp -> global stores in which every instruction writes
-// four complete 128-byte row segments.  (Storing straight from the TMEM register layout makes each
-// store instruction touch 32 different lines: 8x the LSU wavefronts, and that -- not the tensor
-// pipe -- was what bounded the short-K GEMMs.)
+// The store itself is done by store_chunk: registers (thread = row) -> a 4 KB XOR-swizzled
+// shared-memory transpose per warp -> global stores in which every instruction writes four complete
+// 128-byte row segments (storing straight from the row-per-thread layout would make each store
+// instruction touch 32 different lines).
 struct EpiNoState {};
 
 struct EpiStore {
@@ -179,7 +140,6 @@ struct EpiStore {
   __device__ __forceinline__ float* out(int split) const { return C + (size_t)split * split_stride; }
   using Pre = EpiNoState;
   static constexpr int kRowBatch = 8;
-  static constexpr bool kWideDrain = true;
   __device__ __forceinline__ void prefetch(const float*, size_t, Pre&) const {}
   __device__ __forceinline__ void store4(float* c, size_t off, float4 v, const Pre&) const { *reinterpret_cast<float4*>(c + off) = v; }
   __device__ __forceinline__ void store1(float* c, size_t off, float x) const { c[off] = x; }
@@ -196,21 +156,20 @@ struct EpiTanhStoreT {
   __device__ __forceinline__ float* out(int) const { return C; }
   using Pre = EpiNoState;
   static constexpr int kRowBatch = 8;
-  static constexpr bool kWideDrain = true;
   __device__ __forceinline__ void prefetch(const float*, size_t, Pre&) const {}
   __device__ __forceinline__ void store4(float* c, size_t off, float4 v, const Pre&) const { *reinterpret_cast<float4*>(c + off) = v; }
   __device__ __forceinline__ void store1(float* c, size_t off, float x) const { c[off] = x; }
 };
 
 // Logits epilogue: stores the tile of S and folds the row-wise (max, sum exp) of this warp's columns
-// into a per-(row, half tile) partial, so the cross entropy needs no extra pass over S for its
+// into a per-(row, partial slot) partial, so the cross entropy needs no extra pass over S for its
 // log-sum-exp (tensorflow_model.py:227-230).
 template <bool PRECISE>      // PRECISE: expf (3xTF32 mode); else ex2.approx
 struct EpiStoreLseT {
   struct State { float mx, sum; };
   float* C;
   size_t ldc;
-  float2* partial;       // [M, slots]; slot = 2 * n_tile + column half
+  float2* partial;       // [M, slots]; slot = 2 * n_tile + p, p = 0 for column quarters 0 and 2 of the tile, 1 for 1 and 3
   int slots;
   __device__ __forceinline__ float ex(float x) const { return PRECISE ? expf(x) : __expf(x); }
   __device__ __forceinline__ void begin(State& st) const { st.mx = -INFINITY; st.sum = 0.f; }
@@ -221,7 +180,6 @@ struct EpiStoreLseT {
   __device__ __forceinline__ float* out(int) const { return C; }
   using Pre = EpiNoState;
   static constexpr int kRowBatch = 8;
-  static constexpr bool kWideDrain = true;
   __device__ __forceinline__ void prefetch(const float*, size_t, Pre&) const {}
   __device__ __forceinline__ void store4(float* c, size_t off, float4 v, const Pre&) const { *reinterpret_cast<float4*>(c + off) = v; }
   __device__ __forceinline__ void store1(float* c, size_t off, float x) const { c[off] = x; }
@@ -262,7 +220,7 @@ struct EpiStoreLseT {
   }
 };
 
-// Logits pass 1 of the recomputing schedule: ONLY the per-(row, half tile) (max, sum exp) partials -- nothing is stored, so the
+// Logits pass 1 of the recomputing schedule: ONLY the per-(row, partial slot) (max, sum exp) partials -- nothing is stored, so the
 // epilogue neither transposes through shared memory nor writes the 1.07 GB slab (tensorflow_model.py:227-230).
 template <bool PRECISE>
 struct EpiLseOnlyT : EpiStoreLseT<PRECISE> {
@@ -302,7 +260,6 @@ struct EpiSoftmaxGradT {
   __device__ __forceinline__ float* out(int) const { return C; }
   using Pre = EpiNoState;
   static constexpr int kRowBatch = 8;
-  static constexpr bool kWideDrain = true;
   __device__ __forceinline__ void prefetch(const float*, size_t, Pre&) const {}
   __device__ __forceinline__ void store4(float* c, size_t off, float4 v, const Pre&) const {
     if (SPLIT) {
@@ -326,8 +283,8 @@ struct EpiSoftmaxGradT {
 };
 
 // Logits epilogue of the deferred-normalisation schedule (option "exp_slab"): the slab receives U = exp(s - c_row) instead
-// of the logits, c_row a per-example constant known before the product (the example's true-class logit), and the per-(row,
-// half tile) partial holds (max U, sum U).  softmax - onehot is then U with one patched element per row times a per-row
+// of the logits, c_row a per-example constant known before the product (the example's true-class logit), and the partial of
+// each (row, slot) holds (max U, sum U).  softmax - onehot is then U with one patched element per row times a per-row
 // factor 1 / sum U, which the two gradient GEMMs apply to their small operand / result: no pass ever reads the slab back
 // to normalise it (tensorflow_model.py:227-230).  max U is the range guard: the caller falls back to the two-pass
 // schedule when some row's largest U leaves [kExpSlabMin, kExpSlabMax] (common.cuh).  SPLIT (3xTF32): U is written as its tf32 split.
@@ -338,7 +295,7 @@ struct EpiExpSumT {
   float* C_lo;
   size_t ldc;
   const float* offset;   // [M] c_row
-  float2* partial;       // [M, slots]; slot = 2 * n_tile + column half
+  float2* partial;       // [M, slots]; slot = 2 * n_tile + p, p = 0 for column quarters 0 and 2 of the tile, 1 for 1 and 3
   int slots;
   __device__ __forceinline__ void begin(State& st) const { st.mx = 0.f; st.sum = 0.f; }
   __device__ __forceinline__ void end(int m, int slot, int, bool row_ok, State& st) const {
@@ -348,7 +305,6 @@ struct EpiExpSumT {
   __device__ __forceinline__ float* out(int) const { return C; }
   using Pre = EpiNoState;
   static constexpr int kRowBatch = 8;
-  static constexpr bool kWideDrain = true;
   __device__ __forceinline__ void prefetch(const float*, size_t, Pre&) const {}
   __device__ __forceinline__ void store4(float* c, size_t off, float4 v, const Pre&) const {
     if (SPLIT) {
@@ -436,7 +392,7 @@ struct EpiAdam {
     vv = __fadd_rn(__fmul_rn(vv, b2), __fmul_rn(omb2, __fmul_rn(gg, gg)));
     pp = adam_move_dense(pp, lr_t, mm, vv, eps);
   }
-  // Called by an epilogue warp one tile AHEAD of the tile it is about to drain (row m, columns [n0, n0 + ncols)): pulls the
+  // Called by an epilogue thread one tile AHEAD of the tile it is about to drain (row m, columns [n0, n0 + ncols)): pulls the
   // (theta, m, v) lines of that region into L2, so that the update's loads -- only kRowBatch rows of them in flight per
   // thread -- see L2 latency rather than DRAM latency.
   __device__ __forceinline__ void prefetch_tile(int m, int n0, int ncols, int M, int N) const {
@@ -449,8 +405,7 @@ struct EpiAdam {
     }
   }
   struct Pre { float4 p, m, v; };
-  static constexpr int kRowBatch = 4;            // 8 rows in flight spill and measured slower (dY 0.77 vs 0.68 ms)
-  static constexpr bool kWideDrain = false;      // 32 columns per tcgen05.ld: the update needs the registers
+  static constexpr int kRowBatch = 2;            // more rows in flight spill registers at the 168-register cap of the GEMM
   __device__ __forceinline__ void prefetch(const float* c, size_t off, Pre& q) const {
     q.p = *reinterpret_cast<const float4*>(c + off);
     q.m = *reinterpret_cast<const float4*>(Mo + off);
@@ -469,8 +424,6 @@ struct EpiAdam {
     c[off] = p; Mo[off] = m; Vo[off] = v;
   }
 };
-
-constexpr int kEpiStageBytes = 32 * 32 * 4;      // one 32 x 32 fp32 block per epilogue warp
 
 // One 32-column chunk: registers (thread = row) -> swizzled smem -> coalesced global stores.
 // element-wise transform on the way out: functors with a (row, column)-dependent transform define map_at(x, column, state)
@@ -543,55 +496,18 @@ __device__ __forceinline__ void store_chunk(const Epi& epi, const typename Epi::
   __syncwarp();
 }
 
-// Drains this warp's share of one accumulator: columns [col0, col0 + ncols) of the tile, rows
-// m_base .. m_base + 31 (this thread's row is m_base + lane); 64 columns per tcgen05.ld round trip.
-template <class Epi>
-__device__ __forceinline__ void drain_accumulator(const Epi& epi, typename Epi::State& est, uint32_t taddr, int col0, int ncols,
-                                                  int m_base, int lane, int n_tile0, int M, int N, int sp, float* stage) {
-  const int m = m_base + lane;
-  float* cbase = epi.out(sp);
-  int c = col0;
-#pragma unroll 1
-  for (; Epi::kWideDrain && c + 64 <= col0 + ncols; c += 64) {
-    uint32_t r0[32], r1[32];
-    tmem_ld64(taddr + c, r0, r1);
-    tmem_ld_wait();
-    const int n = n_tile0 + c;
-    if (n < N) {
-      if (m < M) epi.observe(m, n, r0, N - n, est);
-      if (epi_stores<Epi>(0)) store_chunk(epi, est, r0, stage, lane, m_base, n, M, N, cbase, epi.ldc);
-    }
-    if (n + 32 < N) {
-      if (m < M) epi.observe(m, n + 32, r1, N - n - 32, est);
-      if (epi_stores<Epi>(0)) store_chunk(epi, est, r1, stage, lane, m_base, n + 32, M, N, cbase, epi.ldc);
-    }
-  }
-#pragma unroll 1
-  for (; c < col0 + ncols; c += 32) {
-    uint32_t r[32];
-    tmem_ld32(taddr + c, r);
-    tmem_ld_wait();
-    const int n = n_tile0 + c;
-    if (n < N) {
-      if (m < M) epi.observe(m, n, r, N - n, est);
-      if (epi_stores<Epi>(0)) store_chunk(epi, est, r, stage, lane, m_base, n, M, N, cbase, epi.ldc);
-    }
-  }
-}
-
-// ---- A-operand transforms ---------------------------------------------------------------------------------
-// Optional warps between TMA and the tensor core: they wait for a stage to land, rewrite the A tile IN PLACE in
-// shared memory (element-wise, so the swizzled layout is untouched), fence the generic-proxy writes for the async
-// proxy and only then release the stage to the MMA issuer.  Used to feed the two target-side gradient GEMMs with
-// dL/dlogits = (softmax(S) - onehot) / B computed on the fly from the LOGITS slab S and the per-row log-sum-exp, so
-// that the separate pass that rewrote the 1.07 GB slab (read + write) disappears:
-//   dv = P . Ytab     A = S, K-major   (rows = examples, K = classes)      -> AXSoftmaxGradK
-//   dY = P^T . v      A = S^T, MN-major (rows = classes, K = examples)     -> AXSoftmaxGradMN
+// ---- A-operand policies -------------------------------------------------------------------------------------
+// Where the producer warpgroup gets the A tile from:
+//   AXNone        : the A operand (TMA when K-major, transposing loads when MN-major)
+//   AXSoftmaxGrad : the A operand is a LOGITS slab S; the loaders turn each element into dL/dlogits =
+//                   (softmax(S) - onehot) / B on its way into shared memory, given the per-row log-sum-exp,
+//                   so that the separate pass that rewrote the slab (read + write) disappears (option
+//                   fuse_softmax_grad):
+//                     dv = P . Ytab     A = S, K-major   (rows = examples, K = classes)  -> AXSoftmaxGrad<true>
+//                     dY = P^T . v      A = S^T, MN-major (rows = classes, K = examples) -> AXSoftmaxGrad<false>
+//   AXGather      : the A tile is gathered from the embedding tables (fused context forward, see launch_ctx_fused)
 struct AXNone {
-  static constexpr int kWarps = 0;
-  struct Pre {};
-  __device__ __forceinline__ void load(int, int, int, int, int, Pre&) const {}
-  __device__ __forceinline__ void apply(uint8_t*, int, int, int, int, int, const Pre&) const {}
+  static constexpr int kKind = 0;
 };
 
 struct SoftmaxGradArgs {
@@ -600,106 +516,138 @@ struct SoftmaxGradArgs {
   int row0;                  // first class held in S (row-sharded target table), 0 otherwise
   float inv_batch;
 };
-// p = exp(x - lse) / B as ONE fused multiply-add and one ex2: 2^(x log2(e) + c), c = -lse log2(e) + log2(1/B).  No branches, so
-// the 32 values of a row are independent instruction streams (a single warp transforms a whole stage: it needs the ILP).
 __device__ __forceinline__ float ex2_approx(float x) {
   float y;
   asm("ex2.approx.ftz.f32 %0, %1;" : "=f"(y) : "f"(x));
   return y;
 }
 constexpr float kLog2e = 1.4426950408889634f;
-__device__ __forceinline__ float4 softmax_grad4(float4 x, float c) {
-  return make_float4(ex2_approx(fmaf(x.x, kLog2e, c)), ex2_approx(fmaf(x.y, kLog2e, c)), ex2_approx(fmaf(x.z, kLog2e, c)),
-                     ex2_approx(fmaf(x.w, kLog2e, c)));
-}
-__device__ __forceinline__ float4 softmax_grad4_tail(float4 x, float c, int y0, int ymax) {     // classes >= ymax are zero fill: keep 0
-  float4 p = softmax_grad4(x, c);
-  p.x = (y0 + 0 < ymax) ? p.x : 0.f; p.y = (y0 + 1 < ymax) ? p.y : 0.f;
-  p.z = (y0 + 2 < ymax) ? p.z : 0.f; p.w = (y0 + 3 < ymax) ? p.w : 0.f;
-  return p;
-}
-// ONE warp rewrites a whole stage (warp w owns every kWarps-th step of the CTA's k-block stream), so kWarps stages are
-// being transformed at any time.  load() runs BEFORE the wait for the stage: the per-example exponent offset and target are in
-// registers by the time the tile has landed.  The "- onehot / B" term touches at most one element per example row and is
-// applied to that element after the row has been rewritten.
-//
-// A tile = BM example rows x BK classes, K-major SWIZZLE_128B: row r at r*128, 16-byte chunk c at (c ^ (r & 7)) * 16.
-// Lane l rewrites rows l, l + 32, l + 64, l + 96.
-template <int NW>
-struct AXSoftmaxGradK {
-  static constexpr int kWarps = NW;
+
+template <bool EX_IS_M>      // true: tile rows are examples (A = S); false: tile K is examples (A = S^T)
+struct AXSoftmaxGrad {
+  static constexpr int kKind = 1;
   SoftmaxGradArgs a;
-  struct Pre { float c[BM / 32]; int tgt[BM / 32]; };
-  __device__ __forceinline__ void load(int lane, int m0, int, int M, int, Pre& p) const {
-    const float lb = log2f(a.inv_batch);
+  // v = A(x, k .. k+3) (rows of S: EX_IS_M) or A(x .. x+3, k) (S^T): the four elements share one example.
+  // p = exp(s - lse) / B as one fused multiply-add and one ex2: 2^(s log2(e) + c), c = -lse log2(e) + log2(1/B).
+  // Elements outside [X, K) are zero fill and stay zero.
+  __device__ __forceinline__ float4 xform(float4 v, int x, int k, int X, int K) const {
+    const int ex = EX_IS_M ? x : k;
+    if (ex >= (EX_IS_M ? X : K)) return v;
+    const float c = fmaf(-a.lse[ex], kLog2e, log2f(a.inv_batch));
+    const int tgt = a.target[ex] - a.row0;
+    const int y0 = EX_IS_M ? k : x, ny = EX_IS_M ? K : X;
+    float e[4] = {v.x, v.y, v.z, v.w};
 #pragma unroll
-    for (int j = 0; j < BM / 32; ++j) {
-      const int b = m0 + lane + 32 * j;
-      p.c[j] = (b < M) ? fmaf(-a.lse[b], kLog2e, lb) : 0.f;
-      p.tgt[j] = (b < M) ? a.target[b] - a.row0 : -1;
-    }
-  }
-  __device__ __forceinline__ void apply(uint8_t* sa, int lane, int m0, int k0, int M, int K, const Pre& p) const {
-    const bool full = k0 + BK <= K;
-#pragma unroll
-    for (int j = 0; j < BM / 32; ++j) {
-      const int r = lane + 32 * j;
-      if (m0 + r >= M) continue;                             // rows past the batch: TMA zero fill, results are discarded
-      uint8_t* row = sa + r * 128;
-      float4 v[8];
-#pragma unroll
-      for (int c = 0; c < 8; ++c) v[c] = *reinterpret_cast<const float4*>(row + ((c ^ (r & 7)) << 4));
-      if (full) {
-#pragma unroll
-        for (int c = 0; c < 8; ++c) v[c] = softmax_grad4(v[c], p.c[j]);
-      } else {
-#pragma unroll
-        for (int c = 0; c < 8; ++c) v[c] = softmax_grad4_tail(v[c], p.c[j], k0 + c * 4, K);
-      }
-#pragma unroll
-      for (int c = 0; c < 8; ++c) *reinterpret_cast<float4*>(row + ((c ^ (r & 7)) << 4)) = v[c];
-      const int e = p.tgt[j] - k0;                           // the example's own class, if it is in this tile: - 1/B
-      if (e >= 0 && e < BK) *(reinterpret_cast<float*>(row + (((e >> 2) ^ (r & 7)) << 4)) + (e & 3)) -= a.inv_batch;
-    }
+    for (int j = 0; j < 4; ++j)
+      e[j] = (y0 + j < ny) ? ex2_approx(fmaf(e[j], kLog2e, c)) - ((y0 + j == tgt) ? a.inv_batch : 0.f) : 0.f;
+    return make_float4(e[0], e[1], e[2], e[3]);
   }
 };
-// A tile = BM classes x BK examples, MN-major SWIZZLE_128B_BASE32B: BM/32 blocks of [BK example rows x 128 B]; in a row the
-// 32-byte unit u (8 classes) sits at (u ^ (row & 3)) * 32.  Lane l rewrites example row l of every block.
-template <int NW>
-struct AXSoftmaxGradMN {
-  static constexpr int kWarps = NW;
-  SoftmaxGradArgs a;
-  struct Pre { float c; int tgt; };
-  __device__ __forceinline__ void load(int lane, int, int k0, int, int K, Pre& p) const {
-    const int b = k0 + lane;
-    p.c = (b < K) ? fmaf(-a.lse[b], kLog2e, log2f(a.inv_batch)) : 0.f;
-    p.tgt = (b < K) ? a.target[b] - a.row0 : -1;
-  }
-  __device__ __forceinline__ void apply(uint8_t* sa, int lane, int m0, int k0, int M, int K, const Pre& p) const {
-    static_assert(BK == 32, "one example row per lane");
-    if (k0 + lane >= K) return;                              // examples past the batch: zero fill stays zero
-    const bool full = m0 + BM <= M;
+
+struct AXGather {
+  static constexpr int kKind = 2;
+  ContextSource cs;
+  Dropout dp;
+  float* Xout;               // nullptr, or [M, 3d]: the dropped-out rows are written once (for dW = X'^T . dU)
+};
+
+// ---- tile loaders (producer warpgroup, thread t in [0, 128)) -----------------------------------------------------
+__device__ __forceinline__ float4 ld4(const float* p) { return __ldg(reinterpret_cast<const float4*>(p)); }
+__device__ __forceinline__ float pick(const float4& v, int j) { return j == 0 ? v.x : j == 1 ? v.y : j == 2 ? v.z : v.w; }
+
+// K-major operand (element (x, k) at base[x * ld + k]), rows x0 .. x0+127, k0 .. k0+31 -> SWIZZLE_128B tile.
+// Thread t owns 16-byte chunk c = t % 8 of rows t / 8 + 16 i.
+template <class AX>
+__device__ __forceinline__ void load_tile_k(uint8_t* dst, const float* base, size_t ld, int x0, int X, int k0, int K, int t,
+                                            const AX& ax) {
+  const int c = t & 7, rg = t >> 3, k = k0 + c * 4;
+  float4 v[8];
 #pragma unroll
-    for (int ch = 0; ch < BM / 32; ++ch) {
-      uint8_t* row = sa + ch * (BK * 128) + lane * 128;
-      float4 v[8];                                           // v[2u + h] = classes m0 + 32 ch + 8 u + 4 h ..+3
-#pragma unroll
-      for (int q = 0; q < 8; ++q) v[q] = *reinterpret_cast<const float4*>(row + (((q >> 1) ^ (lane & 3)) << 5) + ((q & 1) << 4));
-      if (full) {
-#pragma unroll
-        for (int q = 0; q < 8; ++q) v[q] = softmax_grad4(v[q], p.c);
+  for (int i = 0; i < 8; ++i) {
+    const int x = x0 + rg + 16 * i;
+    v[i] = make_float4(0.f, 0.f, 0.f, 0.f);
+    if (x < X) {
+      const float* p = base + (size_t)x * ld + k;
+      if (k + 3 < K) {
+        v[i] = ld4(p);
       } else {
-#pragma unroll
-        for (int q = 0; q < 8; ++q) v[q] = softmax_grad4_tail(v[q], p.c, m0 + ch * 32 + q * 4, M);
+        if (k < K) v[i].x = p[0];
+        if (k + 1 < K) v[i].y = p[1];
+        if (k + 2 < K) v[i].z = p[2];
       }
-#pragma unroll
-      for (int q = 0; q < 8; ++q) *reinterpret_cast<float4*>(row + (((q >> 1) ^ (lane & 3)) << 5) + ((q & 1) << 4)) = v[q];
-      const int e = p.tgt - (m0 + ch * 32);
-      if (e >= 0 && e < 32)
-        *(reinterpret_cast<float*>(row + (((e >> 3) ^ (lane & 3)) << 5) + (((e >> 2) & 1) << 4)) + (e & 3)) -= a.inv_batch;
     }
   }
-};
+#pragma unroll
+  for (int i = 0; i < 8; ++i) {
+    const int r = rg + 16 * i;
+    if constexpr (AX::kKind == 1) v[i] = ax.xform(v[i], x0 + r, k, X, K);
+    *reinterpret_cast<float4*>(dst + r * 128 + ((c ^ (r & 7)) << 4)) = v[i];
+  }
+}
+
+// MN-major operand (element (x, k) at base[k * ld + x]), same tile.  A warp instruction reads 4 k-rows x 32
+// consecutive x (128 B each) and scatters the float4s into 4 tile rows; lane l stores its four elements in the
+// order (s + l / 8) % 4 so that the 32 scalar stores of one instruction hit 32 different banks.
+template <class AX>
+__device__ __forceinline__ void load_tile_mn(uint8_t* dst, const float* base, size_t ld, int x0, int X, int k0, int K, int t,
+                                             const AX& ax) {
+  const int warp = t >> 5, lane = t & 31;
+  float4 v[8];
+#pragma unroll
+  for (int i = 0; i < 8; ++i) {
+    const int idx = warp * 8 + i;
+    const int x = x0 + (idx & 3) * 32 + 4 * (lane >> 2), k = k0 + (idx >> 2) * 4 + (lane & 3);
+    v[i] = make_float4(0.f, 0.f, 0.f, 0.f);
+    if (k < K) {
+      const float* p = base + (size_t)k * ld + x;
+      if (x + 3 < X) {
+        v[i] = ld4(p);
+      } else {
+        if (x < X) v[i].x = p[0];
+        if (x + 1 < X) v[i].y = p[1];
+        if (x + 2 < X) v[i].z = p[2];
+      }
+    }
+  }
+#pragma unroll
+  for (int i = 0; i < 8; ++i) {
+    const int idx = warp * 8 + i;
+    const int r0 = (idx & 3) * 32 + 4 * (lane >> 2), kk = (idx >> 2) * 4 + (lane & 3);
+    if constexpr (AX::kKind == 1) v[i] = ax.xform(v[i], x0 + r0, k0 + kk, X, K);
+#pragma unroll
+    for (int s = 0; s < 4; ++s) {
+      const int j = (s + (lane >> 3)) & 3, r = r0 + j;
+      *reinterpret_cast<float*>(dst + r * 128 + ((((kk >> 2) ^ (r & 7))) << 4) + (kk & 3) * 4) = pick(v[i], j);
+    }
+  }
+}
+
+// gather(cs)[m0 .. m0+127, k-block kb] with dropout, as load_tile_k lays it out (d % 32 == 0: a k-block lies in one
+// of the three segments source token | path | target token)
+__device__ __forceinline__ void load_tile_gather(uint8_t* dst, const AXGather& g, int m0, int M, int kb, bool write_x, int t) {
+  const int c = t & 7, rg = t >> 3;
+  const int kps = g.cs.d / BK, seg = kb / kps;
+  const int col = (kb - seg * kps) * BK + c * 4;
+  const int32_t* ids = seg == 0 ? g.cs.src : seg == 1 ? g.cs.pth : g.cs.tgt;
+  const int K = 3 * g.cs.d;
+  float4 v[8];
+#pragma unroll
+  for (int i = 0; i < 8; ++i) {
+    const int m = m0 + rg + 16 * i;
+    v[i] = make_float4(0.f, 0.f, 0.f, 0.f);
+    if (m < M) v[i] = ld4(((seg == 1) ? table_row(g.cs.path, ids[m], g.cs.d) : table_row(g.cs.tok, ids[m], g.cs.d)) + col);
+  }
+#pragma unroll
+  for (int i = 0; i < 8; ++i) {
+    const int r = rg + 16 * i, m = m0 + r;
+    if (g.dp.enabled) {
+      const float4 mlt = dropout_mult4(g.dp, m, kb * (BK / 4) + c);
+      v[i].x *= mlt.x; v[i].y *= mlt.y; v[i].z *= mlt.z; v[i].w *= mlt.w;
+    }
+    *reinterpret_cast<float4*>(dst + r * 128 + ((c ^ (r & 7)) << 4)) = v[i];
+    if (write_x && m < M) *reinterpret_cast<float4*>(g.Xout + (size_t)m * K + kb * BK + c * 4) = v[i];
+  }
+}
 
 // ---- kernel -------------------------------------------------------------------------------------------
 struct GemmShape {
@@ -709,62 +657,55 @@ struct GemmShape {
   int n_fastest;              // raster order of work items: 1 = consecutive items share the A tile
   int terms;                  // 1 = plain tf32;  3 = 3xTF32: every K block is issued as A_lo.B_hi + A_hi.B_lo + A_hi.B_hi
 };
+// raw operand pointers (the loaders that do not go through TMA); lo = the 3xTF32 residuals or nullptr
+struct GemmPtrs {
+  const float *a, *a_lo, *b, *b_lo;
+  size_t lda, ldb;
+};
 
-template <int BN, int STAGES>
 struct SmemLayout {
   static constexpr int kABytes = BM * BK * 4;          // 16 KB
-  static constexpr int kBBytes = BN * BK * 4;
+  static constexpr int kBBytes = BN * BK * 4;          // 16 KB
   static constexpr int kStageBytes = kABytes + kBBytes;
-  static constexpr int kEpiStageOffset = STAGES * kStageBytes;                 // 8 x 4 KB store-transpose blocks
-  static constexpr int kBarOffset = kEpiStageOffset + kEpiWarps * kEpiStageBytes;
-  static constexpr int kTotal = kBarOffset + 256 + 1024;   // barriers + tmem ptr, + slack for 1024-B alignment
+  static constexpr int kEpiOffset = STAGES * kStageBytes;                     // per consumer warpgroup: 64 x BN fp32
+  static constexpr int kEpiBytes = 64 * BN * 4;
+  static constexpr int kBarOffset = kEpiOffset + 2 * kEpiBytes;
+  static constexpr int kTotal = kBarOffset + 256 + 1024;   // barriers, + slack for 1024-B alignment
   static_assert(kTotal <= 232448, "exceeds the 227 KB of shared memory a CTA can opt into");
 };
 
-template <int BN, int STAGES, bool A_MN, bool B_MN, class Epi, class AX = AXNone>
-__global__ void __launch_bounds__(kThreads + 32 * AX::kWarps, 1)
+template <bool A_MN, bool B_MN, class Epi, class AX = AXNone>
+__global__ void __launch_bounds__(kThreads, 1)
 umma_gemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB,
-                 const __grid_constant__ CUtensorMap tmAlo, const __grid_constant__ CUtensorMap tmBlo, GemmShape gs, Epi epi,
-                 AX ax = AX{}) {
+                 const __grid_constant__ CUtensorMap tmAlo, const __grid_constant__ CUtensorMap tmBlo, GemmShape gs,
+                 GemmPtrs ptr, Epi epi, AX ax = AX{}) {
   if (epi_gate_closed(epi, 0)) return;      // gated fallback pass: nothing to do (uniform over the grid)
-  using L = SmemLayout<BN, STAGES>;
+  using L = SmemLayout;
+  constexpr bool kTmaA = !A_MN && AX::kKind == 0;
+  constexpr bool kTmaB = !B_MN;
+  constexpr uint32_t kTxBytes = (kTmaA ? L::kABytes : 0) + (kTmaB ? L::kBBytes : 0);
   extern __shared__ uint8_t smem_raw[];
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~(uintptr_t)1023);
   uint64_t* full_bar = reinterpret_cast<uint64_t*>(smem + L::kBarOffset);
   uint64_t* empty_bar = full_bar + STAGES;
-  uint64_t* tfull_bar = empty_bar + STAGES;      // [2]
-  uint64_t* tempty_bar = tfull_bar + 2;          // [2]
-  uint64_t* xf_bar = tempty_bar + 2;             // [STAGES] A tile transformed (only with an A transform)
-  uint32_t* tmem_ptr = reinterpret_cast<uint32_t*>(xf_bar + STAGES);
 
-  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-  constexpr uint32_t kTmemCols = (2 * BN <= 256) ? 256 : 512;
-  constexpr bool kXform = AX::kWarps > 0;
+  const int wg = threadIdx.x >> 7, warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
   const int total_items = gs.m_tiles * gs.n_tiles * gs.splits;
   const int total_kblocks = (gs.K + BK - 1) / BK;
 
-  if (warp == 0 && lane == 0) {
-    for (int s = 0; s < STAGES; ++s) {
-      mbar_init(&full_bar[s], 1); mbar_init(&empty_bar[s], 1);
-      if (kXform) mbar_init(&xf_bar[s], 1);
-    }
-    for (int a = 0; a < 2; ++a) { mbar_init(&tfull_bar[a], 1); mbar_init(&tempty_bar[a], kEpiWarps); }
+  if (threadIdx.x == 0) {
+    for (int s = 0; s < STAGES; ++s) { mbar_init(&full_bar[s], 128); mbar_init(&empty_bar[s], 8); }
     asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
   }
-  if (warp == 1) tmem_alloc(tmem_ptr, kTmemCols);
-  tc_fence_before();
   __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem_base = *tmem_ptr;
 
-  // work item -> (m tile, n tile, split): m fastest so CTAs running together share B tiles in L2
   auto decode = [&](int item, int& mt, int& nt, int& sp) {
     if (gs.n_fastest) {
       nt = item % gs.n_tiles;
       const int r = item / gs.n_tiles;
       mt = r % gs.m_tiles;
       sp = r / gs.m_tiles;
-    } else {
+    } else {          // m fastest so CTAs running together share B tiles in L2
       mt = item % gs.m_tiles;
       const int r = item / gs.m_tiles;
       nt = r % gs.n_tiles;
@@ -772,154 +713,126 @@ umma_gemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant_
     }
   };
 
-  if (warp == 0) {
-    // ===================== TMA producer =====================
-    if (lane == 0) {
-      int stage = 0;
-      uint32_t phase = 0;
-      for (int item = blockIdx.x; item < total_items; item += gridDim.x) {
-        int mt, nt, sp;
-        decode(item, mt, nt, sp);
-        const int kb0 = sp * gs.kblocks_per_split;
-        const int kb1 = min(total_kblocks, kb0 + gs.kblocks_per_split);
-        // 3xTF32: the two small cross terms (A_lo.B_hi, A_hi.B_lo) over the whole K range first, then A_hi.B_hi.
-        // The tensor core adds into the fp32 accumulator with truncation, ~half an ulp of the accumulator per
-        // MMA; while only the 2^-11-sized cross terms have been added that loss is negligible, so the
-        // accumulation error is that of ONE pass over K instead of three.
-        auto load_stage = [&](const CUtensorMap* mA, const CUtensorMap* mB, int kb) {
-          mbar_wait(&empty_bar[stage], phase ^ 1);
-          uint8_t* sa = smem + stage * L::kStageBytes;
-          uint8_t* sb = sa + L::kABytes;
-          mbar_expect_tx(&full_bar[stage], L::kStageBytes);
-          if (A_MN) {
-            // global A^T is [K rows, M contiguous]: boxes of {32 m, BK k-rows} (4 KB each)
-#pragma unroll
-            for (int c = 0; c < BM / 32; ++c) tma_load_2d(sa + c * (BK * 128), mA, &full_bar[stage], mt * BM + c * 32, kb * BK);
-          } else {
-            // global A is [M rows, K contiguous]: one box {BK k, BM rows}
-            tma_load_2d(sa, mA, &full_bar[stage], kb * BK, mt * BM);
-          }
-          if (B_MN) {
-#pragma unroll
-            for (int c = 0; c < BN / 32; ++c) tma_load_2d(sb + c * (BK * 128), mB, &full_bar[stage], nt * BN + c * 32, kb * BK);
-          } else {
-            tma_load_2d(sb, mB, &full_bar[stage], kb * BK, nt * BN);
-          }
-          if (++stage == STAGES) { stage = 0; phase ^= 1; }
-        };
-        if (gs.terms == 3) {
-          for (int kb = kb0; kb < kb1; ++kb) load_stage(&tmAlo, &tmB, kb);
-          for (int kb = kb0; kb < kb1; ++kb) load_stage(&tmA, &tmBlo, kb);
-        }
-        for (int kb = kb0; kb < kb1; ++kb) load_stage(&tmA, &tmB, kb);
-      }
-    }
-  } else if (warp == 1) {
-    // ===================== MMA issuer =====================
-    if (lane == 0) {
-      constexpr uint32_t idesc = make_idesc_tf32(BM, BN, A_MN, B_MN);
-      // K-major (SWIZZLE_128B): rows of 128 B, 8-row groups 1024 B apart (SBO); one MMA consumes
-      //   32 B of each row, so the K step is +32 B inside the swizzle row.
-      // MN-major (SWIZZLE_128B_BASE32B): chunks of 32 M/N-elements x BK k-rows (128 B per k-row);
-      //   chunks are BK*128 B apart (LBO), 4-k-row swizzle atoms 512 B apart (SBO); one MMA consumes
-      //   8 k-rows, so the K step is +1024 B.
-      constexpr uint32_t a_lbo = A_MN ? BK * 128 : 0, b_lbo = B_MN ? BK * 128 : 0;
-      constexpr uint32_t a_sbo = A_MN ? 512 : 1024, b_sbo = B_MN ? 512 : 1024;
-      constexpr uint32_t a_lt = A_MN ? kLayoutSw128Base32 : kLayoutSw128, b_lt = B_MN ? kLayoutSw128Base32 : kLayoutSw128;
-      constexpr uint32_t a_kstep = A_MN ? 1024 : UMMA_K * 4, b_kstep = B_MN ? 1024 : UMMA_K * 4;
-      int stage = 0;
-      uint32_t phase = 0;
-      int acc = 0;
-      uint32_t acc_phase = 0;
-      for (int item = blockIdx.x; item < total_items; item += gridDim.x) {
-        int mt, nt, sp;
-        decode(item, mt, nt, sp);
-        const int kb0 = sp * gs.kblocks_per_split;
-        const int kb1 = min(total_kblocks, kb0 + gs.kblocks_per_split);
-        mbar_wait(&tempty_bar[acc], acc_phase ^ 1);          // epilogue has drained this accumulator
-        tc_fence_after();
-        const uint32_t tmem_d = tmem_base + acc * BN;
-        const int n_steps = (kb1 - kb0) * gs.terms;          // 3xTF32: three passes over the K range (see the producer)
-        for (int it = 0; it < n_steps; ++it) {
-          mbar_wait(kXform ? &xf_bar[stage] : &full_bar[stage], phase);    // with a transform: once the A tile has been rewritten
-          tc_fence_after();
-          const uint32_t sa = smem_u32(smem + stage * L::kStageBytes);
-          const uint32_t sb = sa + L::kABytes;
-          const uint64_t adesc = make_smem_desc(sa, a_lbo, a_sbo, a_lt);
-          const uint64_t bdesc = make_smem_desc(sb, b_lbo, b_sbo, b_lt);
-#pragma unroll
-          for (int k = 0; k < BK / UMMA_K; ++k) {
-            mma_tf32(tmem_d, adesc + (uint64_t)((k * a_kstep) >> 4), bdesc + (uint64_t)((k * b_kstep) >> 4), idesc,
-                     (it > 0 || k > 0) ? 1u : 0u);
-          }
-          tc_commit(&empty_bar[stage]);                       // frees the smem stage when the MMAs retire
-          if (++stage == STAGES) { stage = 0; phase ^= 1; }
-        }
-        tc_commit(&tfull_bar[acc]);                           // accumulator complete -> epilogue
-        if (++acc == 2) { acc = 0; acc_phase ^= 1; }
-      }
-    }
-  } else if (kXform && warp >= kEpiWarp0 + kEpiWarps) {
-    // ===================== A-transform warps =====================
-    // warp w takes every kWarps-th step of this CTA's (item, k-block) stream; step g lives in stage g % STAGES
-    constexpr int kXW = kXform ? AX::kWarps : 1;
-    static_assert(STAGES % kXW == 0, "a transform warp must always meet the same stages");
-    const int xw = warp - kEpiWarp0 - kEpiWarps;
-    int g = 0;
+  if (wg == 0) {
+    // ===================== producer warpgroup =====================
+    const int t = threadIdx.x;
+    int stage = 0;
+    uint32_t phase = 0;
     for (int item = blockIdx.x; item < total_items; item += gridDim.x) {
       int mt, nt, sp;
       decode(item, mt, nt, sp);
       const int kb0 = sp * gs.kblocks_per_split;
       const int kb1 = min(total_kblocks, kb0 + gs.kblocks_per_split);
-      for (int kb = kb0; kb < kb1; ++kb, ++g) {
-        if (g % kXW != xw) continue;
-        const int stage = g % STAGES;
-        const uint32_t phase = (uint32_t)(g / STAGES) & 1u;
-        typename AX::Pre pre;
-        ax.load(lane, mt * BM, kb * BK, gs.M, gs.K, pre);     // per-example scalars: in flight while the tile lands
-        mbar_wait(&full_bar[stage], phase);                   // the TMA tiles of this stage have landed
-        ax.apply(smem + stage * L::kStageBytes, lane, mt * BM, kb * BK, gs.M, gs.K, pre);
-        asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
-        __syncwarp();
-        if (lane == 0) mbar_arrive(&xf_bar[stage]);
+      // 3xTF32: the two small cross terms (A_lo.B_hi, A_hi.B_lo) over the whole K range first, then A_hi.B_hi.
+      // While only the 2^-11-sized cross terms have been accumulated, the rounding of the fp32 accumulator
+      // costs nothing that matters, so the accumulation error is that of ONE pass over K instead of three.
+      auto load_stage = [&](bool a_lo, bool b_lo, int kb) {
+        mbar_wait(&empty_bar[stage], phase ^ 1);
+        uint8_t* sa = smem + stage * L::kStageBytes;
+        uint8_t* sb = sa + L::kABytes;
+        const int k0 = kb * BK;
+        if (kTxBytes && t == 0) {
+          mbar_expect_tx(&full_bar[stage], kTxBytes);
+          if (kTmaA) tma_load_2d(sa, a_lo ? &tmAlo : &tmA, &full_bar[stage], k0, mt * BM);
+          if (kTmaB) tma_load_2d(sb, b_lo ? &tmBlo : &tmB, &full_bar[stage], k0, nt * BN);
+        }
+        if constexpr (AX::kKind == 2) {
+          load_tile_gather(sa, ax, mt * BM, gs.M, kb, ax.Xout != nullptr && nt == 0, t);
+        } else if constexpr (!kTmaA) {
+          if (A_MN) load_tile_mn(sa, a_lo ? ptr.a_lo : ptr.a, ptr.lda, mt * BM, gs.M, k0, gs.K, t, ax);
+          else load_tile_k(sa, a_lo ? ptr.a_lo : ptr.a, ptr.lda, mt * BM, gs.M, k0, gs.K, t, ax);
+        }
+        if constexpr (!kTmaB) load_tile_mn(sb, b_lo ? ptr.b_lo : ptr.b, ptr.ldb, nt * BN, gs.N, k0, gs.K, t, AXNone{});
+        if constexpr (!kTmaA || !kTmaB) fence_proxy_async_smem();     // generic-proxy stores -> visible to wgmma
+        mbar_arrive(&full_bar[stage]);
+        if (++stage == STAGES) { stage = 0; phase ^= 1; }
+      };
+      if (gs.terms == 3) {
+        for (int kb = kb0; kb < kb1; ++kb) load_stage(true, false, kb);
+        for (int kb = kb0; kb < kb1; ++kb) load_stage(false, true, kb);
       }
+      for (int kb = kb0; kb < kb1; ++kb) load_stage(false, false, kb);
     }
   } else {
-    // ===================== epilogue warps (TMEM lane quadrant = warp % 4) =====================
-    const int q = warp & 3;                       // TMEM lane quadrant this warp may access
-    const int half = (warp - kEpiWarp0) >> 2;     // which half of the tile's columns it drains
-    constexpr int kChunksPerHalf = BN / 64;
-    int acc = 0;
-    uint32_t acc_phase = 0;
+    // ===================== consumer warpgroups: rows 64 (wg - 1) .. of the tile =====================
+    const int cw = wg - 1, wl = warp & 3;
+    float* stg = reinterpret_cast<float*>(smem + L::kEpiOffset + cw * L::kEpiBytes);    // 8 blocks of 32 x 32
+    int stage = 0;
+    uint32_t phase = 0;
+    float acc[64];
     auto prefetch_item = [&](int it) {            // read-modify-write epilogues: warm L2 with the tile's destination lines
-      if (it >= total_items) return;
+      if (it >= total_items || (wl >> 1)) return;
       int mt2, nt2, sp2;
       decode(it, mt2, nt2, sp2);
-      epi_prefetch_tile(epi, mt2 * BM + q * 32 + lane, nt2 * BN + half * kChunksPerHalf * 32, kChunksPerHalf * 32, gs.M, gs.N, 0);
+      epi_prefetch_tile(epi, mt2 * BM + 64 * cw + 32 * (wl & 1) + lane, nt2 * BN, BN, gs.M, gs.N, 0);
     };
     prefetch_item(blockIdx.x);
     for (int item = blockIdx.x; item < total_items; item += gridDim.x) {
       int mt, nt, sp;
       decode(item, mt, nt, sp);
       prefetch_item(item + gridDim.x);
-      mbar_wait(&tfull_bar[acc], acc_phase);
-      tc_fence_after();
-      const int m = mt * BM + q * 32 + lane;
-      const uint32_t taddr = tmem_base + ((uint32_t)(q * 32) << 16) + acc * BN;
+      const int kb0 = sp * gs.kblocks_per_split;
+      const int kb1 = min(total_kblocks, kb0 + gs.kblocks_per_split);
+      const int n_steps = (kb1 - kb0) * gs.terms;          // 3xTF32: three passes over the K range (see the producer)
+      int prev = 0;
+      for (int it = 0; it < n_steps; ++it) {
+        mbar_wait(&full_bar[stage], phase);
+        const uint32_t sa = smem_u32(smem + stage * L::kStageBytes) + cw * 64 * 128;
+        const uint32_t sb = smem_u32(smem + stage * L::kStageBytes + L::kABytes);
+        wg_fence();
+#pragma unroll
+        for (int k = 0; k < BK / WG_K; ++k)
+          wgmma_tf32(acc, gmma_desc(sa + k * WG_K * 4), gmma_desc(sb + k * WG_K * 4), (it > 0 || k > 0) ? 1u : 0u);
+        wg_commit();
+        wg_wait<1>();                                       // the previous stage's products have retired: release it
+        if (it > 0 && lane == 0) mbar_arrive(&empty_bar[prev]);
+        prev = stage;
+        if (++stage == STAGES) { stage = 0; phase ^= 1; }
+      }
+      wg_wait<0>();
+      if (n_steps > 0 && lane == 0) mbar_arrive(&empty_bar[prev]);
+
+      // Epilogue.  The accumulator goes through shared memory (8 XOR-swizzled 32 x 32 blocks per warpgroup:
+      // block (row half, column quarter)) so that each thread then holds one row's 32 consecutive columns, the
+      // layout the functors' row-wise math and store_chunk's coalesced stores work on.  Warp wl drains row half
+      // wl & 1, column quarters wl >> 1 and (wl >> 1) + 2.
+      wg_bar_sync(1 + cw);                                  // the previous tile's epilogue has read its blocks
+#pragma unroll
+      for (int j = 0; j < BN / 8; ++j) {
+#pragma unroll
+        for (int i = 0; i < 2; ++i) {
+          const int r = 16 * wl + (lane >> 2) + 8 * i, cc = 8 * j + 2 * (lane & 3);
+          const int b = (r >> 5) | ((cc >> 5) << 1), rr = r & 31, c32 = cc & 31;
+          *reinterpret_cast<float2*>(stg + b * 1024 + rr * 32 + (((c32 >> 2) ^ (rr & 7)) << 2) + (c32 & 3)) =
+              make_float2(acc[4 * j + 2 * i], acc[4 * j + 2 * i + 1]);
+        }
+      }
+      wg_bar_sync(1 + cw);
+      const int m_base = mt * BM + 64 * cw + 32 * (wl & 1), m = m_base + lane;
+      float* cbase = epi.out(sp);
       typename Epi::State est;
       epi.begin(est);
-      drain_accumulator(epi, est, taddr, half * kChunksPerHalf * 32, kChunksPerHalf * 32, mt * BM + q * 32, lane, nt * BN,
-                        gs.M, gs.N, sp, reinterpret_cast<float*>(smem + L::kEpiStageOffset + (warp - kEpiWarp0) * kEpiStageBytes));
-      epi.end(m, 2 * nt + half, sp, m < gs.M, est);
-      tc_fence_before();
-      __syncwarp();
-      if (lane == 0) mbar_arrive(&tempty_bar[acc]);
-      if (++acc == 2) { acc = 0; acc_phase ^= 1; }
+#pragma unroll 1
+      for (int qq = 0; qq < 2; ++qq) {
+        const int q = (wl >> 1) + 2 * qq;
+        float* blk = stg + ((wl & 1) | (q << 1)) * 1024;
+        uint32_t r[32];
+#pragma unroll
+        for (int c4 = 0; c4 < 8; ++c4) {
+          const float4 x = *reinterpret_cast<const float4*>(blk + lane * 32 + ((c4 ^ (lane & 7)) << 2));
+          r[4 * c4] = __float_as_uint(x.x); r[4 * c4 + 1] = __float_as_uint(x.y);
+          r[4 * c4 + 2] = __float_as_uint(x.z); r[4 * c4 + 3] = __float_as_uint(x.w);
+        }
+        __syncwarp();
+        const int n = nt * BN + 32 * q;
+        if (n < gs.N) {
+          if (m < gs.M) epi.observe(m, n, r, gs.N - n, est);
+          if (epi_stores<Epi>(0)) store_chunk(epi, est, r, blk, lane, m_base, n, gs.M, gs.N, cbase, epi.ldc);
+        }
+      }
+      epi.end(m, 2 * nt + (wl >> 1), sp, m < gs.M, est);
     }
   }
-  tc_fence_before();
-  __syncthreads();
-  if (warp == 1) tmem_dealloc(tmem_base, kTmemCols);
 }
 
 // ---- host side ------------------------------------------------------------------------------------------
@@ -938,16 +851,15 @@ inline EncodeTiledFn get_encode_fn() {
   return fn;
 }
 
-// 2-D fp32 tensor map over a row-major [rows, cols] matrix with row pitch ld (floats); box = {32 cols, box_rows}.
-// Encoded maps are kept in a small per-thread cache: a training step issues the same dozen (buffer, shape)
-// combinations every time, so after the first step no launch calls into the driver for a descriptor.
+// 2-D fp32 tensor map over a row-major [rows, cols] matrix with row pitch ld (floats); box = {32 cols, box_rows},
+// SWIZZLE_128B.  Encoded maps are kept in a small per-thread cache: a training step issues the same dozen
+// (buffer, shape) combinations every time, so after the first step no launch calls into the driver for a descriptor.
 struct TensorMapKey {
   const float* base;
   uint64_t rows, cols, ld;
   uint32_t box_rows;
-  bool atom32;
   bool operator==(const TensorMapKey& o) const {
-    return base == o.base && rows == o.rows && cols == o.cols && ld == o.ld && box_rows == o.box_rows && atom32 == o.atom32;
+    return base == o.base && rows == o.rows && cols == o.cols && ld == o.ld && box_rows == o.box_rows;
   }
 };
 struct TensorMapCache {
@@ -956,10 +868,9 @@ struct TensorMapCache {
   CUtensorMap map[kCap];
   int n = 0, next = 0;
 };
-inline bool make_tensor_map(CUtensorMap* map, const float* base, uint64_t rows, uint64_t cols, uint64_t ld, uint32_t box_rows,
-                            bool atom32) {
+inline bool make_tensor_map(CUtensorMap* map, const float* base, uint64_t rows, uint64_t cols, uint64_t ld, uint32_t box_rows) {
   static thread_local TensorMapCache cache;
-  const TensorMapKey k{base, rows, cols, ld, box_rows, atom32};
+  const TensorMapKey k{base, rows, cols, ld, box_rows};
   for (int i = 0; i < cache.n; ++i)
     if (cache.key[i] == k) { *map = cache.map[i]; return true; }
   EncodeTiledFn fn = get_encode_fn();
@@ -969,8 +880,7 @@ inline bool make_tensor_map(CUtensorMap* map, const float* base, uint64_t rows, 
   cuuint32_t box[2] = {32, box_rows};
   cuuint32_t estr[2] = {1, 1};
   CUresult r = fn(map, CU_TENSOR_MAP_DATA_TYPE_FLOAT32, 2, const_cast<float*>(base), dims, strides, box, estr,
-                  CU_TENSOR_MAP_INTERLEAVE_NONE, atom32 ? CU_TENSOR_MAP_SWIZZLE_128B_ATOM_32B : CU_TENSOR_MAP_SWIZZLE_128B,
-                  CU_TENSOR_MAP_L2_PROMOTION_L2_256B,
+                  CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B,
                   CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
   if (r != CUDA_SUCCESS) return false;
   const int slot = (cache.n < TensorMapCache::kCap) ? cache.n++ : (cache.next++ % TensorMapCache::kCap);
@@ -990,27 +900,10 @@ struct Operand {
   const float* lo = nullptr;
 };
 
-template <int BN, int STAGES, bool A_MN, bool B_MN, class Epi, class AX = AXNone>
-inline cudaError_t launch_cfg(cudaStream_t st, int M, int N, int K, int splits, const Operand& A, const Operand& B, const Epi& epi,
-                              int num_sms, const AX& ax = AX{}) {
-  using L = SmemLayout<BN, STAGES>;
-  CUtensorMap tmA, tmB, tmAlo, tmBlo;
-  const bool three = A.lo != nullptr && B.lo != nullptr;
-  if ((A.lo != nullptr) != (B.lo != nullptr)) return cudaErrorInvalidValue;
-  auto mapA = [&](CUtensorMap* m, const float* base) {
-    return A_MN ? make_tensor_map(m, base, (uint64_t)K, (uint64_t)M, A.ld, BK, true)
-                : make_tensor_map(m, base, (uint64_t)M, (uint64_t)K, A.ld, BM, false);
-  };
-  auto mapB = [&](CUtensorMap* m, const float* base) {
-    return B_MN ? make_tensor_map(m, base, (uint64_t)K, (uint64_t)N, B.ld, BK, true)
-                : make_tensor_map(m, base, (uint64_t)N, (uint64_t)K, B.ld, BN, false);
-  };
-  if (!mapA(&tmA, A.base) || !mapB(&tmB, B.base)) return cudaErrorInvalidValue;
-  if (three) { if (!mapA(&tmAlo, A.lo) || !mapB(&tmBlo, B.lo)) return cudaErrorInvalidValue; }
-  else { tmAlo = tmA; tmBlo = tmB; }
+inline GemmShape make_shape(int M, int N, int K, int splits, int terms) {
   GemmShape gs;
   gs.M = M; gs.N = N; gs.K = K;
-  gs.terms = three ? 3 : 1;
+  gs.terms = terms;
   gs.m_tiles = (M + BM - 1) / BM;
   gs.n_tiles = (N + BN - 1) / BN;
   const int total_kblocks = (K + BK - 1) / BK;
@@ -1020,14 +913,40 @@ inline cudaError_t launch_cfg(cudaStream_t st, int M, int N, int K, int splits, 
   gs.splits = (total_kblocks + gs.kblocks_per_split - 1) / gs.kblocks_per_split;
   // few, wide n-tiles under many m-tiles: walk n fastest so the (large) A tile is fetched from HBM once
   gs.n_fastest = (gs.n_tiles < gs.m_tiles) ? 1 : 0;
-  if (AX::kWarps > 0 && three) return cudaErrorInvalidValue;      // the transforms rewrite a single fp32 tile
-  auto kern = umma_gemm_kernel<BN, STAGES, A_MN, B_MN, Epi, AX>;
-  cudaError_t e = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, L::kTotal);
+  return gs;
+}
+
+template <bool A_MN, bool B_MN, class Epi, class AX>
+inline cudaError_t launch_kernel(cudaStream_t st, const CUtensorMap& tmA, const CUtensorMap& tmB, const CUtensorMap& tmAlo,
+                                 const CUtensorMap& tmBlo, const GemmShape& gs, const GemmPtrs& ptr, const Epi& epi, int num_sms,
+                                 const AX& ax) {
+  auto kern = umma_gemm_kernel<A_MN, B_MN, Epi, AX>;
+  cudaError_t e = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, SmemLayout::kTotal);
   if (e != cudaSuccess) return e;
   int grid = gs.m_tiles * gs.n_tiles * gs.splits;
   if (grid > num_sms) grid = num_sms;
-  kern<<<grid, kThreads + 32 * AX::kWarps, L::kTotal, st>>>(tmA, tmB, tmAlo, tmBlo, gs, epi, ax);
+  kern<<<grid, kThreads, SmemLayout::kTotal, st>>>(tmA, tmB, tmAlo, tmBlo, gs, ptr, epi, ax);
   return cudaGetLastError();
+}
+
+template <bool A_MN, bool B_MN, class Epi, class AX = AXNone>
+inline cudaError_t launch_cfg(cudaStream_t st, int M, int N, int K, int splits, const Operand& A, const Operand& B, const Epi& epi,
+                              int num_sms, const AX& ax = AX{}) {
+  CUtensorMap tmA{}, tmB{}, tmAlo{}, tmBlo{};
+  const bool three = A.lo != nullptr && B.lo != nullptr;
+  if ((A.lo != nullptr) != (B.lo != nullptr)) return cudaErrorInvalidValue;
+  if (AX::kKind != 0 && three) return cudaErrorInvalidValue;      // the transforms rewrite a single fp32 tile
+  if (!A_MN && AX::kKind == 0) {
+    if (!make_tensor_map(&tmA, A.base, (uint64_t)M, (uint64_t)K, A.ld, BM)) return cudaErrorInvalidValue;
+    if (three && !make_tensor_map(&tmAlo, A.lo, (uint64_t)M, (uint64_t)K, A.ld, BM)) return cudaErrorInvalidValue;
+  }
+  if (!B_MN) {
+    if (!make_tensor_map(&tmB, B.base, (uint64_t)N, (uint64_t)K, B.ld, BN)) return cudaErrorInvalidValue;
+    if (three && !make_tensor_map(&tmBlo, B.lo, (uint64_t)N, (uint64_t)K, B.ld, BN)) return cudaErrorInvalidValue;
+  }
+  const GemmPtrs ptr{A.base, A.lo, B.base, B.lo, A.ld, B.ld};
+  return launch_kernel<A_MN, B_MN, Epi, AX>(st, tmA, tmB, tmAlo, tmBlo, make_shape(M, N, K, splits, three ? 3 : 1), ptr, epi,
+                                            num_sms, ax);
 }
 
 // number of split-K slices launch_cfg will actually produce
@@ -1039,15 +958,32 @@ inline int effective_splits(int K, int splits) {
   return (total_kblocks + per - 1) / per;
 }
 
-// Runtime dispatch over operand majors.  BN = 256 and BN = 192 both run 4 stages (192 / 160 KB) next to
-// the 32 KB of epilogue transpose blocks.
-template <int BN, int STAGES, class Epi>
+// (max, sum exp) partial slots per logits row: one per (row, tile, column parity of the draining warps)
+inline int lse_slots(int n) { return 2 * ((n + BN - 1) / BN); }
+
+// Runtime dispatch over operand majors.
+template <class Epi>
 inline cudaError_t launch(cudaStream_t st, int M, int N, int K, int splits, const Operand& A, const Operand& B, const Epi& epi,
                           int num_sms) {
-  if (!A.major_mn && !B.major_mn) return launch_cfg<BN, STAGES, false, false, Epi>(st, M, N, K, splits, A, B, epi, num_sms);
-  if (!A.major_mn && B.major_mn) return launch_cfg<BN, STAGES, false, true, Epi>(st, M, N, K, splits, A, B, epi, num_sms);
-  if (A.major_mn && !B.major_mn) return launch_cfg<BN, STAGES, true, false, Epi>(st, M, N, K, splits, A, B, epi, num_sms);
-  return launch_cfg<BN, STAGES, true, true, Epi>(st, M, N, K, splits, A, B, epi, num_sms);
+  if (!A.major_mn && !B.major_mn) return launch_cfg<false, false, Epi>(st, M, N, K, splits, A, B, epi, num_sms);
+  if (!A.major_mn && B.major_mn) return launch_cfg<false, true, Epi>(st, M, N, K, splits, A, B, epi, num_sms);
+  if (A.major_mn && !B.major_mn) return launch_cfg<true, false, Epi>(st, M, N, K, splits, A, B, epi, num_sms);
+  return launch_cfg<true, true, Epi>(st, M, N, K, splits, A, B, epi, num_sms);
+}
+
+// Fused context forward:  H[M, N] = epi( dropout(gather(cs))[M, K = 3d] . W[K, N] )  (tensorflow_model.py:238-252)
+// in one kernel -- the producer warpgroup gathers the embedding rows straight into the swizzled A stage, so the
+// gathered context matrix X' is never read back from HBM.  W row-major [K, N] (N contiguous).  Xout: nullptr or
+// [M, K] (written once when a backward pass needs X').  Precondition (checked by the caller): d % 32 == 0.
+template <class Epi>
+inline cudaError_t launch_ctx_fused(cudaStream_t st, int M, int N, const float* W, size_t ldw, const ContextSource& cs,
+                                    const Dropout& dp, float* Xout, const Epi& epi, int num_sms) {
+  const int K = 3 * cs.d;
+  GemmShape gs = make_shape(M, N, K, 1, 1);
+  gs.n_fastest = 1;          // the CTAs that run together share gathered rows through L2
+  const CUtensorMap none{};
+  const GemmPtrs ptr{nullptr, nullptr, W, nullptr, 0, ldw};
+  return launch_kernel<false, true, Epi, AXGather>(st, none, none, none, none, gs, ptr, epi, num_sms, AXGather{cs, dp, Xout});
 }
 
 // TMA constraints on an operand: 16-byte aligned base, row pitch a multiple of 16 bytes.

@@ -166,7 +166,7 @@ class PathAttentionEngine:
     def __init__(self, dims: EngineDims, device: int = 0, training: bool = True):
         import torch
         if not torch.cuda.is_available():
-            raise RuntimeError("PathAttentionEngine needs a CUDA device (B200); no CPU fallback exists")
+            raise RuntimeError("PathAttentionEngine needs a CUDA device (H100); no CPU fallback exists")
         self.torch = torch
         self.lib = load_library()
         self.dims = dims
@@ -289,7 +289,7 @@ class PathAttentionEngine:
 
     def selftest_gemm(self, A, B, a_mn: bool, b_mn: bool, M: int, N: int, K: int, bn: int = 192, splits: int = 1,
                       three: bool = False):
-        """Test hook: C[M,N] = A.B on the tcgen05 path.  A is [M,K] (a_mn False) or [K,M] (True) row-major,
+        """Test hook: C[M,N] = A.B on the tensor-core (wgmma) path.  A is [M,K] (a_mn False) or [K,M] (True) row-major,
         B is [N,K] (b_mn False) or [K,N] (True); returns C (slices summed on the host side of the test).
         three: as 3xTF32 (operands split on the device first)."""
         torch = self.torch

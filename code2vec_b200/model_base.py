@@ -1,4 +1,4 @@
-"""The model-backend seam of the reference (model_base.py:11-182), restated for the B200 backends.
+"""The model-backend seam of the reference (model_base.py:11-182), restated for the engine's backends.
 
 A backend written against the reference's `Code2VecModelBase` finds the same names here: the two
 result tuples, the constructor's order of events (verify the configuration, size the datasets,

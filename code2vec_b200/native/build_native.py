@@ -9,7 +9,9 @@ LIB = os.path.join(HERE, "libc2v_batcher.so")
 
 
 def needs_build() -> bool:
-    return (not os.path.exists(LIB)) or os.path.getmtime(LIB) < os.path.getmtime(SRC)
+    # this file counts as a source: it holds the compiler flags
+    newest = max(os.path.getmtime(SRC), os.path.getmtime(os.path.abspath(__file__)))
+    return (not os.path.exists(LIB)) or os.path.getmtime(LIB) < newest
 
 
 def build(force: bool = False) -> str:

@@ -1,5 +1,5 @@
 /*
- * c2v_b200.h -- C ABI of the B200-native path-attention engine (libc2v_b200.so).
+ * c2v_b200.h -- C ABI of the H100-native (sm_90a) path-attention engine (libc2v_b200.so).
  *
  * This is the drop-in boundary for code2vec's ONE hot path.  The reference (tech-srl/code2vec)
  * has no FFI of its own: its seam is the Python ABC Code2VecModelBase (model_base.py:37-182)
@@ -71,11 +71,11 @@ typedef struct c2v_tensors {
 /* Arithmetic of the three big matrix products (projection, logits, their gradients).
  *   C2V_MATH_FP32  : fp32 FFMA on the SIMT pipe -- the reference's own arithmetic class
  *                    (cuBLAS/Eigen SGEMM); used for bit-level top-k parity.
- *   C2V_MATH_TF32  : tcgen05.mma kind::tf32 (fp32 storage, 10-bit mantissa operands, fp32
- *                    accumulate in TMEM) -- what TensorFlow itself runs on Ampere+ GPUs.
+ *   C2V_MATH_TF32  : wgmma tf32 (fp32 storage, 10-bit mantissa operands, fp32
+ *                    accumulate in registers) -- what TensorFlow itself runs on Ampere+ GPUs.
  *   C2V_MATH_3XTF32: the same tensor-core kernels at fp32-equivalent accuracy: every operand is
  *                    split into tf32 high and low parts (x = hi + lo up to 2^-22 |x|) and a product
- *                    is issued as a_lo.b_hi + a_hi.b_lo + a_hi.b_hi into the same fp32 TMEM
+ *                    is issued as a_lo.b_hi + a_hi.b_lo + a_hi.b_hi into the same fp32 register
  *                    accumulator (the dropped a_lo.b_lo term is O(2^-22) relative); tanh / exp in the
  *                    epilogues use the correctly rounded library forms.  The reference's arithmetic
  *                    class (fp32 tf.matmul, tensorflow_model.py:226,252,297) on tensor cores. */
@@ -105,8 +105,8 @@ int c2v_bind_adam_state(c2v_engine* e, const c2v_tensors* m, const c2v_tensors* 
 
 /* Options: "math_mode" (c2v_math_mode), "deterministic" (reserved: only 0 is accepted -- the
  * embedding scatter-add uses float atomics; every other reduction is fixed-order), "cta_pair"
- * (tcgen05 GEMMs as CTA pairs, tcgen05.mma.cta_group::2: 0 never, 1 always, 2 auto = per GEMM,
- * wherever it measured faster; default 2), "dy_late" (where the target-table gradient GEMM dY = P^T.v -- with the
+ * (0, 1 or 2, default 2: accepted for ABI compatibility
+ * (it once selected CTA-pair GEMMs); the sm_90a GEMM has no CTA-pair form and ignores it), "dy_late" (where the target-table gradient GEMM dY = P^T.v -- with the
  * target table's Adam step in its epilogue when armed -- runs: 0 = right after dv on the caller's
  * stream, "target_grads_ready" fires earliest; 1 = default: inside the context backward pass, next
  * to the embedding scatter-add; 2 = on an engine-owned stream right after dv, joined before the
@@ -142,11 +142,11 @@ int c2v_bind_adam_state(c2v_engine* e, const c2v_tensors* m, const c2v_tensors* 
  * "exp_slab_fallbacks" counts those steps (the read synchronises the device), "sort_peer_access" (row-sharded
  * tables over peer memory: 0 never, 1 = default: when a table exceeds 2 GB, 2 always -- the step's row indices are
  * counting-sorted by (owner, 2 MB page) before the peer gather / scatter-add).
- * Experimental schedules, all correct, all measured slower on B200 and therefore 0 by default (DESIGN.md sections
+ * Experimental schedules, all correct, all 0 by default (DESIGN.md sections
  * 4.6 - 4.8): "fuse_gather" (the gather feeds the context GEMM's shared-memory stages directly), "fuse_softmax_grad"
  * (dv / dY turn logits into dL/dlogits as their A tiles land; tf32 mode), "recompute_logits" (the logits GEMM runs
  * twice instead of storing logits), "adam_epilogue_prefetch" (the dY GEMM's Adam epilogue prefetches the (theta, m, v)
- * lines of its next tile into L2: dY 0.77 ms instead of 0.69). */
+ * lines of its next tile into L2). */
 int c2v_set_option(c2v_engine* e, const char* key, int64_t value);
 int c2v_get_option(const c2v_engine* e, const char* key, int64_t* value);
 
@@ -201,7 +201,7 @@ int c2v_sampled_train_step(c2v_engine* e, const int32_t* src, const int32_t* pat
 int c2v_adam_step(c2v_engine* e, float lr, float beta1, float beta2, float eps, int64_t t,
                   void* stream);
 
-/* Folds the TARGET_WORDS_VOCAB part of that update into the backward pass (tcgen05 path, full
+/* Folds the TARGET_WORDS_VOCAB part of that update into the backward pass (tensor-core path, full
  * softmax): once armed, the next target-gradient product dY = P^T.v applies Adam step t to
  * (theta, m, v) of the target table in its epilogue -- bit-identical to c2v_adam_step, but dY is
  * never written (the bound target gradient buffer keeps stale values) and the 401 MB table is not
@@ -343,7 +343,7 @@ int c2v_predict_batch_host(c2v_engine* e, const int32_t* h_src, const int32_t* h
                            int32_t normalize, int32_t* h_topk_idx, float* h_topk_val,
                            float* h_code_vec, float* h_attn, void* stream);
 
-/* Test hook for the tcgen05 GEMM building block: C = A . B with tf32 operands.  a_mn / b_mn
+/* Test hook for the tensor-core (wgmma) GEMM building block: C = A . B with tf32 operands.  a_mn / b_mn
  * select the operand layout (0: K contiguous, element (x,k) at p[x*ld+k]; 1: M resp. N
  * contiguous, element (x,k) at p[k*ld+x]); bn is the N tile (192 or 256); with splits > 1,
  * slice s of the K range is written to C + s*M*ldc.  Returns the number of slices (> 0) or an

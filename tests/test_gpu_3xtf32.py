@@ -1,5 +1,5 @@
-"""C2V_MATH_3XTF32: the tcgen05 GEMM issued as a_lo.b_hi + a_hi.b_lo + a_hi.b_hi on tf32 (hi, lo) operand
-splits, fp32 accumulation in TMEM -- fp32-equivalent results on the tensor cores.  The building block is
+"""C2V_MATH_3XTF32: the wgmma GEMM issued as a_lo.b_hi + a_hi.b_lo + a_hi.b_hi on tf32 (hi, lo) operand
+splits, fp32 accumulation in registers -- fp32-equivalent results on the tensor cores.  The building block is
 checked against a float64 product at an fp32-class bound (about 2000x tighter than the plain tf32 bound of
 tests/test_gpu_umma.py) for every operand layout; the whole path in this mode runs the fp32 parity tests of
 tests/test_gpu_parity.py (math = 2) at their fp32 tolerances."""

@@ -1,7 +1,7 @@
 """Target-table Adam folded into the dY epilogue (c2v_arm_target_adam, option "fuse_target_adam").
 The epilogue applies the same correctly rounded fp32 operations as adam_kernel to the same
 accumulator values, so the target table and its two slots must come out BIT-identical to the
-unfused train_step + adam_step pair (tensorflow_model.py:232), on both tcgen05 kernels, with ragged
+unfused train_step + adam_step pair (tensorflow_model.py:232), with every cta_pair setting, with ragged
 tile tails, over several steps, together with lazy Adam and through the host entry point."""
 import numpy as np
 import pytest

@@ -18,7 +18,7 @@ LARGE = O.Dims(token_vocab=3001, path_vocab=2003, target_vocab=2600, embed_dim=2
 
 GAP_EPS = 1e-6
 LOSS_TOL = 1e-4
-# the two fp32-class arithmetic modes: 0 = fp32 FFMA on the SIMT pipe, 2 = 3xTF32 on the tensor cores (tcgen05)
+# the two fp32-class arithmetic modes: 0 = fp32 FFMA on the SIMT pipe, 2 = 3xTF32 on the tensor cores (wgmma)
 FP32_MODES = [0, 2]
 
 

@@ -1,4 +1,4 @@
-"""The tensor-core path (math_mode = tf32: tcgen05.mma kind::tf32, fp32 accumulate) against the fp32
+"""The tensor-core path (math_mode = tf32: wgmma tf32, fp32 accumulate) against the fp32
 oracle.  tf32 operands keep 10 mantissa bits, so outputs are compared at tf32-level tolerances
 (stated per assertion); the loss bound of BASELINE.json (1e-4) still holds."""
 import numpy as np
@@ -72,7 +72,7 @@ def test_tf32_train_step(dims, B, cta_pair):
 
 @pytest.mark.parametrize("dims,B,keep", [(TINY, 64, 1.0), (TINY, 64, 0.75), (MID, 48, 0.75), (LARGE, 12, 0.75), (MID, 3, 1.0)])
 def test_fused_gather_projection_is_bit_identical_to_the_unfused_path(dims, B, keep):
-    """ctx_fused.cuh (gather -> dropout -> tcgen05 projection -> tanh in one kernel) feeds the tensor core the same
+    """umma::launch_ctx_fused (gather -> dropout -> wgmma projection -> tanh in one kernel) feeds the tensor core the same
     operand image TMA would have loaded from a materialised X', so everything downstream of it must carry the same
     bits as with option fuse_gather = 0: code vectors, attention, loss, and the gradients that do not go through
     float atomics (dW reads the X' the fused kernel wrote out)."""
@@ -100,8 +100,8 @@ def test_fused_gather_projection_is_bit_identical_to_the_unfused_path(dims, B, k
 
 @pytest.mark.parametrize("dims,B", [(TINY, 64), (ODD, 37), (MID, 48), (LARGE, 12)])
 def test_softmax_gradient_computed_inside_the_gradient_gemms(dims, B):
-    """Option fuse_softmax_grad (off by default: measured slower on B200, see DESIGN.md): the dv = P.Ytab and dY = P^T.v GEMMs read the LOGITS slab and turn each A tile
-    into (softmax - onehot)/B in shared memory (umma_gemm.cuh, AXSoftmaxGradK / AXSoftmaxGradMN) instead of reading a slab
+    """Option fuse_softmax_grad (off by default): the dv = P.Ytab and dY = P^T.v GEMMs read the LOGITS slab and turn each A tile
+    into (softmax - onehot)/B in shared memory (umma_gemm.cuh, AXSoftmaxGrad<true> / AXSoftmaxGrad<false>, in the GEMM's loaders) instead of reading a slab
     that a separate pass rewrote.  Same gradients as with the separate pass, to the rounding of one exp (ex2.approx vs expf
     on values that are then cut to tf32 anyway), and as the oracle's at the tf32 tolerance."""
     src, pth, tgt, mask, target = O.synthetic_batch(dims, B, seed=51)
@@ -125,7 +125,7 @@ def test_softmax_gradient_computed_inside_the_gradient_gemms(dims, B):
 @pytest.mark.parametrize("math", [1, 2])
 @pytest.mark.parametrize("dims,B", [(TINY, 64), (ODD, 37), (MID, 48)])
 def test_recomputed_logits_schedule_matches_the_stored_one(dims, B, math):
-    """Option recompute_logits (off by default: a 0.06 ms gain in tf32, a loss in 3xTF32): the logits GEMM runs twice -- once leaving only the
+    """Option recompute_logits (off by default): the logits GEMM runs twice -- once leaving only the
     log-sum-exp partials, once writing (softmax - onehot)/B from its epilogue -- so the [B, Y] slab is written once and never
     rewritten.  The gradients must be those of the schedule that stores logits and rewrites them (same products, same exp),
     the loss may differ by the fp32-vs-tensor-core rounding of the one true-class logit per example."""

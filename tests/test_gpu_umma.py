@@ -1,5 +1,5 @@
-"""The tcgen05 (kind::tf32) GEMM building block against a float64 product, for every operand
-layout combination the engine uses, with M/N/K tails (TMA zero fill) and split-K.
+"""The wgmma (tf32) GEMM building block against a float64 product, for every operand
+layout combination the engine uses, with M/N/K tails (zero fill) and split-K.
 Tolerance: tf32 operands carry 10 mantissa bits -> relative error per product <= 2^-10; with
 random data the result error is far below 4e-3 * sum_k |a||b|, while a wrong shared-memory
 descriptor / swizzle gives O(1) errors."""
@@ -19,7 +19,7 @@ TINY = O.Dims(token_vocab=101, path_vocab=51, target_vocab=101, embed_dim=32, co
 @pytest.mark.parametrize("M,N,K,bn,splits", [(128, 192, 32, 192, 1), (256, 384, 384, 192, 1), (300, 200, 100, 192, 1),
                                               (1024, 1000, 384, 256, 1), (130, 384, 4100, 192, 7), (384, 384, 2000, 192, 48)])
 def test_umma_gemm_matches_float64(a_mn, b_mn, M, N, K, bn, splits, cta_pair):
-    """cta_pair = 1: the tcgen05.mma.cta_group::2 kernel (UMMA 256 x BN over two SMs, umma_gemm2.cuh)."""
+    """cta_pair is accepted and ignored on sm_90a: both settings must give the same correct product."""
     import torch
     eng, _ = make_engine(TINY, max_batch=8)
     eng.set_option("cta_pair", cta_pair)

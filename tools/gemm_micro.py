@@ -1,4 +1,4 @@
-"""Times the tcgen05 GEMM kernels alone (c2v_selftest_gemm) at the shapes of the train step."""
+"""Times the tensor-core (wgmma) GEMM kernels alone (c2v_selftest_gemm) at the shapes of the train step."""
 import os
 import sys
 

@@ -1,5 +1,5 @@
 #!/usr/bin/env python
-"""End-to-end check of the whole user path on one B200: a synthetic java14m-shaped `.c2v` file ->
+"""End-to-end check of the whole user path on one GPU: a synthetic java14m-shaped `.c2v` file ->
 PathContextReader (native tensoriser, prefetch thread) -> Code2VecModel.train() -> C-ABI engine.
 Prints one JSON line with examples/s and path-contexts/s as the reference's own progress line would
 report them (tensorflow_model.py:424-430).  Not part of bench.py: text parsing is host work outside
