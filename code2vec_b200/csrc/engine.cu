@@ -143,6 +143,29 @@ struct PhaseLog {
   int64_t count = 0;
 };
 
+// Schedule of the softmax head (logits -> cross entropy -> dL/dlogits -> dv, dY) for one call: head_schedule() picks it
+enum HeadSchedule {
+  HEAD_SIMT,        // fp32: SIMT logits; the fused step's xent_kernel writes P = dL/dlogits in place
+  HEAD_TWO_PASS,    // logits (+ log-sum-exp partials), rewritten to P by softmax_grad_kernel
+  HEAD_LOADERS,     // logits (+ partials), turned into P by the dv / dY GEMMs' A loaders (tf32, option fuse_softmax_grad)
+  HEAD_RECOMPUTE,   // a log-sum-exp-only logits pass, then a second one whose epilogue writes P (option recompute_logits)
+  HEAD_EXP_SLAB,    // U = exp(s - true logit), normalised by per-row factors inside dv / dY (option exp_slab)
+};
+
+// How the dv / dY GEMMs read the slab: as P, as P with row i scaled by row_scale[i] (exp_slab: dv's reduction applies the
+// factor, dY's code vectors come scaled by it), or as logits that the GEMMs' A loaders turn into P (loaders, sg)
+struct SlabDesc {
+  const float* row_scale = nullptr;
+  bool loaders = false;
+  umma::SoftmaxGradArgs sg{};
+};
+
+struct PendingDy {            // a dY = P^T . v deferred into context_backward (option dy_late == 1); v == nullptr: none
+  const float* v = nullptr;
+  int B = 0;
+  SlabDesc slab;
+};
+
 struct c2v_engine {
   PhaseLog phase[PH_COUNT];
   int profile = 0;
@@ -186,24 +209,20 @@ struct c2v_engine {
                              // dv / dY GEMMs, so no pass re-reads the slab to turn logits into dL/dlogits (DESIGN.md section 4.9).  Rows
                              // outside the fp32 window make that step fall back, on the device, to the two-pass schedule.
   bool slab_flag_zeroed = false;
-  bool slab_exp_live = false;         // c2v_target_forward left U (not logits) in the slab: c2v_target_backward finishes that schedule
+  HeadSchedule split_fwd = HEAD_SIMT;   // schedule of the last c2v_target_forward, for c2v_target_backward (HEAD_SIMT once consumed)
   int gather_occ[2] = {0, 0};         // resident CTAs per SM of gather_ctx_kernel<false / true>, queried once
   int adam_epi_prefetch = 0; // option "adam_epilogue_prefetch" (off by default): the dY epilogue's Adam update prefetches its (theta, m, v)
                              // lines into L2 one tile ahead
-  const float* row_scale = nullptr;   // while the step's dv GEMM runs: the per-example factor its split-K reduction applies
   int fuse_sg = 0;           // option "fuse_softmax_grad": dv / dY compute dL/dlogits from the logits slab on the fly (tf32 mode):
                              // the GEMM's loaders transform each A element on its way into shared memory, which removes the 2.1 GB
                              // softmax-gradient pass but takes the A operand off TMA; off by default
-  bool sg_live = false;      // ws.S holds LOGITS and sg describes how dv / dY turn them into dL/dlogits
-  umma::SoftmaxGradArgs sg{};
   int fuse_gather = 0;       // option "fuse_gather": gather -> projection -> tanh as one kernel on the tf32 path (umma::launch_ctx_fused);
                              // bit-identical to the two-kernel path; off by default
   int cta_pair = 2;          // option "cta_pair": accepted and validated, no effect (the sm_90a GEMM has no CTA-pair form)
   int num_sms;
   cudaEvent_t ev_tgt_ready = nullptr;   // recorded after dY (caller-owned)
   int dy_late = 1;                      // where dY = P^T.v runs: 0 after dv, 1 inside context_backward, 2 on side2 after dv
-  const float* pending_dy_v = nullptr;  // code vectors of the deferred dY product
-  int pending_dy_B = 0;
+  PendingDy pending_dy;
   cudaStream_t side = nullptr;          // engine-owned: the embedding scatter-add runs here, next to the dY / dW GEMMs
   cudaEvent_t ev_fork = nullptr, ev_join = nullptr;
   cudaStream_t copy = nullptr;          // engine-owned: host -> device copies of c2v_train_batch_async
@@ -287,12 +306,40 @@ inline int rest_ok(const c2v_engine* e) {
 }
 inline bool is_tc(const c2v_engine* e) { return e->math_mode != C2V_MATH_FP32; }          // tensor-core (wgmma) GEMMs
 inline bool is_3x(const c2v_engine* e) { return e->math_mode == C2V_MATH_3XTF32; }        // ... as 3xTF32
+inline bool aligned16(const void* p) { return reinterpret_cast<uintptr_t>(p) % 16 == 0; }
 
-// tensor-core GEMM launchers (umma_gemm.cuh): runtime dispatch over the operand majors, or the majors fixed at compile
-// time (the fused-epilogue GEMMs each have one layout, so only that instantiation is built): AMN / BMN = operand is
-// M- resp. N-contiguous in memory
-#define C2V_UMMA(...) umma::launch(__VA_ARGS__)
-#define C2V_UMMA_FIXED(AMN, BMN, EPI, ...) umma::launch_cfg<AMN, BMN, EPI>(__VA_ARGS__)
+enum HeadApi { API_STEP, API_TARGET_FORWARD, API_TARGET_BACKWARD, API_LOSS };
+
+// The one place that decides the softmax head's schedule, for the API asking and its code vectors v:
+//   fused step       fp32 -> SIMT; recompute_logits -> RECOMPUTE (wins over exp_slab); exp_slab -> EXP_SLAB (both only
+//                    without fuse_softmax_grad); tf32 with fuse_softmax_grad -> LOADERS; otherwise TWO_PASS
+//   target_forward   tensor core, v 16-B aligned, exp_slab, not fuse_softmax_grad, grads bound -> EXP_SLAB (recompute_logits
+//                    does not apply here); otherwise TWO_PASS (lse partials) if tensor core and aligned, else SIMT
+//   target_backward  the forward left U in the slab -> EXP_SLAB; otherwise tf32 with fuse_softmax_grad -> LOADERS, else
+//                    softmax_grad_kernel<3xTF32> rewrites the slab (TWO_PASS, SIMT in fp32)
+//   c2v_loss         tensor core and aligned -> TWO_PASS (lse partials + xent_combine_kernel), else SIMT (xent_kernel)
+// run_logits sends a call that is not on the tensor cores to the SIMT GEMM, which only stores logits: none of the
+// schedules above asks it for more.
+HeadSchedule head_schedule(const c2v_engine* e, HeadApi api, const float* v) {
+  const bool tc_aligned = is_tc(e) && aligned16(v);
+  switch (api) {
+    case API_STEP:
+      if (!is_tc(e)) return HEAD_SIMT;
+      if (e->recompute && !e->fuse_sg) return HEAD_RECOMPUTE;
+      if (e->exp_slab && !e->fuse_sg) return HEAD_EXP_SLAB;
+      return (e->fuse_sg && !is_3x(e)) ? HEAD_LOADERS : HEAD_TWO_PASS;
+    case API_TARGET_FORWARD:
+      if (!tc_aligned) return HEAD_SIMT;
+      return (e->exp_slab && !e->fuse_sg && e->has_grad) ? HEAD_EXP_SLAB : HEAD_TWO_PASS;
+    case API_TARGET_BACKWARD:
+      if (e->split_fwd == HEAD_EXP_SLAB) return HEAD_EXP_SLAB;
+      if (!is_tc(e)) return HEAD_SIMT;
+      return (e->fuse_sg && !is_3x(e)) ? HEAD_LOADERS : HEAD_TWO_PASS;
+    case API_LOSS:
+      return tc_aligned ? HEAD_TWO_PASS : HEAD_SIMT;
+  }
+  return HEAD_SIMT;
+}
 
 template <class T> T* wsp(c2v_engine* e, size_t off) { return reinterpret_cast<T*>(e->wbase + off); }
 
@@ -627,10 +674,10 @@ int run_ctx_fwd(c2v_engine* e, cudaStream_t st, const ContextSource& cs, const D
     umma::Operand opB{x3 ? wsp<float>(e, e->ws.W_hi) : e->theta.W, (size_t)D, true, x3 ? wsp<float>(e, e->ws.W_lo) : nullptr};
     if (x3) {
       umma::EpiTanhStorePrecise ep{H, (size_t)D};
-      C2V_LAUNCH(e, C2V_CUDA(e, (C2V_UMMA_FIXED(false, true, umma::EpiTanhStorePrecise, st, cs.rows, D, K, 1, opA, opB, ep, e->num_sms))));
+      C2V_LAUNCH(e, C2V_CUDA(e, (umma::launch_cfg<false, true, umma::EpiTanhStorePrecise>(st, cs.rows, D, K, 1, opA, opB, ep, e->num_sms))));
     } else {
       umma::EpiTanhStore ep{H, (size_t)D};
-      C2V_LAUNCH(e, C2V_CUDA(e, (C2V_UMMA_FIXED(false, true, umma::EpiTanhStore, st, cs.rows, D, K, 1, opA, opB, ep, e->num_sms))));
+      C2V_LAUNCH(e, C2V_CUDA(e, (umma::launch_cfg<false, true, umma::EpiTanhStore>(st, cs.rows, D, K, 1, opA, opB, ep, e->num_sms))));
     }
     return C2V_OK;
   }
@@ -642,74 +689,67 @@ int run_ctx_fwd(c2v_engine* e, cudaStream_t st, const ContextSource& cs, const D
   return C2V_OK;
 }
 
-// S[B, Y] = v . Ytab^T   (tensorflow_model.py:226,297)
-// with_lse (tf32 path only): also emit per-(row, partial slot) log-sum-exp partials (umma::lse_slots) into ws.lse_part.
-// grad != nullptr: the pass writes dL/dlogits (EpiSoftmaxGrad); lse_only: nothing but the log-sum-exp partials.
-struct LogitsGrad { const float* lse; const int32_t* target; int row0; float inv_batch; };
-// exp_offset != nullptr: the pass writes U = exp(logit - exp_offset[row]) and (max U, sum U) partials (EpiExpSum).
-// gate != nullptr (with_lse): the launch is the exp_slab schedule's fallback, a no-op while *gate == 0; it reuses the operand
-// splits the step's first pass made.
-int run_logits(c2v_engine* e, cudaStream_t st, const float* v, int B, float* S, bool with_lse = false, bool lse_only = false,
-               const LogitsGrad* grad = nullptr, const float* exp_offset = nullptr, const int* gate = nullptr) {
+// What the logits GEMM S[B, Y] = v . Ytab^T (tensorflow_model.py:226,297) leaves in ws.S; "partials" are the per-(row,
+// partial slot) (max, sum exp) pairs (umma::lse_slots) it also writes to ws.lse_part
+enum LogitsOut {
+  LOGITS_STORE,            // the logits
+  LOGITS_STORE_LSE,        // the logits and their partials
+  LOGITS_LSE_ONLY,         // the partials only
+  LOGITS_SOFTMAX_GRAD,     // dL/dlogits = (softmax - onehot) * inv_batch, from the log-sum-exp in LogitsArgs::sg
+  LOGITS_EXP_SUM,          // U = exp(s - LogitsArgs::exp_offset[row]) and (max U, sum U) partials
+  LOGITS_STORE_LSE_GATED,  // as LOGITS_STORE_LSE while *LogitsArgs::gate != 0, else nothing (the exp_slab fallback)
+};
+struct LogitsArgs {
+  const float* exp_offset;
+  const int* gate;
+  umma::SoftmaxGradArgs sg;
+};
+
+template <bool X3>
+int launch_logits(c2v_engine* e, cudaStream_t st, const float* v, int B, LogitsOut out, const LogitsArgs& a) {
   const int D = e->dims.code_dim, Y = e->dims.target_vocab;
-  { int rcl = end_target_lazy(e, st); if (rcl) return rcl; }      // a pass over the whole table needs every row current
-  if (is_tc(e) && (reinterpret_cast<uintptr_t>(v) % 16 == 0)) {
-    const bool x3 = is_3x(e);
-    umma::Operand opA{v, (size_t)D, false};
-    umma::Operand opB{e->theta.tgt, (size_t)D, false};
-    if (x3) {      // fp32-faithful: both operands as tf32 (hi, lo) pairs; the table is re-split on every pass over it
-      int rcs;
-      if (!gate) {
-        if ((rcs = split_small(e, st, v, (size_t)B * D, e->ws.v_hi, e->ws.v_lo))) return rcs;
-        if ((rcs = split_small(e, st, e->theta.tgt, (size_t)Y * D, e->ws.tgt_hi, e->ws.tgt_lo))) return rcs;
-      }
-      e->tgt_split_valid = true;
-      opA.base = wsp<float>(e, e->ws.v_hi); opA.lo = wsp<float>(e, e->ws.v_lo);
-      opB.base = wsp<float>(e, e->ws.tgt_hi); opB.lo = wsp<float>(e, e->ws.tgt_lo);
+  umma::Operand opA{v, (size_t)D, false};
+  umma::Operand opB{e->theta.tgt, (size_t)D, false};
+  if (X3) {      // fp32-faithful: both operands as tf32 (hi, lo) pairs; the gated fallback reuses the previous pass's splits
+    int rcs;
+    if (out != LOGITS_STORE_LSE_GATED) {
+      if ((rcs = split_small(e, st, v, (size_t)B * D, e->ws.v_hi, e->ws.v_lo))) return rcs;
+      if ((rcs = split_small(e, st, e->theta.tgt, (size_t)Y * D, e->ws.tgt_hi, e->ws.tgt_lo))) return rcs;
     }
-    PhaseTimer pt(e, PH_LOGITS, st);
-    const int slots = umma::lse_slots(Y);
-    if (exp_offset && x3) {
-      umma::EpiExpSumT<true, true> ep{S, wsp<float>(e, e->ws.S_lo), e->ws.ldS, exp_offset, wsp<float2>(e, e->ws.lse_part), slots};
-      C2V_LAUNCH(e, C2V_CUDA(e, (C2V_UMMA_FIXED(false, false, decltype(ep), st, B, Y, D, 1, opA, opB, ep, e->num_sms))));
-    } else if (exp_offset) {
-      umma::EpiExpSumT<false, false> ep{S, nullptr, e->ws.ldS, exp_offset, wsp<float2>(e, e->ws.lse_part), slots};
-      C2V_LAUNCH(e, C2V_CUDA(e, (C2V_UMMA_FIXED(false, false, decltype(ep), st, B, Y, D, 1, opA, opB, ep, e->num_sms))));
-    } else if (gate && x3) {
-      umma::EpiStoreLseGatedT<true> ep{{S, e->ws.ldS, wsp<float2>(e, e->ws.lse_part), slots}, gate};
-      C2V_LAUNCH(e, C2V_CUDA(e, (C2V_UMMA_FIXED(false, false, decltype(ep), st, B, Y, D, 1, opA, opB, ep, e->num_sms))));
-    } else if (gate) {
-      umma::EpiStoreLseGatedT<false> ep{{S, e->ws.ldS, wsp<float2>(e, e->ws.lse_part), slots}, gate};
-      C2V_LAUNCH(e, C2V_CUDA(e, (C2V_UMMA_FIXED(false, false, decltype(ep), st, B, Y, D, 1, opA, opB, ep, e->num_sms))));
-    } else if (grad && x3) {
-      umma::EpiSoftmaxGradT<true, true> ep{S, wsp<float>(e, e->ws.S_lo), e->ws.ldS, grad->lse, grad->target, grad->row0, grad->inv_batch, B};
-      C2V_LAUNCH(e, C2V_CUDA(e, (C2V_UMMA_FIXED(false, false, decltype(ep), st, B, Y, D, 1, opA, opB, ep, e->num_sms))));
-    } else if (grad) {
-      umma::EpiSoftmaxGradT<false, false> ep{S, nullptr, e->ws.ldS, grad->lse, grad->target, grad->row0, grad->inv_batch, B};
-      C2V_LAUNCH(e, C2V_CUDA(e, (C2V_UMMA_FIXED(false, false, decltype(ep), st, B, Y, D, 1, opA, opB, ep, e->num_sms))));
-    } else if (lse_only && x3) {
-      umma::EpiLseOnlyT<true> ep{{S, e->ws.ldS, wsp<float2>(e, e->ws.lse_part), slots}};
-      C2V_LAUNCH(e, C2V_CUDA(e, (C2V_UMMA_FIXED(false, false, decltype(ep), st, B, Y, D, 1, opA, opB, ep, e->num_sms))));
-    } else if (lse_only) {
-      umma::EpiLseOnlyT<false> ep{{S, e->ws.ldS, wsp<float2>(e, e->ws.lse_part), slots}};
-      C2V_LAUNCH(e, C2V_CUDA(e, (C2V_UMMA_FIXED(false, false, decltype(ep), st, B, Y, D, 1, opA, opB, ep, e->num_sms))));
-    } else if (with_lse && x3) {
-      umma::EpiStoreLsePrecise ep{S, e->ws.ldS, wsp<float2>(e, e->ws.lse_part), umma::lse_slots(Y)};
-      C2V_LAUNCH(e, C2V_CUDA(e, (C2V_UMMA_FIXED(false, false, umma::EpiStoreLsePrecise, st, B, Y, D, 1, opA, opB, ep, e->num_sms))));
-    } else if (with_lse) {
-      umma::EpiStoreLse ep{S, e->ws.ldS, wsp<float2>(e, e->ws.lse_part), umma::lse_slots(Y)};
-      C2V_LAUNCH(e, C2V_CUDA(e, (C2V_UMMA_FIXED(false, false, umma::EpiStoreLse, st, B, Y, D, 1, opA, opB, ep, e->num_sms))));
-    } else {
-      umma::EpiStore ep{S, e->ws.ldS, 0};
-      C2V_LAUNCH(e, C2V_CUDA(e, (C2V_UMMA(st, B, Y, D, 1, opA, opB, ep, e->num_sms))));
-    }
-    return C2V_OK;
+    e->tgt_split_valid = true;
+    opA.base = wsp<float>(e, e->ws.v_hi); opA.lo = wsp<float>(e, e->ws.v_lo);
+    opB.base = wsp<float>(e, e->ws.tgt_hi); opB.lo = wsp<float>(e, e->ws.tgt_lo);
   }
+  PhaseTimer pt(e, PH_LOGITS, st);
+  float* S = wsp<float>(e, e->ws.S);
+  float* S_lo = X3 ? wsp<float>(e, e->ws.S_lo) : nullptr;
+  const size_t ld = e->ws.ldS;
+  const umma::EpiStoreLseT<X3> lse{S, ld, wsp<float2>(e, e->ws.lse_part), umma::lse_slots(Y)};
+  auto go = [&](auto ep) -> int {
+    C2V_LAUNCH(e, C2V_CUDA(e, (umma::launch_cfg<false, false, decltype(ep)>(st, B, Y, D, 1, opA, opB, ep, e->num_sms))));
+    return C2V_OK;
+  };
+  switch (out) {
+    case LOGITS_STORE: return go(umma::EpiStore{S, ld, 0});
+    case LOGITS_STORE_LSE: return go(lse);
+    case LOGITS_LSE_ONLY: return go(umma::EpiLseOnlyT<X3>{lse});
+    case LOGITS_SOFTMAX_GRAD:
+      return go(umma::EpiSoftmaxGradT<X3, X3>{S, S_lo, ld, a.sg.lse, a.sg.target, a.sg.row0, a.sg.inv_batch, B});
+    case LOGITS_EXP_SUM: return go(umma::EpiExpSumT<X3, X3>{S, S_lo, ld, a.exp_offset, lse.partial, lse.slots});
+    case LOGITS_STORE_LSE_GATED: return go(umma::EpiStoreLseGatedT<X3>{lse, a.gate});
+  }
+  return C2V_OK;
+}
+
+int run_logits(c2v_engine* e, cudaStream_t st, const float* v, int B, LogitsOut out, const LogitsArgs& a = {}) {
+  { int rcl = end_target_lazy(e, st); if (rcl) return rcl; }      // a pass over the whole table needs every row current
+  if (is_tc(e) && aligned16(v)) return is_3x(e) ? launch_logits<true>(e, st, v, B, out, a) : launch_logits<false>(e, st, v, B, out, a);
+  const int D = e->dims.code_dim;
   PhaseTimer pt(e, PH_LOGITS, st);
   simt::RowsK al{v, (size_t)D};
   simt::RowsK bl{e->theta.tgt, (size_t)D};
-  simt::StoreC ep{S, e->ws.ldS, 0};
-  C2V_LAUNCH(e, C2V_CUDA(e, simt::launch(st, B, Y, D, 1, al, bl, ep)));
+  simt::StoreC ep{wsp<float>(e, e->ws.S), e->ws.ldS, 0};
+  C2V_LAUNCH(e, C2V_CUDA(e, simt::launch(st, B, e->dims.target_vocab, D, 1, al, bl, ep)));
   return C2V_OK;
 }
 
@@ -728,7 +768,7 @@ int forward_impl(c2v_engine* e, cudaStream_t st, const int32_t* src, const int32
 int topk_impl(c2v_engine* e, cudaStream_t st, const float* code_vec, int B, int32_t* idx, float* val, int normalize) {
   if (normalize < 0 || normalize > 2) return fail(e, C2V_ERR_INVALID, "normalize must be 0 (logits), 1 (softmax over k) or 2 (full softmax)");
   float* S = wsp<float>(e, e->ws.S);
-  int rc = run_logits(e, st, code_vec, B, S);
+  int rc = run_logits(e, st, code_vec, B, LOGITS_STORE);
   if (rc) return rc;
   const int Y = e->dims.target_vocab;
   const int k = e->dims.top_k < Y ? e->dims.top_k : Y;
@@ -741,10 +781,18 @@ int topk_impl(c2v_engine* e, cudaStream_t st, const float* code_vec, int B, int3
   return C2V_OK;
 }
 
+int run_dy(c2v_engine* e, cudaStream_t st, const float* v, int B, const SlabDesc& slab);
+
+// the dY product target_grad_gemms deferred, if any
+int run_pending_dy(c2v_engine* e, cudaStream_t st) {
+  if (!e->pending_dy.v) return C2V_OK;
+  const PendingDy p = e->pending_dy;
+  e->pending_dy = PendingDy{};
+  return run_dy(e, st, p.v, p.B, p.slab);
+}
+
 // Backward of everything below the code vector, given dv: gradients of a, W and the two
 // embedding tables (SURVEY A.2).
-int run_dy(c2v_engine* e, cudaStream_t st, const float* v, int B);
-
 int context_backward(c2v_engine* e, cudaStream_t st, const ContextSource& cs, const float* mask, int B,
                      const Dropout& dp, const float* dv) {
   const int D = e->dims.code_dim, d = e->dims.embed_dim, K3 = 3 * d, N = cs.rows;
@@ -753,11 +801,7 @@ int context_backward(c2v_engine* e, cudaStream_t st, const ContextSource& cs, co
   float* da_part = wsp<float>(e, e->ws.da_part);
   float* part = wsp<float>(e, e->ws.part);
   int rc;
-  if (e->pending_dy_v && !is_tc(e)) {   // fp32 path: nothing to overlap with, run it first
-    const float* pv = e->pending_dy_v;
-    e->pending_dy_v = nullptr;
-    if ((rc = run_dy(e, st, pv, e->pending_dy_B))) return rc;
-  }
+  if (!is_tc(e) && (rc = run_pending_dy(e, st))) return rc;     // fp32 path: nothing to overlap with, run it first
   const bool x3 = is_tc(e) && is_3x(e);
   float* H_lo = x3 ? wsp<float>(e, e->ws.H_lo) : nullptr;
   rc = launch_attn_bwd(e, st, H, alpha, dv, wsp<float>(e, e->ws.v), B, da_part, H_lo);    // H now holds dU (3xTF32: its high parts, H_lo the rest)
@@ -773,7 +817,7 @@ int context_backward(c2v_engine* e, cudaStream_t st, const ContextSource& cs, co
       umma::Operand opA{H, (size_t)D, false, H_lo};
       umma::Operand opB{x3 ? wsp<float>(e, e->ws.W_hi) : e->theta.W, (size_t)D, false, x3 ? wsp<float>(e, e->ws.W_lo) : nullptr};
       umma::EpiStore ep{dXg, (size_t)K3, 0};
-      C2V_LAUNCH(e, C2V_CUDA(e, (C2V_UMMA(st, N, K3, D, 1, opA, opB, ep, e->num_sms))));
+      C2V_LAUNCH(e, C2V_CUDA(e, (umma::launch(st, N, K3, D, 1, opA, opB, ep, e->num_sms))));
     }
     if (e->lazy) {
       if (e->lazy_grads_pending)
@@ -811,18 +855,14 @@ int context_backward(c2v_engine* e, cudaStream_t st, const ContextSource& cs, co
     }
     if ((rc = early_catchup(e, e->side))) return rc;
     C2V_CUDA(e, cudaEventRecord(e->ev_join, e->side));
-    if (e->pending_dy_v) {   // deferred dYtab = P^T . v, concurrent with the scatter-add
-      const float* pv = e->pending_dy_v;
-      e->pending_dy_v = nullptr;
-      if ((rc = run_dy(e, st, pv, e->pending_dy_B))) return rc;
-    }
+    if ((rc = run_pending_dy(e, st))) return rc;     // concurrent with the scatter-add
     {  // dW = X'^T . dU on the gathered X' kept from the forward pass
       PhaseTimer pt(e, PH_DW, st);
       umma::Operand opA{Xg, (size_t)K3, true, x3 ? wsp<float>(e, e->ws.Xg_lo) : nullptr};
       umma::Operand opB{H, (size_t)D, true, H_lo};
       const int ks = umma::effective_splits(N, kSplitDw);
       umma::EpiStore ep{part, (size_t)D, (size_t)K3 * D};
-      C2V_LAUNCH(e, C2V_CUDA(e, (C2V_UMMA(st, K3, D, N, kSplitDw, opA, opB, ep, e->num_sms))));
+      C2V_LAUNCH(e, C2V_CUDA(e, (umma::launch(st, K3, D, N, kSplitDw, opA, opB, ep, e->num_sms))));
       rc = launch_colsum(e, st, part, (size_t)K3 * D, ks, K3 * D, e->grad.W);
       if (rc) return rc;
     }
@@ -863,8 +903,8 @@ int context_backward(c2v_engine* e, cudaStream_t st, const ContextSource& cs, co
   return C2V_OK;
 }
 
-// Given P = dL/dlogits in the S slab:  dv = P . Ytab  (split-K over |Y|, fixed-order reduction).
-int run_dv(c2v_engine* e, cudaStream_t st, int B, float* dv) {
+// Given P = dL/dlogits in the S slab (as `slab` describes it):  dv = P . Ytab  (split-K over |Y|, fixed-order reduction).
+int run_dv(c2v_engine* e, cudaStream_t st, int B, float* dv, const SlabDesc& slab) {
   const int D = e->dims.code_dim, Y = e->dims.target_vocab;
   float* S = wsp<float>(e, e->ws.S);
   float* part = wsp<float>(e, e->ws.part);
@@ -887,14 +927,14 @@ int run_dv(c2v_engine* e, cudaStream_t st, int B, float* dv) {
     if (want > kSplitDv) want = kSplitDv;
     const int ks = umma::effective_splits(Y, want);
     umma::EpiStore ep{part, (size_t)D, (size_t)B * D};
-    if (e->sg_live) {       // A = the logits slab, turned into dL/dlogits by the GEMM's loaders
-      umma::AXSoftmaxGrad<true> ax{e->sg};
+    if (slab.loaders) {       // A = the logits slab, turned into dL/dlogits by the GEMM's loaders
+      umma::AXSoftmaxGrad<true> ax{slab.sg};
       C2V_LAUNCH(e, C2V_CUDA(e, (umma::launch_cfg<false, true, umma::EpiStore, umma::AXSoftmaxGrad<true>>(st, B, D, Y, want, opA, opB, ep,
                                                                                                             e->num_sms, ax))));
     } else {
-      C2V_LAUNCH(e, C2V_CUDA(e, (C2V_UMMA(st, B, D, Y, want, opA, opB, ep, e->num_sms))));
+      C2V_LAUNCH(e, C2V_CUDA(e, (umma::launch(st, B, D, Y, want, opA, opB, ep, e->num_sms))));
     }
-    return launch_colsum(e, st, part, (size_t)B * D, ks, B * D, dv, e->row_scale, D);
+    return launch_colsum(e, st, part, (size_t)B * D, ks, B * D, dv, slab.row_scale, D);
   }
   simt::RowsK al{S, e->ws.ldS};
   simt::ColsX bl{e->theta.tgt, (size_t)D};
@@ -905,14 +945,14 @@ int run_dv(c2v_engine* e, cudaStream_t st, int B, float* dv) {
 }
 
 // dYtab = P^T . v  into the bound target-table gradient; then the caller's "target_grads_ready" event.
-int run_dy(c2v_engine* e, cudaStream_t st, const float* v, int B) {
+int run_dy(c2v_engine* e, cudaStream_t st, const float* v, int B, const SlabDesc& slab) {
   const int D = e->dims.code_dim, Y = e->dims.target_vocab;
   float* S = wsp<float>(e, e->ws.S);
   {
     PhaseTimer pt(e, PH_DY, st);
-    if (is_3x(e) && (reinterpret_cast<uintptr_t>(v) % 16 != 0))
+    if (is_3x(e) && !aligned16(v))
       return fail(e, C2V_ERR_INVALID, "3xTF32: the code vectors must be 16-byte aligned");
-    if (is_tc(e) && (reinterpret_cast<uintptr_t>(v) % 16 == 0)) {
+    if (is_tc(e) && aligned16(v)) {
       umma::Operand opA{S, e->ws.ldS, true};
       umma::Operand opB{v, (size_t)D, true};
       if (is_3x(e)) {
@@ -921,31 +961,27 @@ int run_dy(c2v_engine* e, cudaStream_t st, const float* v, int B) {
         opA.lo = wsp<float>(e, e->ws.S_lo);
         opB.base = wsp<float>(e, e->ws.v_hi); opB.lo = wsp<float>(e, e->ws.v_lo);
       }
+      auto go = [&](auto ep) -> int {
+        if (slab.loaders)       // A = the logits slab, turned into dL/dlogits by the GEMM's loaders
+          C2V_LAUNCH(e, C2V_CUDA(e, (umma::launch_cfg<true, true, decltype(ep), umma::AXSoftmaxGrad<false>>(
+                                        st, Y, D, B, 1, opA, opB, ep, e->num_sms, umma::AXSoftmaxGrad<false>{slab.sg}))));
+        else
+          C2V_LAUNCH(e, C2V_CUDA(e, (umma::launch_cfg<true, true, decltype(ep)>(st, Y, D, B, 1, opA, opB, ep, e->num_sms))));
+        return C2V_OK;
+      };
+      int rc;
       if (e->tgt_armed && e->has_adam) {
         // dYtab never reaches memory: the epilogue applies TF1 Adam to the target table in place
         const double lr_t = (double)e->tgt_lr * sqrt(1.0 - pow((double)e->tgt_b2, (double)e->tgt_t)) /
                             (1.0 - pow((double)e->tgt_b1, (double)e->tgt_t));
-        umma::EpiAdam ep{e->theta.tgt, e->am.tgt, e->av.tgt, (size_t)D, (float)lr_t, e->tgt_b1, e->tgt_b2, e->tgt_eps,
-                         1.f - e->tgt_b1, 1.f - e->tgt_b2, e->adam_epi_prefetch};
-        if (e->sg_live) {
-          umma::AXSoftmaxGrad<false> ax{e->sg};
-          C2V_LAUNCH(e, C2V_CUDA(e, (umma::launch_cfg<true, true, umma::EpiAdam, umma::AXSoftmaxGrad<false>>(st, Y, D, B, 1, opA, opB, ep,
-                                                                                                               e->num_sms, ax))));
-        } else {
-          C2V_LAUNCH(e, C2V_CUDA(e, (C2V_UMMA_FIXED(true, true, umma::EpiAdam, st, Y, D, B, 1, opA, opB, ep, e->num_sms))));
-        }
+        if ((rc = go(umma::EpiAdam{e->theta.tgt, e->am.tgt, e->av.tgt, (size_t)D, (float)lr_t, e->tgt_b1, e->tgt_b2, e->tgt_eps,
+                                   1.f - e->tgt_b1, 1.f - e->tgt_b2, e->adam_epi_prefetch})))
+          return rc;
         e->tgt_armed = false;
         e->tgt_fused_t = e->tgt_t;
         e->tgt_split_valid = false;
-      } else {
-        umma::EpiStore ep{e->grad.tgt, (size_t)D, 0};
-        if (e->sg_live) {
-          umma::AXSoftmaxGrad<false> ax{e->sg};
-          C2V_LAUNCH(e, C2V_CUDA(e, (umma::launch_cfg<true, true, umma::EpiStore, umma::AXSoftmaxGrad<false>>(st, Y, D, B, 1, opA, opB, ep,
-                                                                                                                e->num_sms, ax))));
-        } else {
-          C2V_LAUNCH(e, C2V_CUDA(e, (C2V_UMMA(st, Y, D, B, 1, opA, opB, ep, e->num_sms))));
-        }
+      } else if ((rc = go(umma::EpiStore{e->grad.tgt, (size_t)D, 0}))) {
+        return rc;
       }
     } else {
       simt::ColsX al{S, e->ws.ldS};
@@ -961,25 +997,90 @@ int run_dy(c2v_engine* e, cudaStream_t st, const float* v, int B) {
 // The two target-table gradient products.  With option "dy_late" (default) only dv runs here and dY is
 // deferred into context_backward, where it overlaps the NVLink / L2-atomic bound scatter-add of the
 // embedding gradients (dY needs P and v only, not the context backward).
-int target_grad_gemms(c2v_engine* e, cudaStream_t st, const float* v, int B, float* dv) {
-  int rc = run_dv(e, st, B, dv);
+int target_grad_gemms(c2v_engine* e, cudaStream_t st, const float* v, int B, float* dv, const SlabDesc& slab) {
+  int rc = run_dv(e, st, B, dv, slab);
   if (rc) return rc;
   if (e->dy_late == 2 && is_tc(e)) {
     // dY (and the target table's Adam step in its epilogue) is HBM-bound and independent of the context
     // backward pass: it runs on its own stream from here until context_backward joins it
     C2V_CUDA(e, cudaEventRecord(e->ev_fork2, st));
     C2V_CUDA(e, cudaStreamWaitEvent(e->side2, e->ev_fork2, 0));
-    if ((rc = run_dy(e, e->side2, v, B))) return rc;
+    if ((rc = run_dy(e, e->side2, v, B, slab))) return rc;
     C2V_CUDA(e, cudaEventRecord(e->ev_join2, e->side2));
     e->dy_in_flight = true;
     return C2V_OK;
   }
   if (e->dy_late) {
-    e->pending_dy_v = v;
-    e->pending_dy_B = B;
+    e->pending_dy = PendingDy{v, B, slab};
     return C2V_OK;
   }
-  return run_dy(e, st, v, B);
+  return run_dy(e, st, v, B, slab);
+}
+
+// Turns the slab into P = dL/dlogits = (softmax - onehot) * inv_batch for the dv / dY GEMMs, inside the caller's PH_XENT
+// timer; returns in `slab` how they read it, and in `v_dy` the code vectors dY multiplies.  Two-pass: softmax_grad_kernel
+// rewrites the logits (3xTF32: as P's split).  Loaders: nothing runs here, the GEMMs' A loaders do it.  exp_slab: the slab
+// holds U, already patched; the same rewrite runs gated, for rows that left the fp32 window only (reset_factors: it also
+// sets their factors to 1 and counts the fallback), and dY gets the code vectors scaled by the rows' factors.
+int slab_to_p(c2v_engine* e, cudaStream_t st, HeadSchedule hs, const float* v, int B, const umma::SoftmaxGradArgs& g,
+              SlabDesc* slab, const float** v_dy, bool reset_factors = false) {
+  *v_dy = v;
+  if (hs == HEAD_LOADERS) {
+    slab->loaders = true;
+    slab->sg = g;
+    return C2V_OK;
+  }
+  float* S = wsp<float>(e, e->ws.S);
+  const int Y = e->dims.target_vocab, D = e->dims.code_dim;
+  const bool gated = hs == HEAD_EXP_SLAB;
+  const int* gate = gated ? wsp<int>(e, e->ws.slab_flag) : nullptr;
+  float* rscale = wsp<float>(e, e->ws.rscale);
+  float* reset = gated && reset_factors ? rscale : nullptr;
+  unsigned* count = reset ? reinterpret_cast<unsigned*>(wsp<int>(e, e->ws.slab_flag)) + 1 : nullptr;
+  // the fallback only has to be correct; a small grid keeps the closed gate cheap
+  const int chunks = gated ? 2 : (int)((e->ws.ldS / 4 + 256 * 8 - 1) / (256 * 8));
+  if (is_3x(e))
+    C2V_LAUNCH(e, (softmax_grad_kernel<true><<<dim3(chunks, B), 256, 0, st>>>(S, e->ws.ldS, Y, g.lse, g.target, g.inv_batch, g.row0,
+                                                                             wsp<float>(e, e->ws.S_lo), gate, reset, count)));
+  else
+    C2V_LAUNCH(e, (softmax_grad_kernel<false><<<dim3(chunks, B), 256, 0, st>>>(S, e->ws.ldS, Y, g.lse, g.target, g.inv_batch, g.row0,
+                                                                              nullptr, gate, reset, count)));
+  if (gated) {
+    float* vs = wsp<float>(e, e->ws.v_scaled);
+    C2V_LAUNCH(e, (scale_rows_kernel<<<(unsigned)(((size_t)B * D + 255) / 256), 256, 0, st>>>(v, rscale, vs, D, (size_t)B * D)));
+    slab->row_scale = rscale;
+    *v_dy = vs;
+  }
+  return C2V_OK;
+}
+
+// exp_slab schedule (DESIGN.md section 4.9), up to the loss statistics: each row's true-class logit in fp32 (ws.true_logit,
+// also copied to tl_out when given), the logits pass that writes U = exp(s - true logit) with (max U, sum U) partials, the
+// caller's combine of those partials (it raises the range flag for rows that left the fp32 window), and the gated
+// two-pass logits the device runs only for such rows.
+template <class Combine>
+int exp_slab_logits(c2v_engine* e, cudaStream_t st, const float* v, int B, const int32_t* target, int row0, float* tl_out,
+                    Combine combine) {
+  float* tl = wsp<float>(e, e->ws.true_logit);
+  int* flag = wsp<int>(e, e->ws.slab_flag);
+  if (!e->slab_flag_zeroed) {
+    C2V_CUDA(e, cudaMemsetAsync(flag, 0, 64, st));
+    e->slab_flag_zeroed = true;
+  }
+  int rc;
+  if ((rc = end_target_lazy(e, st))) return rc;      // the true-class rows are read below: every target row must be current
+  {
+    PhaseTimer pt(e, PH_XENT, st);
+    C2V_LAUNCH(e, (true_logit_kernel<<<(B + 7) / 8, 256, 0, st>>>(v, e->theta.tgt, target, row0, e->dims.target_vocab, e->dims.code_dim,
+                                                                  B, tl, flag)));
+    if (tl_out) C2V_CUDA(e, cudaMemcpyAsync(tl_out, tl, (size_t)B * 4, cudaMemcpyDeviceToDevice, st));
+  }
+  if ((rc = run_logits(e, st, v, B, LOGITS_EXP_SUM, LogitsArgs{tl}))) return rc;
+  {
+    PhaseTimer pt(e, PH_XENT, st);
+    if ((rc = combine())) return rc;
+  }
+  return run_logits(e, st, v, B, LOGITS_STORE_LSE_GATED, LogitsArgs{nullptr, flag});
 }
 
 int train_step_impl(c2v_engine* e, cudaStream_t st, const int32_t* src, const int32_t* pth, const int32_t* tgt,
@@ -997,95 +1098,60 @@ int train_step_impl(c2v_engine* e, cudaStream_t st, const int32_t* src, const in
   float* S = wsp<float>(e, e->ws.S);
   float* loss_b = wsp<float>(e, e->ws.loss_b);
   float* lse = wsp<float>(e, e->ws.lse);
+  float2* part = wsp<float2>(e, e->ws.lse_part);
+  const int n_tiles = umma::lse_slots(Y);       // partial slots per row
   int rc;
   if ((rc = run_ctx_fwd(e, st, cs, dp, H, true))) return rc;
   if ((rc = launch_attn_fwd(e, st, H, mask, B, alpha, v))) return rc;
-  const bool fused_lse = (is_tc(e));
   const float invB = 1.0f / (float)B;
-  if (fused_lse && e->recompute && !e->fuse_sg) {
+  const umma::SoftmaxGradArgs g{lse, target, 0, invB};
+  const HeadSchedule hs = head_schedule(e, API_STEP, v);
+  const float* v_dy = v;
+  SlabDesc slab;
+  if (hs == HEAD_RECOMPUTE) {
     // the slab is written ONCE, as dL/dlogits: pass 1 of the logits GEMM leaves only log-sum-exp partials, the true-class
     // logit comes from a B-row dot product, pass 2 repeats the product and its epilogue writes (softmax - onehot) / B
-    if ((rc = run_logits(e, st, v, B, S, false, true))) return rc;
+    if ((rc = run_logits(e, st, v, B, LOGITS_LSE_ONLY))) return rc;
     float* tl = wsp<float>(e, e->ws.true_logit);
     {
       PhaseTimer pt(e, PH_XENT, st);
       C2V_LAUNCH(e, (true_logit_kernel<<<(B + 7) / 8, 256, 0, st>>>(v, e->theta.tgt, target, 0, Y, e->dims.code_dim, B, tl)));
-      C2V_LAUNCH(e, (xent_combine_kernel<<<B, 256, 0, st>>>(wsp<float2>(e, e->ws.lse_part), umma::lse_slots(Y), S, e->ws.ldS, target,
-                                                            loss_b, lse, tl)));
+      C2V_LAUNCH(e, (xent_combine_kernel<<<B, 256, 0, st>>>(part, n_tiles, S, e->ws.ldS, target, loss_b, lse, tl)));
       C2V_LAUNCH(e, (loss_reduce_kernel<<<1, 256, 0, st>>>(loss_b, B, invB, loss_out)));
     }
-    e->sg_live = false;
-    const LogitsGrad lg{lse, target, 0, invB};
-    if ((rc = run_logits(e, st, v, B, S, false, false, &lg))) return rc;
-    if ((rc = target_grad_gemms(e, st, v, B, dv))) return rc;
-    return context_backward(e, st, cs, mask, B, dp, dv);
-  }
-  if (fused_lse && e->exp_slab && !e->fuse_sg) {
+    if ((rc = run_logits(e, st, v, B, LOGITS_SOFTMAX_GRAD, LogitsArgs{nullptr, nullptr, g}))) return rc;
+  } else if (hs == HEAD_EXP_SLAB) {
     // deferred normalisation: U = exp(s - true logit) from the logits epilogue, one patched element and one factor per row;
     // the gated kernels after the combine are the two-pass schedule, run by the device only when a row left the fp32 window
-    const int D = e->dims.code_dim;
-    const int n_tiles = umma::lse_slots(Y);
     float* tl = wsp<float>(e, e->ws.true_logit);
     float* rscale = wsp<float>(e, e->ws.rscale);
-    float* vs = wsp<float>(e, e->ws.v_scaled);
     int* flag = wsp<int>(e, e->ws.slab_flag);
     float* S_lo = is_3x(e) ? wsp<float>(e, e->ws.S_lo) : nullptr;
-    if (!e->slab_flag_zeroed) {
-      C2V_CUDA(e, cudaMemsetAsync(flag, 0, 64, st));
-      e->slab_flag_zeroed = true;
-    }
-    if ((rc = end_target_lazy(e, st))) return rc;      // the true-class rows are read below: every target row must be current
+    rc = exp_slab_logits(e, st, v, B, target, 0, nullptr, [&]() -> int {
+      C2V_LAUNCH(e, (expsum_combine_kernel<<<B, 256, 0, st>>>(part, n_tiles, S, S_lo, e->ws.ldS, Y, target, tl, tl, invB, loss_b, lse,
+                                                              rscale, flag)));
+      return C2V_OK;
+    });
+    if (rc) return rc;
     {
       PhaseTimer pt(e, PH_XENT, st);
-      C2V_LAUNCH(e, (true_logit_kernel<<<(B + 7) / 8, 256, 0, st>>>(v, e->theta.tgt, target, 0, Y, D, B, tl, flag)));
-    }
-    if ((rc = run_logits(e, st, v, B, S, false, false, nullptr, tl))) return rc;
-    {
-      PhaseTimer pt(e, PH_XENT, st);
-      C2V_LAUNCH(e, (expsum_combine_kernel<<<B, 256, 0, st>>>(wsp<float2>(e, e->ws.lse_part), n_tiles, S, S_lo, e->ws.ldS, Y, target, tl, tl, invB,
-                                                              loss_b, lse, rscale, flag)));
-    }
-    if ((rc = run_logits(e, st, v, B, S, true, false, nullptr, nullptr, flag))) return rc;
-    {
-      PhaseTimer pt(e, PH_XENT, st);
-      C2V_LAUNCH(e, (xent_combine_kernel<<<B, 256, 0, st>>>(wsp<float2>(e, e->ws.lse_part), n_tiles, S, e->ws.ldS, target, loss_b, lse, nullptr, flag,
-                                                            rscale, reinterpret_cast<unsigned*>(flag) + 1)));
-      const int chunks = 2;        // the fallback only has to be correct; a small grid keeps the closed gate cheap
-      if (S_lo) C2V_LAUNCH(e, (softmax_grad_kernel<true><<<dim3(chunks, B), 256, 0, st>>>(S, e->ws.ldS, Y, lse, target, invB, 0, S_lo, flag)));
-      else C2V_LAUNCH(e, (softmax_grad_kernel<false><<<dim3(chunks, B), 256, 0, st>>>(S, e->ws.ldS, Y, lse, target, invB, 0, nullptr, flag)));
-      C2V_LAUNCH(e, (scale_rows_kernel<<<(unsigned)(((size_t)B * D + 255) / 256), 256, 0, st>>>(v, rscale, vs, D, (size_t)B * D)));
+      C2V_LAUNCH(e, (xent_combine_kernel<<<B, 256, 0, st>>>(part, n_tiles, S, e->ws.ldS, target, loss_b, lse, nullptr, flag, rscale,
+                                                            reinterpret_cast<unsigned*>(flag) + 1)));
+      if ((rc = slab_to_p(e, st, hs, v, B, g, &slab, &v_dy))) return rc;
       C2V_LAUNCH(e, (loss_reduce_kernel<<<1, 256, 0, st>>>(loss_b, B, invB, loss_out)));
     }
-    e->sg_live = false;
-    e->row_scale = rscale;
-    rc = target_grad_gemms(e, st, vs, B, dv);
-    e->row_scale = nullptr;
-    if (rc) return rc;
-    return context_backward(e, st, cs, mask, B, dp, dv);
-  }
-  if ((rc = run_logits(e, st, v, B, S, fused_lse))) return rc;
-  {
+  } else {
+    if ((rc = run_logits(e, st, v, B, hs == HEAD_SIMT ? LOGITS_STORE : LOGITS_STORE_LSE))) return rc;
     PhaseTimer pt(e, PH_XENT, st);
-    if (fused_lse) {
-      const int n_tiles = umma::lse_slots(Y);       // partial slots per row
-      C2V_LAUNCH(e, (xent_combine_kernel<<<B, 256, 0, st>>>(wsp<float2>(e, e->ws.lse_part), n_tiles, S, e->ws.ldS, target,
-                                                            loss_b, lse)));
-      const int chunks = (int)((e->ws.ldS / 4 + 256 * 8 - 1) / (256 * 8));
-      e->sg_live = false;
-      if (is_3x(e))
-        C2V_LAUNCH(e, (softmax_grad_kernel<true><<<dim3(chunks, B), 256, 0, st>>>(S, e->ws.ldS, Y, lse, target, invB, 0, wsp<float>(e, e->ws.S_lo))));
-      else if (e->fuse_sg) {
-        // no pass over the slab: the dv and dY GEMMs turn logits into (softmax - onehot) / B as their A tiles land
-        e->sg = umma::SoftmaxGradArgs{lse, target, 0, invB};
-        e->sg_live = true;
-      } else
-        C2V_LAUNCH(e, (softmax_grad_kernel<false><<<dim3(chunks, B), 256, 0, st>>>(S, e->ws.ldS, Y, lse, target, invB, 0, nullptr)));
-    } else {
+    if (hs == HEAD_SIMT) {
       C2V_LAUNCH(e, (xent_kernel<<<B, kXentThreads, 0, st>>>(S, e->ws.ldS, target, Y, invB, loss_b, lse, 1)));
+    } else {
+      C2V_LAUNCH(e, (xent_combine_kernel<<<B, 256, 0, st>>>(part, n_tiles, S, e->ws.ldS, target, loss_b, lse)));
+      if ((rc = slab_to_p(e, st, hs, v, B, g, &slab, &v_dy))) return rc;
     }
     C2V_LAUNCH(e, (loss_reduce_kernel<<<1, 256, 0, st>>>(loss_b, B, invB, loss_out)));
   }
-  if ((rc = target_grad_gemms(e, st, v, B, dv))) return rc;
+  if ((rc = target_grad_gemms(e, st, v_dy, B, dv, slab))) return rc;
   return context_backward(e, st, cs, mask, B, dp, dv);
 }
 
@@ -1504,8 +1570,8 @@ int c2v_loss(c2v_engine* e, const float* code_vec, const int32_t* target, int32_
   float* S = wsp<float>(e, e->ws.S);
   const float invB = 1.0f / (float)B;
   const int Y = e->dims.target_vocab;
-  const bool fused = is_tc(e) && (reinterpret_cast<uintptr_t>(code_vec) % 16 == 0);
-  if ((rc = run_logits(e, st, code_vec, B, S, fused))) return rc;
+  const bool fused = head_schedule(e, API_LOSS, code_vec) == HEAD_TWO_PASS;
+  if ((rc = run_logits(e, st, code_vec, B, fused ? LOGITS_STORE_LSE : LOGITS_STORE))) return rc;
   {
     PhaseTimer pt(e, PH_XENT, st);
     if (fused)      // the logits epilogue already folded each tile into (max, sum exp) partials
@@ -1701,42 +1767,30 @@ int c2v_target_forward(c2v_engine* e, const float* code_all, int32_t Bt, const i
   cudaStream_t st = (cudaStream_t)stream;
   float* S = wsp<float>(e, e->ws.S);
   const int Y = e->dims.target_vocab;
-  const bool fused = (is_tc(e)) && (reinterpret_cast<uintptr_t>(code_all) % 16 == 0);
   const int n_tiles = umma::lse_slots(Y);
-  e->slab_exp_live = false;
-  if (fused && e->exp_slab && !e->fuse_sg && e->has_grad) {
-    // deferred normalisation over a row-sharded table: (c_b, sum U) stand in for (row max, sum exp) in the cross-rank combine
+  float2* part = wsp<float2>(e, e->ws.lse_part);
+  const HeadSchedule hs = head_schedule(e, API_TARGET_FORWARD, code_all);
+  e->split_fwd = hs;
+  if (hs == HEAD_EXP_SLAB) {
+    // deferred normalisation over a row-sharded table: (c_b, sum U) stand in for (row max, sum exp) in the cross-rank combine;
+    // a row that left the fp32 window has the statistics that go to the other ranks redone the classic way
     float* tl = wsp<float>(e, e->ws.true_logit);
     int* flag = wsp<int>(e, e->ws.slab_flag);
-    if (!e->slab_flag_zeroed) {
-      C2V_CUDA(e, cudaMemsetAsync(flag, 0, 64, st));
-      e->slab_flag_zeroed = true;
-    }
-    if ((rc = end_target_lazy(e, st))) return rc;
-    {
-      PhaseTimer pt(e, PH_XENT, st);
-      C2V_LAUNCH(e, (true_logit_kernel<<<(Bt + 7) / 8, 256, 0, st>>>(code_all, e->theta.tgt, target, row_offset, Y, e->dims.code_dim, Bt, tl, flag)));
-      C2V_CUDA(e, cudaMemcpyAsync(true_logit, tl, (size_t)Bt * 4, cudaMemcpyDeviceToDevice, st));
-    }
-    if ((rc = run_logits(e, st, code_all, Bt, S, false, false, nullptr, tl))) return rc;
-    {
-      PhaseTimer pt(e, PH_XENT, st);
-      C2V_LAUNCH(e, (expsum_rows_kernel<<<Bt, 256, 0, st>>>(wsp<float2>(e, e->ws.lse_part), n_tiles, tl, row_max, row_sum, flag)));
-    }
-    // a row left the fp32 window: the statistics that go to the other ranks are redone the classic way (gated, usually a no-op)
-    if ((rc = run_logits(e, st, code_all, Bt, S, true, false, nullptr, nullptr, flag))) return rc;
-    {
-      PhaseTimer pt(e, PH_XENT, st);
-      C2V_LAUNCH(e, (row_maxsum_kernel<<<Bt, 256, 0, st>>>(wsp<float2>(e, e->ws.lse_part), n_tiles, S, e->ws.ldS, Y, target, row_offset, row_max,
-                                                           row_sum, true_logit, 1, flag)));
-    }
-    e->slab_exp_live = true;
+    rc = exp_slab_logits(e, st, code_all, Bt, target, row_offset, true_logit, [&]() -> int {
+      C2V_LAUNCH(e, (expsum_rows_kernel<<<Bt, 256, 0, st>>>(part, n_tiles, tl, row_max, row_sum, flag)));
+      return C2V_OK;
+    });
+    if (rc) return rc;
+    PhaseTimer pt(e, PH_XENT, st);
+    C2V_LAUNCH(e, (row_maxsum_kernel<<<Bt, 256, 0, st>>>(part, n_tiles, S, e->ws.ldS, Y, target, row_offset, row_max, row_sum, true_logit,
+                                                         1, flag)));
     return C2V_OK;
   }
-  if ((rc = run_logits(e, st, code_all, Bt, S, fused))) return rc;
+  const bool fused = hs == HEAD_TWO_PASS;
+  if ((rc = run_logits(e, st, code_all, Bt, fused ? LOGITS_STORE_LSE : LOGITS_STORE))) return rc;
   PhaseTimer pt(e, PH_XENT, st);
-  C2V_LAUNCH(e, (row_maxsum_kernel<<<Bt, 256, 0, st>>>(fused ? wsp<float2>(e, e->ws.lse_part) : nullptr, n_tiles, S, e->ws.ldS, Y, target,
-                                                       row_offset, row_max, row_sum, true_logit)));
+  C2V_LAUNCH(e, (row_maxsum_kernel<<<Bt, 256, 0, st>>>(fused ? part : nullptr, n_tiles, S, e->ws.ldS, Y, target, row_offset, row_max,
+                                                       row_sum, true_logit)));
   return C2V_OK;
 }
 
@@ -1760,51 +1814,29 @@ int c2v_target_backward(c2v_engine* e, const float* code_all, int32_t Bt, const 
   if (!e->has_grad) return fail(e, C2V_ERR_STATE, "gradients not bound (c2v_bind_grads)");
   C2V_CUDA(e, cudaSetDevice(e->device));
   cudaStream_t st = (cudaStream_t)stream;
-  float* S = wsp<float>(e, e->ws.S);
-  if (e->slab_exp_live) {
-    // the slab holds U = exp(s - c_b): patch the true-class elements, hand the rows' factors to the two GEMMs
-    e->slab_exp_live = false;
-    e->sg_live = false;
-    const int Y = e->dims.target_vocab, D = e->dims.code_dim;
-    float* tl = wsp<float>(e, e->ws.true_logit);
-    float* rscale = wsp<float>(e, e->ws.rscale);
-    float* vs = wsp<float>(e, e->ws.v_scaled);
-    int* flag = wsp<int>(e, e->ws.slab_flag);
+  const HeadSchedule hs = head_schedule(e, API_TARGET_BACKWARD, code_all);
+  e->split_fwd = HEAD_SIMT;
+  const umma::SoftmaxGradArgs g{lse, target, row_offset, inv_batch};
+  SlabDesc slab;
+  if (hs == HEAD_EXP_SLAB) {
+    // the slab holds U = exp(s - c_b): patch the true-class elements and set the rows' factors; for a row that left the fp32
+    // window the logits are computed again (gated) and rewritten with the global log-sum-exp, and its factor becomes 1
     float* S_lo = is_3x(e) ? wsp<float>(e, e->ws.S_lo) : nullptr;
+    int* flag = wsp<int>(e, e->ws.slab_flag);
     {
       PhaseTimer pt(e, PH_XENT, st);
-      C2V_LAUNCH(e, (expsum_finish_kernel<<<(Bt + 255) / 256, 256, 0, st>>>(S, S_lo, e->ws.ldS, Y, target, row_offset, tl, lse, inv_batch, Bt, rscale, flag)));
+      C2V_LAUNCH(e, (expsum_finish_kernel<<<(Bt + 255) / 256, 256, 0, st>>>(wsp<float>(e, e->ws.S), S_lo, e->ws.ldS, e->dims.target_vocab,
+                                                                            target, row_offset, wsp<float>(e, e->ws.true_logit), lse,
+                                                                            inv_batch, Bt, wsp<float>(e, e->ws.rscale), flag)));
     }
-    // fallback (gated): logits again, then the classic rewrite with the global log-sum-exp; the rows' factors become 1
-    if ((rc = run_logits(e, st, code_all, Bt, S, true, false, nullptr, nullptr, flag))) return rc;
-    {
-      PhaseTimer pt(e, PH_XENT, st);
-      if (S_lo) C2V_LAUNCH(e, (softmax_grad_kernel<true><<<dim3(2, Bt), 256, 0, st>>>(S, e->ws.ldS, Y, lse, target, inv_batch, row_offset, S_lo, flag, rscale,
-                                                                                    reinterpret_cast<unsigned*>(flag) + 1)));
-      else C2V_LAUNCH(e, (softmax_grad_kernel<false><<<dim3(2, Bt), 256, 0, st>>>(S, e->ws.ldS, Y, lse, target, inv_batch, row_offset, nullptr, flag, rscale,
-                                                                                 reinterpret_cast<unsigned*>(flag) + 1)));
-      C2V_LAUNCH(e, (scale_rows_kernel<<<(unsigned)(((size_t)Bt * D + 255) / 256), 256, 0, st>>>(code_all, rscale, vs, D, (size_t)Bt * D)));
-    }
-    e->row_scale = rscale;
-    rc = target_grad_gemms(e, st, vs, Bt, dv_partial);
-    e->row_scale = nullptr;
-    return rc;
+    if ((rc = run_logits(e, st, code_all, Bt, LOGITS_STORE_LSE_GATED, LogitsArgs{nullptr, flag}))) return rc;
   }
+  const float* v_dy;
   {
     PhaseTimer pt(e, PH_XENT, st);
-    const int chunks = (int)((e->ws.ldS / 4 + 256 * 8 - 1) / (256 * 8));
-    e->sg_live = false;
-    if (is_3x(e))
-      C2V_LAUNCH(e, (softmax_grad_kernel<true><<<dim3(chunks, Bt), 256, 0, st>>>(S, e->ws.ldS, e->dims.target_vocab, lse, target, inv_batch,
-                                                                               row_offset, wsp<float>(e, e->ws.S_lo))));
-    else if (is_tc(e) && e->fuse_sg) {
-      e->sg = umma::SoftmaxGradArgs{lse, target, row_offset, inv_batch};
-      e->sg_live = true;
-    } else
-      C2V_LAUNCH(e, (softmax_grad_kernel<false><<<dim3(chunks, Bt), 256, 0, st>>>(S, e->ws.ldS, e->dims.target_vocab, lse, target, inv_batch,
-                                                                                row_offset, nullptr)));
+    if ((rc = slab_to_p(e, st, hs, code_all, Bt, g, &slab, &v_dy, true))) return rc;
   }
-  return target_grad_gemms(e, st, code_all, Bt, dv_partial);
+  return target_grad_gemms(e, st, v_dy, Bt, dv_partial, slab);
 }
 
 int c2v_context_backward(c2v_engine* e, const int32_t* src, const int32_t* path, const int32_t* tgt, const float* mask,
@@ -1968,7 +2000,7 @@ int c2v_selftest_gemm3(c2v_engine* e, int32_t a_mn, int32_t b_mn, int32_t bn, in
   if (!umma::operand_ok(opA) || !umma::operand_ok(opB)) return fail(e, C2V_ERR_INVALID, "operand not TMA-compatible");
   umma::EpiStore ep{C, ldc, (size_t)M * ldc};
   if (bn != 192 && bn != 256) return fail(e, C2V_ERR_INVALID, "bn must be 192 or 256");
-  C2V_LAUNCH(e, C2V_CUDA(e, (C2V_UMMA(st, M, N, K, splits, opA, opB, ep, e->num_sms))));
+  C2V_LAUNCH(e, C2V_CUDA(e, (umma::launch(st, M, N, K, splits, opA, opB, ep, e->num_sms))));
   return umma::effective_splits(K, splits);
 }
 
