@@ -2,18 +2,21 @@
 // mantissa), fp32 accumulation in registers  (C2V_MATH_TF32; C2V_MATH_3XTF32 issues three products).
 //
 // Persistent, warp-specialised, one CTA of three warpgroups per SM:
-//   warpgroup 0     : producer -- fills a 4-stage shared-memory ring.  K-major operands arrive by TMA
-//                     (cp.async.bulk.tensor, 128-byte swizzle, issued by one thread); MN-major operands are
-//                     loaded by all 128 threads and transposed on the way into shared memory, because
-//                     wgmma takes 32-bit (tf32) operands K-major only.  An A-operand policy (AX*) may
-//                     instead compute the A tile (softmax gradient of a logits tile, embedding gather).
+//   warpgroup 0     : producer -- fills a 4-stage shared-memory ring.  Operands arrive by TMA
+//                     (cp.async.bulk.tensor, 128-byte swizzle, issued by one thread).  wgmma takes 32-bit
+//                     (tf32) operands K-major only, so an MN-major operand lands as four 32 x 32 boxes that
+//                     the four producer warps then transpose in place (transpose_box); the loads of the next
+//                     steps stay in flight meanwhile.  An A-operand policy (AX*) may instead compute the A
+//                     tile (softmax gradient of a logits tile, embedding gather).
 //   warpgroups 1, 2 : consumers -- each owns 64 rows of the 128-row tile and issues
 //                     wgmma.mma_async m64n128k8 (tf32) into a 64-register accumulator per thread;
 //                     then the fused epilogue (store / tanh / log-sum-exp partials / split-K slice / Adam).
-// Every stage is published by an mbarrier (TMA transaction bytes + one arrival per producer thread) and
+// Every stage is published by an mbarrier (K-major TMA transaction bytes + one arrival per producer thread;
+// MN-major boxes report to a second, per-stage "landed" barrier that the transposing warps wait on) and
 // released by one arrival per consumer warp once the wgmma group that read it has retired.
 // Out-of-range rows / K-tail are zero-filled (by TMA or by the loaders), so any M, N, K work; split-K
-// over blockIdx-independent work items.
+// over blockIdx-independent work items.  Every operand needs a 16-byte aligned base and a row pitch that is a
+// multiple of 4 floats (operand_ok).
 #pragma once
 #include <cuda.h>
 #include <cuda_runtime.h>
@@ -51,6 +54,9 @@ __device__ __forceinline__ void mbar_expect_tx(uint64_t* bar, uint32_t bytes) { 
 }
 __device__ __forceinline__ void mbar_arrive(uint64_t* bar) {
   asm volatile("mbarrier.arrive.shared::cta.b64 _, [%0];" ::"r"(smem_u32(bar)) : "memory");
+}
+__device__ __forceinline__ void mbar_arrive_expect_tx(uint64_t* bar, uint32_t bytes) {
+  asm volatile("mbarrier.arrive.expect_tx.shared::cta.b64 _, [%0], %1;" ::"r"(smem_u32(bar)), "r"(bytes) : "memory");
 }
 __device__ __forceinline__ bool mbar_try_wait(uint64_t* bar, uint32_t parity) {
   uint32_t ok;
@@ -498,7 +504,7 @@ __device__ __forceinline__ void store_chunk(const Epi& epi, const typename Epi::
 
 // ---- A-operand policies -------------------------------------------------------------------------------------
 // Where the producer warpgroup gets the A tile from:
-//   AXNone        : the A operand (TMA when K-major, transposing loads when MN-major)
+//   AXNone        : the A operand (TMA; MN-major tiles are then transposed in shared memory)
 //   AXSoftmaxGrad : the A operand is a LOGITS slab S; the loaders turn each element into dL/dlogits =
 //                   (softmax(S) - onehot) / B on its way into shared memory, given the per-row log-sum-exp,
 //                   so that the separate pass that rewrote the slab (read + write) disappears (option
@@ -523,23 +529,30 @@ __device__ __forceinline__ float ex2_approx(float x) {
 }
 constexpr float kLog2e = 1.4426950408889634f;
 
-template <bool EX_IS_M>      // true: tile rows are examples (A = S); false: tile K is examples (A = S^T)
+template <bool EX_IS_M>      // true: tile rows are examples (A = S, K-major); false: tile K is examples (A = S^T, MN-major)
 struct AXSoftmaxGrad {
   static constexpr int kKind = 1;
   SoftmaxGradArgs a;
-  // v = A(x, k .. k+3) (rows of S: EX_IS_M) or A(x .. x+3, k) (S^T): the four elements share one example.
-  // p = exp(s - lse) / B as one fused multiply-add and one ex2: 2^(s log2(e) + c), c = -lse log2(e) + log2(1/B).
-  // Elements outside [X, K) are zero fill and stay zero.
+  // p = exp(s - lse) / B as one fused multiply-add and one ex2: 2^(s log2(e) + c), c = -lse log2(e) + log2(1/B);
+  // example ex's c and true class (relative to row0):
+  __device__ __forceinline__ void example(int ex, float& c, int& tgt) const {
+    c = fmaf(-a.lse[ex], kLog2e, log2f(a.inv_batch));
+    tgt = a.target[ex] - a.row0;
+  }
+  // element s = S(ex, y) of an example with (c, tgt)
+  __device__ __forceinline__ float p(float s, int y, float c, int tgt) const {
+    return ex2_approx(fmaf(s, kLog2e, c)) - ((y == tgt) ? a.inv_batch : 0.f);
+  }
+  // K-major: v = A(x, k .. k+3), the four elements share example x.  Elements outside [X, K) are zero fill and stay zero.
   __device__ __forceinline__ float4 xform(float4 v, int x, int k, int X, int K) const {
-    const int ex = EX_IS_M ? x : k;
-    if (ex >= (EX_IS_M ? X : K)) return v;
-    const float c = fmaf(-a.lse[ex], kLog2e, log2f(a.inv_batch));
-    const int tgt = a.target[ex] - a.row0;
-    const int y0 = EX_IS_M ? k : x, ny = EX_IS_M ? K : X;
+    static_assert(EX_IS_M, "the MN-major tile is transformed element by element as it is transposed (umma_gemm_kernel)");
+    if (x >= X) return v;
+    float c;
+    int tgt;
+    example(x, c, tgt);
     float e[4] = {v.x, v.y, v.z, v.w};
 #pragma unroll
-    for (int j = 0; j < 4; ++j)
-      e[j] = (y0 + j < ny) ? ex2_approx(fmaf(e[j], kLog2e, c)) - ((y0 + j == tgt) ? a.inv_batch : 0.f) : 0.f;
+    for (int j = 0; j < 4; ++j) e[j] = (k + j < K) ? p(e[j], k + j, c, tgt) : 0.f;
     return make_float4(e[0], e[1], e[2], e[3]);
   }
 };
@@ -553,7 +566,6 @@ struct AXGather {
 
 // ---- tile loaders (producer warpgroup, thread t in [0, 128)) -----------------------------------------------------
 __device__ __forceinline__ float4 ld4(const float* p) { return __ldg(reinterpret_cast<const float4*>(p)); }
-__device__ __forceinline__ float pick(const float4& v, int j) { return j == 0 ? v.x : j == 1 ? v.y : j == 2 ? v.z : v.w; }
 
 // K-major operand (element (x, k) at base[x * ld + k]), rows x0 .. x0+127, k0 .. k0+31 -> SWIZZLE_128B tile.
 // Thread t owns 16-byte chunk c = t % 8 of rows t / 8 + 16 i.
@@ -585,41 +597,29 @@ __device__ __forceinline__ void load_tile_k(uint8_t* dst, const float* base, siz
   }
 }
 
-// MN-major operand (element (x, k) at base[k * ld + x]), same tile.  A warp instruction reads 4 k-rows x 32
-// consecutive x (128 B each) and scatters the float4s into 4 tile rows; lane l stores its four elements in the
-// order (s + l / 8) % 4 so that the 32 scalar stores of one instruction hit 32 different banks.
-template <class AX>
-__device__ __forceinline__ void load_tile_mn(uint8_t* dst, const float* base, size_t ld, int x0, int X, int k0, int K, int t,
-                                             const AX& ax) {
-  const int warp = t >> 5, lane = t & 31;
-  float4 v[8];
+// MN-major operand (element (x, k) at base[k * ld + x]), same tile.  TMA brings it in as four boxes: box q holds
+// x0 + 32q .. +31 for the stage's 32 k, as 32 swizzled 128-byte rows (k) of 32 x, at bytes 4096q .. of the tile --
+// the bytes that rows 32q .. 32q+31 of the K-major tile occupy.  So each warp rewrites one box in place: lane l
+// reads column x = 32q + l, one element per k-row (a warp reads one 128-byte row at a time: no bank conflict),
+// f(s, k) maps each element on the way, and the lane writes its tile row as 8 swizzled float4 chunks (each 8-lane
+// store phase covers 8 distinct 16-byte bank groups).  TMA's zero fill of out-of-range x and k carries over.
+// The box is 1024-byte aligned, so the swizzle is an XOR on one per-lane base address (element (l, k) at
+// (box + 4l) ^ ((k & 7) << 4) + 128k, chunk c of row l at (box + 128l) ^ ((l & 7) << 4) ^ (c << 4)): written so, as
+// shared-memory instructions, the addresses cost one XOR each instead of 40 loop-invariant registers.
+template <class F>
+__device__ __forceinline__ void transpose_box(uint8_t* box, int lane, const F& f) {
+  const uint32_t rd = smem_u32(box) + lane * 4, wr = (smem_u32(box) + lane * 128) ^ ((lane & 7) << 4);
+  float v[BK];
 #pragma unroll
-  for (int i = 0; i < 8; ++i) {
-    const int idx = warp * 8 + i;
-    const int x = x0 + (idx & 3) * 32 + 4 * (lane >> 2), k = k0 + (idx >> 2) * 4 + (lane & 3);
-    v[i] = make_float4(0.f, 0.f, 0.f, 0.f);
-    if (k < K) {
-      const float* p = base + (size_t)k * ld + x;
-      if (x + 3 < X) {
-        v[i] = ld4(p);
-      } else {
-        if (x < X) v[i].x = p[0];
-        if (x + 1 < X) v[i].y = p[1];
-        if (x + 2 < X) v[i].z = p[2];
-      }
-    }
+  for (int k = 0; k < BK; ++k) {
+    asm volatile("ld.shared.f32 %0, [%1];" : "=f"(v[k]) : "r"((rd ^ ((k & 7) << 4)) + k * 128) : "memory");
+    v[k] = f(v[k], k);
   }
+  __syncwarp();
 #pragma unroll
-  for (int i = 0; i < 8; ++i) {
-    const int idx = warp * 8 + i;
-    const int r0 = (idx & 3) * 32 + 4 * (lane >> 2), kk = (idx >> 2) * 4 + (lane & 3);
-    if constexpr (AX::kKind == 1) v[i] = ax.xform(v[i], x0 + r0, k0 + kk, X, K);
-#pragma unroll
-    for (int s = 0; s < 4; ++s) {
-      const int j = (s + (lane >> 3)) & 3, r = r0 + j;
-      *reinterpret_cast<float*>(dst + r * 128 + ((((kk >> 2) ^ (r & 7))) << 4) + (kk & 3) * 4) = pick(v[i], j);
-    }
-  }
+  for (int c = 0; c < BK / 4; ++c)
+    asm volatile("st.shared.v4.f32 [%0], {%1, %2, %3, %4};" ::"r"(wr ^ (c << 4)), "f"(v[4 * c]), "f"(v[4 * c + 1]), "f"(v[4 * c + 2]),
+                 "f"(v[4 * c + 3]) : "memory");
 }
 
 // gather(cs)[m0 .. m0+127, k-block kb] with dropout, as load_tile_k lays it out (d % 32 == 0: a k-block lies in one
@@ -657,10 +657,10 @@ struct GemmShape {
   int n_fastest;              // raster order of work items: 1 = consecutive items share the A tile
   int terms;                  // 1 = plain tf32;  3 = 3xTF32: every K block is issued as A_lo.B_hi + A_hi.B_lo + A_hi.B_hi
 };
-// raw operand pointers (the loaders that do not go through TMA); lo = the 3xTF32 residuals or nullptr
+// the A operand as a raw pointer, for the one loader that does not go through TMA (load_tile_k: AXSoftmaxGrad<true>)
 struct GemmPtrs {
-  const float *a, *a_lo, *b, *b_lo;
-  size_t lda, ldb;
+  const float* a;
+  size_t lda;
 };
 
 struct SmemLayout {
@@ -670,7 +670,8 @@ struct SmemLayout {
   static constexpr int kEpiOffset = STAGES * kStageBytes;                     // per consumer warpgroup: 64 x BN fp32
   static constexpr int kEpiBytes = 64 * BN * 4;
   static constexpr int kBarOffset = kEpiOffset + 2 * kEpiBytes;
-  static constexpr int kTotal = kBarOffset + 256 + 1024;   // barriers, + slack for 1024-B alignment
+  static constexpr int kTotal = kBarOffset + 256 + 1024;   // barriers (full, empty, landed per stage), + slack for 1024-B alignment
+  static_assert(3 * STAGES * 8 <= 256, "the barriers fit their block");
   static_assert(kTotal <= 232448, "exceeds the 227 KB of shared memory a CTA can opt into");
 };
 
@@ -681,20 +682,28 @@ umma_gemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant_
                  GemmPtrs ptr, Epi epi, AX ax = AX{}) {
   if (epi_gate_closed(epi, 0)) return;      // gated fallback pass: nothing to do (uniform over the grid)
   using L = SmemLayout;
-  constexpr bool kTmaA = !A_MN && AX::kKind == 0;
+  static_assert(!(A_MN && AX::kKind == 2), "the gathered A tile is K-major");
+  constexpr bool kTmaA = !A_MN && AX::kKind == 0;     // K-major tiles TMA writes as wgmma reads them
   constexpr bool kTmaB = !B_MN;
   constexpr uint32_t kTxBytes = (kTmaA ? L::kABytes : 0) + (kTmaB ? L::kBBytes : 0);
+  constexpr uint32_t kMnTxBytes = (A_MN ? L::kABytes : 0) + (B_MN ? L::kBBytes : 0);    // MN-major tiles, transposed after landing
+  // How many steps the producer's TMA loads run ahead of the step it completes (transposes and publishes).  The
+  // consumers free step i-1's stage only after issuing step i, so the producer must have published step i-STAGES+1
+  // before it waits for the stage of step i: at most STAGES-2 steps ahead.
+  constexpr int kLag = kMnTxBytes ? STAGES - 2 : 0;
+  static_assert(kLag <= STAGES - 2, "the producer would wait for a stage only a step it has not published can free");
   extern __shared__ uint8_t smem_raw[];
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~(uintptr_t)1023);
-  uint64_t* full_bar = reinterpret_cast<uint64_t*>(smem + L::kBarOffset);
-  uint64_t* empty_bar = full_bar + STAGES;
+  uint64_t* full_bar = reinterpret_cast<uint64_t*>(smem + L::kBarOffset);     // the stage is ready for the MMA
+  uint64_t* empty_bar = full_bar + STAGES;                                     // the MMA has read the stage
+  uint64_t* landed_bar = empty_bar + STAGES;                                   // the MN-major boxes have landed
 
   const int wg = threadIdx.x >> 7, warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
   const int total_items = gs.m_tiles * gs.n_tiles * gs.splits;
   const int total_kblocks = (gs.K + BK - 1) / BK;
 
   if (threadIdx.x == 0) {
-    for (int s = 0; s < STAGES; ++s) { mbar_init(&full_bar[s], 128); mbar_init(&empty_bar[s], 8); }
+    for (int s = 0; s < STAGES; ++s) { mbar_init(&full_bar[s], 128); mbar_init(&empty_bar[s], 8); mbar_init(&landed_bar[s], 1); }
     asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
   }
   __syncthreads();
@@ -716,42 +725,98 @@ umma_gemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant_
   if (wg == 0) {
     // ===================== producer warpgroup =====================
     const int t = threadIdx.x;
-    int stage = 0;
-    uint32_t phase = 0;
-    for (int item = blockIdx.x; item < total_items; item += gridDim.x) {
-      int mt, nt, sp;
-      decode(item, mt, nt, sp);
-      const int kb0 = sp * gs.kblocks_per_split;
-      const int kb1 = min(total_kblocks, kb0 + gs.kblocks_per_split);
-      // 3xTF32: the two small cross terms (A_lo.B_hi, A_hi.B_lo) over the whole K range first, then A_hi.B_hi.
-      // While only the 2^-11-sized cross terms have been accumulated, the rounding of the fp32 accumulator
-      // costs nothing that matters, so the accumulation error is that of ONE pass over K instead of three.
-      auto load_stage = [&](bool a_lo, bool b_lo, int kb) {
-        mbar_wait(&empty_bar[stage], phase ^ 1);
-        uint8_t* sa = smem + stage * L::kStageBytes;
-        uint8_t* sb = sa + L::kABytes;
-        const int k0 = kb * BK;
-        if (kTxBytes && t == 0) {
-          mbar_expect_tx(&full_bar[stage], kTxBytes);
-          if (kTmaA) tma_load_2d(sa, a_lo ? &tmAlo : &tmA, &full_bar[stage], k0, mt * BM);
-          if (kTmaB) tma_load_2d(sb, b_lo ? &tmBlo : &tmB, &full_bar[stage], k0, nt * BN);
-        }
-        if constexpr (AX::kKind == 2) {
-          load_tile_gather(sa, ax, mt * BM, gs.M, kb, ax.Xout != nullptr && nt == 0, t);
-        } else if constexpr (!kTmaA) {
-          if (A_MN) load_tile_mn(sa, a_lo ? ptr.a_lo : ptr.a, ptr.lda, mt * BM, gs.M, k0, gs.K, t, ax);
-          else load_tile_k(sa, a_lo ? ptr.a_lo : ptr.a, ptr.lda, mt * BM, gs.M, k0, gs.K, t, ax);
-        }
-        if constexpr (!kTmaB) load_tile_mn(sb, b_lo ? ptr.b_lo : ptr.b, ptr.ldb, nt * BN, gs.N, k0, gs.K, t, AXNone{});
-        if constexpr (!kTmaA || !kTmaB) fence_proxy_async_smem();     // generic-proxy stores -> visible to wgmma
-        mbar_arrive(&full_bar[stage]);
-        if (++stage == STAGES) { stage = 0; phase ^= 1; }
-      };
-      if (gs.terms == 3) {
-        for (int kb = kb0; kb < kb1; ++kb) load_stage(true, false, kb);
-        for (int kb = kb0; kb < kb1; ++kb) load_stage(false, true, kb);
+    // The step sequence the consumers run: work items; per item, 3xTF32's three passes -- the two small cross terms
+    // (A_lo.B_hi, A_hi.B_lo) over the whole K range first, then A_hi.B_hi (while only the 2^-11-sized cross terms have
+    // been accumulated, the rounding of the fp32 accumulator costs nothing that matters, so the accumulation error is
+    // that of ONE pass over K instead of three); per pass, the K blocks.  Cursors walk it: `ld` issues a step's loads,
+    // `tr` completes the step kLag steps behind (all-K-major: one cursor does both).
+    struct Cursor {
+      int item, mt, nt, kb, kb0, kb1, pass;      // pass 0: A_lo.B_hi, 1: A_hi.B_lo, 2: A_hi.B_hi
+      int stage;
+      uint32_t phase;
+    };
+    auto seek = [&](Cursor& c) {                 // the first step of work item c.item or of the next one that has a step
+      for (; c.item < total_items; c.item += gridDim.x) {
+        int sp;
+        decode(c.item, c.mt, c.nt, sp);
+        c.kb = c.kb0 = sp * gs.kblocks_per_split;
+        c.kb1 = min(total_kblocks, c.kb0 + gs.kblocks_per_split);
+        c.pass = gs.terms == 3 ? 0 : 2;
+        if (c.kb0 < c.kb1) return;
       }
-      for (int kb = kb0; kb < kb1; ++kb) load_stage(false, false, kb);
+    };
+    auto next = [&](Cursor& c) {
+      if (++c.stage == STAGES) { c.stage = 0; c.phase ^= 1; }
+      if (++c.kb < c.kb1) return;
+      if (c.pass < 2) { ++c.pass; c.kb = c.kb0; return; }
+      c.item += gridDim.x;
+      seek(c);
+    };
+    // issue: wait for the stage to be free; K-major TMA on full_bar, MN-major boxes on landed_bar; the loaders that
+    // compute their A tile (gather, K-major softmax gradient) write it now
+    auto issue = [&](const Cursor& c) {
+      mbar_wait(&empty_bar[c.stage], c.phase ^ 1);
+      uint8_t* sa = smem + c.stage * L::kStageBytes;
+      uint8_t* sb = sa + L::kABytes;
+      const int k0 = c.kb * BK;
+      const bool a_lo = c.pass == 0, b_lo = c.pass == 1;
+      if (t == 0) {
+        if (kTxBytes) {
+          mbar_expect_tx(&full_bar[c.stage], kTxBytes);
+          if (kTmaA) tma_load_2d(sa, a_lo ? &tmAlo : &tmA, &full_bar[c.stage], k0, c.mt * BM);
+          if (kTmaB) tma_load_2d(sb, b_lo ? &tmBlo : &tmB, &full_bar[c.stage], k0, c.nt * BN);
+        }
+        if (kMnTxBytes) {
+          mbar_arrive_expect_tx(&landed_bar[c.stage], kMnTxBytes);
+#pragma unroll
+          for (int q = 0; q < 4; ++q) {
+            if (A_MN) tma_load_2d(sa + q * 4096, a_lo ? &tmAlo : &tmA, &landed_bar[c.stage], c.mt * BM + 32 * q, k0);
+            if (B_MN) tma_load_2d(sb + q * 4096, b_lo ? &tmBlo : &tmB, &landed_bar[c.stage], c.nt * BN + 32 * q, k0);
+          }
+        }
+      }
+      if constexpr (AX::kKind == 2) load_tile_gather(sa, ax, c.mt * BM, gs.M, c.kb, ax.Xout != nullptr && c.nt == 0, t);
+      else if constexpr (!A_MN && !kTmaA) load_tile_k(sa, ptr.a, ptr.lda, c.mt * BM, gs.M, k0, gs.K, t, ax);
+    };
+    // complete: transpose the MN-major tiles in place (warp w: box w of each), then publish the stage
+    auto complete = [&](const Cursor& c) {
+      uint8_t* sa = smem + c.stage * L::kStageBytes;
+      uint8_t* sb = sa + L::kABytes;
+      if constexpr (kMnTxBytes != 0) {
+        if constexpr (A_MN && AX::kKind == 1) {
+          // S^T: tile K is examples.  Lane l fetches example k0 + l's (c, target) before the wait; element (x, k)
+          // takes example k's from lane k.
+          const int k0 = c.kb * BK, x = c.mt * BM + 32 * warp + lane;
+          float ce = 0.f;
+          int te = -1;
+          if (k0 + lane < gs.K) ax.example(k0 + lane, ce, te);
+          mbar_wait(&landed_bar[c.stage], c.phase);
+          transpose_box(sa + warp * 4096, lane, [&](float s, int k) {
+            const float ck = __shfl_sync(0xffffffffu, ce, k);
+            const int tk = __shfl_sync(0xffffffffu, te, k);
+            return (x < gs.M && k0 + k < gs.K) ? ax.p(s, x, ck, tk) : 0.f;
+          });
+        } else {
+          mbar_wait(&landed_bar[c.stage], c.phase);
+          if constexpr (A_MN) transpose_box(sa + warp * 4096, lane, [](float s, int) { return s; });
+        }
+        if constexpr (B_MN) transpose_box(sb + warp * 4096, lane, [](float s, int) { return s; });
+      }
+      if constexpr (!kTmaA || !kTmaB) fence_proxy_async_smem();     // generic-proxy stores -> visible to wgmma
+      mbar_arrive(&full_bar[c.stage]);
+    };
+    Cursor ld{static_cast<int>(blockIdx.x), 0, 0, 0, 0, 0, 0, 0, 0u};
+    seek(ld);
+    if constexpr (kLag == 0) {
+      // all-K-major: one cursor (the lagging loop below, run with kLag = 0, was 10-19% slower on these GEMMs on an H100)
+      for (; ld.item < total_items; next(ld)) { issue(ld); complete(ld); }
+    } else {
+      Cursor tr = ld;
+      for (int ahead = 0; tr.item < total_items;) {      // ahead: steps issued and not yet completed
+        const bool more = ld.item < total_items;
+        if (more) { issue(ld); next(ld); ++ahead; }
+        if (ahead > kLag || !more) { complete(tr); next(tr); --ahead; }
+      }
     }
   } else {
     // ===================== consumer warpgroups: rows 64 (wg - 1) .. of the tile =====================
@@ -900,6 +965,12 @@ struct Operand {
   const float* lo = nullptr;
 };
 
+// The tensor map of an operand with X rows (M or N) and depth K: K-major, boxes of 32 k x 128 rows, as wgmma reads
+// them; MN-major, boxes of 32 x x 32 k-rows, four per stage, that the producer transposes.
+inline bool operand_map(CUtensorMap* map, const float* base, bool major_mn, int X, int K, size_t ld) {
+  return major_mn ? make_tensor_map(map, base, (uint64_t)K, (uint64_t)X, ld, BK) : make_tensor_map(map, base, (uint64_t)X, (uint64_t)K, ld, BM);
+}
+
 inline GemmShape make_shape(int M, int N, int K, int splits, int terms) {
   GemmShape gs;
   gs.M = M; gs.N = N; gs.K = K;
@@ -936,15 +1007,13 @@ inline cudaError_t launch_cfg(cudaStream_t st, int M, int N, int K, int splits, 
   const bool three = A.lo != nullptr && B.lo != nullptr;
   if ((A.lo != nullptr) != (B.lo != nullptr)) return cudaErrorInvalidValue;
   if (AX::kKind != 0 && three) return cudaErrorInvalidValue;      // the transforms rewrite a single fp32 tile
-  if (!A_MN && AX::kKind == 0) {
-    if (!make_tensor_map(&tmA, A.base, (uint64_t)M, (uint64_t)K, A.ld, BM)) return cudaErrorInvalidValue;
-    if (three && !make_tensor_map(&tmAlo, A.lo, (uint64_t)M, (uint64_t)K, A.ld, BM)) return cudaErrorInvalidValue;
+  if (A_MN || AX::kKind == 0) {
+    if (!operand_map(&tmA, A.base, A_MN, M, K, A.ld)) return cudaErrorInvalidValue;
+    if (three && !operand_map(&tmAlo, A.lo, A_MN, M, K, A.ld)) return cudaErrorInvalidValue;
   }
-  if (!B_MN) {
-    if (!make_tensor_map(&tmB, B.base, (uint64_t)N, (uint64_t)K, B.ld, BN)) return cudaErrorInvalidValue;
-    if (three && !make_tensor_map(&tmBlo, B.lo, (uint64_t)N, (uint64_t)K, B.ld, BN)) return cudaErrorInvalidValue;
-  }
-  const GemmPtrs ptr{A.base, A.lo, B.base, B.lo, A.ld, B.ld};
+  if (!operand_map(&tmB, B.base, B_MN, N, K, B.ld)) return cudaErrorInvalidValue;
+  if (three && !operand_map(&tmBlo, B.lo, B_MN, N, K, B.ld)) return cudaErrorInvalidValue;
+  const GemmPtrs ptr{A.base, A.ld};
   return launch_kernel<A_MN, B_MN, Epi, AX>(st, tmA, tmB, tmAlo, tmBlo, make_shape(M, N, K, splits, three ? 3 : 1), ptr, epi,
                                             num_sms, ax);
 }
@@ -982,11 +1051,12 @@ inline cudaError_t launch_ctx_fused(cudaStream_t st, int M, int N, const float* 
   GemmShape gs = make_shape(M, N, K, 1, 1);
   gs.n_fastest = 1;          // the CTAs that run together share gathered rows through L2
   const CUtensorMap none{};
-  const GemmPtrs ptr{nullptr, nullptr, W, nullptr, 0, ldw};
-  return launch_kernel<false, true, Epi, AXGather>(st, none, none, none, none, gs, ptr, epi, num_sms, AXGather{cs, dp, Xout});
+  CUtensorMap tmW{};
+  if (!operand_map(&tmW, W, true, N, K, ldw)) return cudaErrorInvalidValue;
+  return launch_kernel<false, true, Epi, AXGather>(st, none, tmW, none, none, gs, GemmPtrs{nullptr, 0}, epi, num_sms, AXGather{cs, dp, Xout});
 }
 
-// TMA constraints on an operand: 16-byte aligned base, row pitch a multiple of 16 bytes.
+// TMA constraints on an operand of either major: 16-byte aligned base, row pitch a multiple of 16 bytes.
 inline bool operand_ok(const Operand& o) {
   return (reinterpret_cast<uintptr_t>(o.base) % 16 == 0) && (o.ld % 4 == 0);
 }
