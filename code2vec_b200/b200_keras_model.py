@@ -106,7 +106,7 @@ class Code2VecModel(_TFNumericsModel):
         cfg = self.config
         self.log("Starting training...")
         reader = PathContextReader(vocabs=self.vocabs, model_input_tensors_former=_TrainInputFormer(), config=cfg,
-                                   estimator_action=EstimatorAction.Train, repeat_endlessly=True)
+                                   estimator_action=EstimatorAction.Train, repeat_endlessly=True, shuffle_seed=self._seed)
         batches = _with_next(_prefetch(reader.get_dataset()))
         former = _TrainInputFormer()
         steps = cfg.train_steps_per_epoch

@@ -82,6 +82,31 @@ def _with_next(iterable):
     yield cur, None
 
 
+DEFAULT_DETERMINISTIC_SEED = 1       # the seed of a C2V_DETERMINISTIC=1 run that names none
+
+
+def run_determinism(environ, now=time.time):
+    """(deterministic, seed) of a training run from its environment.  C2V_DETERMINISTIC=1 sets the engine option
+    "deterministic" (a step's results depend only on its inputs, seeds and options); C2V_SEED=<int >= 0> fixes the dropout
+    seed and the training reader's shuffle seed.  Without C2V_SEED the seed is DEFAULT_DETERMINISTIC_SEED in a
+    deterministic run and derived from the clock otherwise; it is logged either way, so any run can be replayed."""
+    flag = environ.get("C2V_DETERMINISTIC", "0") or "0"
+    if flag not in ("0", "1"):
+        raise ValueError("C2V_DETERMINISTIC must be 0 or 1, got %r" % flag)
+    deterministic = flag == "1"
+    raw = environ.get("C2V_SEED", "")
+    if raw:
+        try:
+            seed = int(raw)
+        except ValueError:
+            raise ValueError("C2V_SEED must be a non-negative integer, got %r" % raw) from None
+        if seed < 0:
+            raise ValueError("C2V_SEED must be a non-negative integer, got %r" % raw)
+    else:
+        seed = DEFAULT_DETERMINISTIC_SEED if deterministic else int(now()) & 0x7FFFFFFF
+    return deterministic, seed
+
+
 _CKPT_MAGIC = b"C2VB200\0"
 _CKPT_SUFFIX = ".c2v_b200"
 
@@ -134,11 +159,15 @@ class Code2VecModel(Code2VecModelBase):
         self.log("b200 backend arithmetic: train = %s, evaluate/predict = %s (C2V_MATH=fp32|tf32|3xtf32 forces one for both)" % (
             {0: "fp32 FFMA", 1: "tf32 tensor cores", 2: "3xTF32 tensor cores (fp32-equivalent)"}[self._math_train],
             {0: "fp32 FFMA", 1: "tf32 tensor cores", 2: "3xTF32 tensor cores (fp32-equivalent)"}[self._math_eval]))
+        # C2V_DETERMINISTIC / C2V_SEED: reproducible training runs (run_determinism)
+        self._deterministic, self._seed = run_determinism(os.environ)
+        self.log("b200 backend run: deterministic = %d, seed = %d (C2V_DETERMINISTIC=%d C2V_SEED=%d replays it)" % (
+            self._deterministic, self._seed, self._deterministic, self._seed))
         # C2V_HINT_NEXT=1: pass each next batch to the engine (c2v_hint_next_batch); off by default
         self._hint_next = os.environ.get("C2V_HINT_NEXT", "0") == "1"
         if self.config.is_training:
-            self.trainer = Trainer(self.engine, keep_prob=self.config.DROPOUT_KEEP_RATE, seed=int(time.time()) & 0x7FFFFFFF,
-                                   adam=self._ADAM)
+            self.trainer = Trainer(self.engine, keep_prob=self.config.DROPOUT_KEEP_RATE, seed=self._seed, adam=self._ADAM,
+                                   deterministic=self._deterministic)
 
     def _create_inner_model(self):
         self._make_engine()
@@ -229,7 +258,7 @@ class Code2VecModel(Code2VecModelBase):
         multi_batch_start_time = time.time()
         num_batches_to_save_and_eval = max(int(cfg.train_steps_per_epoch * cfg.SAVE_EVERY_EPOCHS), 1)
         train_reader = PathContextReader(vocabs=self.vocabs, model_input_tensors_former=_TrainInputFormer(),
-                                         config=cfg, estimator_action=EstimatorAction.Train)
+                                         config=cfg, estimator_action=EstimatorAction.Train, shuffle_seed=self._seed)
         self.log("Started reader...")
         former = _TrainInputFormer()
         # pinned-host batch ring + copy stream (batch_ring.py): the reader thread draws every batch straight into a

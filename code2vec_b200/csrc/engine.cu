@@ -40,6 +40,7 @@ struct Workspace {
   size_t stamp_tok, stamp_path, last_tok, last_path, lr_tab;     // lazy Adam bookkeeping
   size_t stamp_tgt, last_tgt;                                    // ... of the target table (sampled softmax)
   size_t perm, bkt_count, bkt_cursor, bkt_starts;                            // locality-sorted peer gather / scatter (sharded tables)
+  size_t det_keys[2], det_vals[2], det_hist, det_offs, det_starts, det_part;  // deterministic embedding-gradient sort + reduce
   size_t total;
   size_t ldS;
 };
@@ -122,6 +123,14 @@ Workspace carve(const c2v_dims& d) {
   w.W_lo = take(X * D * 4);
   w.v_hi = take(B * D * 4);
   w.v_lo = take(B * D * 4);
+  // option "deterministic": ping-pong keys / values of the 3 N entries, per-tile digit histograms and their scan, and two
+  // chunk-partial slots of d floats per K entries (det_slot)
+  const size_t M = 3 * N, tiles = (M + kDetSortTile - 1) / kDetSortTile;
+  for (int i = 0; i < 2; ++i) { w.det_keys[i] = take(M * 4); w.det_vals[i] = take(M * 4); }
+  w.det_hist = take(kDetRadix * tiles * 4);
+  w.det_offs = take(kDetRadix * tiles * 4);
+  w.det_starts = take((kDetRadix * tiles + 1) * 4);
+  w.det_part = take(2 * ((M + kDetChunk - 1) / kDetChunk) * (size_t)d.embed_dim * 4);
   w.total = off;
   return w;
 }
@@ -617,6 +626,49 @@ int sort_entries(c2v_engine* e, cudaStream_t st, const ContextSource& cs, const 
   return C2V_OK;
 }
 
+// Option "deterministic": the sum of each referenced gradient row in the fixed order of DESIGN.md section 5.1 -- a stable radix
+// sort of the `count` entries by key (keys in [0, nkeys]; nkeys marks an entry that contributes nothing), then chunk sums and
+// their combine.  Every referenced row is stored (the rows are zero before); no atomics, so the result is the same on every run.
+template <class KeyFn, class Contrib>
+int det_row_sums(c2v_engine* e, cudaStream_t st, const KeyFn& key, int count, uint32_t nkeys, const Contrib& contrib,
+                 const DetDest& dst) {
+  if (count <= 0) return C2V_OK;
+  int bits = 1;
+  while (bits < 32 && (1ull << bits) <= nkeys) ++bits;
+  uint32_t* keys[2] = {wsp<uint32_t>(e, e->ws.det_keys[0]), wsp<uint32_t>(e, e->ws.det_keys[1])};
+  int32_t* vals[2] = {wsp<int32_t>(e, e->ws.det_vals[0]), wsp<int32_t>(e, e->ws.det_vals[1])};
+  int32_t* hist = wsp<int32_t>(e, e->ws.det_hist);
+  int32_t* offs = wsp<int32_t>(e, e->ws.det_offs);
+  int blocks = (count + 255) / 256;
+  if (blocks > e->num_sms * 8) blocks = e->num_sms * 8;
+  C2V_LAUNCH(e, (det_keys_kernel<KeyFn><<<blocks, 256, 0, st>>>(key, count, keys[0], vals[0])));
+  const int tiles = (count + kDetSortTile - 1) / kDetSortTile;
+  int cur = 0;
+  for (int shift = 0; shift < bits; shift += 8, cur ^= 1) {
+    C2V_LAUNCH(e, (det_hist_kernel<<<tiles, kDetSortThreads, 0, st>>>(keys[cur], count, shift, hist)));
+    C2V_LAUNCH(e, (bucket_scan_kernel<<<1, 1024, 0, st>>>(hist, offs, wsp<int32_t>(e, e->ws.det_starts), kDetRadix * tiles)));
+    C2V_LAUNCH(e, (det_scatter_kernel<<<tiles, kDetSortThreads, 0, st>>>(keys[cur], vals[cur], count, shift, offs, keys[cur ^ 1],
+                                                                         vals[cur ^ 1])));
+  }
+  const unsigned grid = (unsigned)((count + 255) / 256);
+  float* part = wsp<float>(e, e->ws.det_part);
+  C2V_LAUNCH(e, (det_chunk_kernel<Contrib><<<grid, 256, 0, st>>>(keys[cur], vals[cur], count, nkeys, contrib, dst, part)));
+  C2V_LAUNCH(e, (det_combine_kernel<<<grid, 256, 0, st>>>(keys[cur], count, nkeys, dst, part)));
+  return C2V_OK;
+}
+
+// The embedding-gradient scatter of a train step in deterministic mode, from dX' in dXg.  simt_order: the contributions are
+// formed as simt::ScatterDx forms them ((g * m) * s), else as scatter_dx_kernel does (g * (m * s)).
+int det_scatter(c2v_engine* e, cudaStream_t st, const ContextSource& cs, const float* mask, const Dropout& dp, const float* dXg,
+                bool simt_order) {
+  const c2v_dims& d = e->dims;
+  const DetStepKeys key{cs.src, cs.pth, cs.tgt, mask, d.token_vocab, (uint32_t)(d.token_vocab + d.path_vocab)};
+  const DetDest dst{e->gr_tok.base[0], e->gr_path.base[0], d.token_vocab, d.embed_dim};      // world 1: row r at base[0] + r d
+  if (simt_order)
+    return det_row_sums(e, st, key, 3 * cs.rows, key.nkeys, DetStepContrib<true>{dXg, dp, e->grad_scale, d.embed_dim}, dst);
+  return det_row_sums(e, st, key, 3 * cs.rows, key.nkeys, DetStepContrib<false>{dXg, dp, e->grad_scale, d.embed_dim}, dst);
+}
+
 // Grid of the gather: one wave of resident CTAs (8 warps each; a warp strides over the rows), never more CTAs than rows / 8.
 unsigned gather_blocks(c2v_engine* e, int rows, bool split) {
   int& occ = e->gather_occ[split ? 1 : 0];
@@ -849,6 +901,8 @@ int context_backward(c2v_engine* e, cudaStream_t st, const ContextSource& cs, co
         if ((rc = sort_entries(e, e->side, cs, bp))) return rc;
         C2V_LAUNCH(e, (scatter_sorted_kernel<<<(3 * N + 7) / 8, 256, 0, e->side>>>(cs, dp, mask, wsp<int32_t>(e, e->ws.perm), dXg, e->gr_tok,
                                                                                e->gr_path, e->grad_scale)));
+      } else if (e->deterministic) {      // sorted, fixed-order row sums instead of float atomics
+        if ((rc = det_scatter(e, e->side, cs, mask, dp, dXg, false))) return rc;
       } else {
         C2V_LAUNCH(e, (scatter_dx_kernel<<<(N + 7) / 8, 256, 0, e->side>>>(cs, dp, mask, dXg, e->gr_tok, e->gr_path, e->grad_scale)));
       }
@@ -896,8 +950,15 @@ int context_backward(c2v_engine* e, cudaStream_t st, const ContextSource& cs, co
     PhaseTimer pt(e, PH_DX_SCATTER, st);
     simt::RowsK al{H, (size_t)D};
     simt::RowsK bl{e->theta.W, (size_t)D};
-    simt::ScatterDx ep{cs, e->gr_tok, e->gr_path, mask, dp, e->grad_scale};
-    C2V_LAUNCH(e, C2V_CUDA(e, simt::launch(st, N, K3, D, 1, al, bl, ep)));
+    if (e->deterministic) {        // dX' is stored, then summed row by row in a fixed order
+      float* dXg = wsp<float>(e, e->ws.dXg);
+      simt::StoreC ep{dXg, (size_t)K3, 0};
+      C2V_LAUNCH(e, C2V_CUDA(e, simt::launch(st, N, K3, D, 1, al, bl, ep)));
+      if ((rc = det_scatter(e, st, cs, mask, dp, dXg, true))) return rc;
+    } else {
+      simt::ScatterDx ep{cs, e->gr_tok, e->gr_path, mask, dp, e->grad_scale};
+      C2V_LAUNCH(e, C2V_CUDA(e, simt::launch(st, N, K3, D, 1, al, bl, ep)));
+    }
     e->emb_grads_clean = false;
   }
   return C2V_OK;
@@ -1207,8 +1268,11 @@ int sampled_train_step_impl(c2v_engine* e, cudaStream_t st, const int32_t* src, 
     // their gradient rows cleared) before the forward kernel read them; the update of this step is deferred
     // like an embedding row's.  Dense Adam: the bound buffer is dense, so it is cleared first.
     if (!e->tgt_lazy) C2V_CUDA(e, cudaMemsetAsync(e->grad.tgt, 0, (size_t)e->dims.target_vocab * D * 4, st));
-    C2V_LAUNCH(e, (sampled_softmax_bwd_kernel<<<B + S * ((B + kSampledChunk - 1) / kSampledChunk), kSampledThreads, 0, st>>>(
-        v, dl, target, sampled, B, S, D, e->grad.tgt)));
+    if (e->deterministic)     // one block per distinct row, terms in a fixed order, no atomics
+      C2V_LAUNCH(e, (sampled_softmax_bwd_det_kernel<<<B + S, kSampledThreads, 0, st>>>(v, dl, target, sampled, B, S, D, e->grad.tgt)));
+    else
+      C2V_LAUNCH(e, (sampled_softmax_bwd_kernel<<<B + S * ((B + kSampledChunk - 1) / kSampledChunk), kSampledThreads, 0, st>>>(
+          v, dl, target, sampled, B, S, D, e->grad.tgt)));
   }
   if (e->ev_tgt_ready) C2V_CUDA(e, cudaEventRecord(e->ev_tgt_ready, st));
   return context_backward(e, st, cs, mask, B, dp, dv);
@@ -1410,8 +1474,13 @@ int c2v_set_option(c2v_engine* e, const char* key, int64_t value) {
     return C2V_OK;
   }
   if (!strcmp(key, "deterministic")) {
-    if (value) return fail(e, C2V_ERR_UNSUPPORTED, "deterministic (sorted) embedding scatter-add is not built; float atomics only");
-    e->deterministic = 0;
+    if (value != 0 && value != 1) return fail(e, C2V_ERR_INVALID, "deterministic must be 0 or 1");
+    if (value && e->table_world > 1)
+      return fail(e, C2V_ERR_UNSUPPORTED, "deterministic: the embedding tables are row-sharded over more than one rank, and the "
+                                          "cross-rank red.add scatter into them is order-free");
+    if (value && (int64_t)e->dims.token_vocab + e->dims.path_vocab >= INT32_MAX)
+      return fail(e, C2V_ERR_UNSUPPORTED, "deterministic: token_vocab + path_vocab must be below 2^31");
+    e->deterministic = (int)value;
     return C2V_OK;
   }
   if (!strcmp(key, "profile")) { e->profile = value ? 1 : 0; return C2V_OK; }
@@ -1661,6 +1730,9 @@ int c2v_bind_table_shards(c2v_engine* e, const c2v_table_shards* params, const c
   const int w = params->world;
   if (!(w == 1 || w == 2 || w == 4 || w == 8)) return fail(e, C2V_ERR_INVALID, "world must be 1, 2, 4 or 8");
   if (grads && grads->world != w) return fail(e, C2V_ERR_INVALID, "params / grads world mismatch");
+  if (e->deterministic && w > 1)
+    return fail(e, C2V_ERR_UNSUPPORTED, "deterministic is set: row-sharded tables over more than one rank take order-free "
+                                        "cross-rank red.adds (set deterministic to 0 first)");
   int shift = 0;
   while ((1 << shift) < w) ++shift;
   auto fill = [&](ShardedTable& t, float* const* ptrs) -> bool {
@@ -2013,6 +2085,23 @@ int c2v_selftest_split(c2v_engine* e, const float* x, float* hi, float* lo, size
   if (blocks < 1) blocks = 1;
   C2V_LAUNCH(e, (split_tf32_kernel<<<(unsigned)blocks, 256, 0, (cudaStream_t)stream>>>(x, hi, lo, count / 4)));
   return C2V_OK;
+}
+
+int c2v_selftest_row_sum(c2v_engine* e, int32_t table_id, const int32_t* rows, const float* vals, int32_t count, float* out,
+                         void* stream) {
+  if (!e || !rows || !vals || !out) return C2V_ERR_INVALID;
+  if (!e->wbase) return fail(e, C2V_ERR_STATE, "workspace not bound (c2v_bind_workspace)");
+  if (table_id != 0 && table_id != 1) return fail(e, C2V_ERR_INVALID, "table_id must be 0 (token table) or 1 (path table)");
+  if (count < 0 || (int64_t)count > 3ll * e->dims.max_batch * e->dims.max_contexts)
+    return fail(e, C2V_ERR_INVALID, "count must be in [0, 3 * max_batch * max_contexts]");
+  if (((uintptr_t)vals | (uintptr_t)out) % 16) return fail(e, C2V_ERR_INVALID, "vals and out must be 16-byte aligned");
+  if ((int64_t)e->dims.token_vocab + e->dims.path_vocab >= INT32_MAX)
+    return fail(e, C2V_ERR_UNSUPPORTED, "token_vocab + path_vocab must be below 2^31");
+  C2V_CUDA(e, cudaSetDevice(e->device));
+  const c2v_dims& d = e->dims;
+  const DetDest dst{out, out, d.token_vocab, d.embed_dim};
+  return det_row_sums(e, (cudaStream_t)stream, DetListKeys{rows, table_id ? d.token_vocab : 0}, count,
+                      (uint32_t)(d.token_vocab + d.path_vocab), DetListContrib{vals, d.embed_dim}, dst);
 }
 
 int64_t c2v_launch_count(const c2v_engine* e) { return e ? e->launches : 0; }

@@ -1327,4 +1327,253 @@ adam_sweep_kernel(float* __restrict__ p, float* __restrict__ g, float* __restric
   }
 }
 
+// ---------------------------------------------------------------------------------------------
+// Deterministic embedding-gradient reduction (option "deterministic", DESIGN.md section 5.1).
+//
+// The entries e = 3 n + seg of a batch are keyed by (table, row): key = row for the token table (seg 0, 2), T + row for the
+// path table (seg 1), and nkeys = T + P for masked contexts, which therefore sort behind every real key and are never
+// summed.  A stable LSD radix sort (8-bit digits: per-tile histograms, bucket_scan_kernel, stable per-tile scatter)
+// lists each row's entries in increasing e.  A row's entries are then cut into chunks of kDetChunk, aligned at the row's
+// first entry; each chunk is summed left to right from +0.0f by one warp, and the chunk sums of a row are added left to
+// right from +0.0f.  The gradient row is zero before the step, so the sum is stored, not added.
+// ---------------------------------------------------------------------------------------------
+constexpr int kDetChunk = 32;                 // K: entries per chunk
+constexpr int kDetSortThreads = 256;
+constexpr int kDetSortTile = 4096;            // entries per radix-sort tile (16 rounds of 256)
+constexpr int kDetRadix = 256;                // 8-bit digits
+
+// key of entry e of a train step's batch
+struct DetStepKeys {
+  const int32_t* src;
+  const int32_t* pth;
+  const int32_t* tgt;
+  const float* mask;
+  int T;          // token rows: path keys start here
+  uint32_t nkeys; // T + P: the key of a masked entry
+  __device__ __forceinline__ uint32_t operator()(int e) const {
+    const int n = e / 3, seg = e - 3 * n;
+    if (mask[n] == 0.f) return nkeys;
+    return seg == 1 ? (uint32_t)(T + pth[n]) : (uint32_t)(seg == 0 ? src[n] : tgt[n]);
+  }
+};
+// key of entry e of c2v_selftest_row_sum: one row list of one table
+struct DetListKeys {
+  const int32_t* rows;
+  int base;       // 0 (token table) or T (path table)
+  __device__ __forceinline__ uint32_t operator()(int e) const { return (uint32_t)(base + rows[e]); }
+};
+
+template <class KeyFn>
+__global__ void __launch_bounds__(256)
+det_keys_kernel(const __grid_constant__ KeyFn key, int count, uint32_t* __restrict__ keys, int32_t* __restrict__ vals) {
+  for (int e = blockIdx.x * 256 + threadIdx.x; e < count; e += gridDim.x * 256) {
+    keys[e] = key(e);
+    vals[e] = e;
+  }
+}
+
+// hist[digit * tiles + tile] = entries of the tile whose key has this digit at `shift`
+__global__ void __launch_bounds__(kDetSortThreads)
+det_hist_kernel(const uint32_t* __restrict__ keys, int count, int shift, int32_t* __restrict__ hist) {
+  __shared__ int32_t h[kDetRadix];
+  h[threadIdx.x] = 0;
+  __syncthreads();
+  const int lo = blockIdx.x * kDetSortTile, hi = min(count, lo + kDetSortTile);
+  for (int i = lo + threadIdx.x; i < hi; i += kDetSortThreads) atomicAdd(&h[(keys[i] >> shift) & (kDetRadix - 1)], 1);
+  __syncthreads();
+  hist[threadIdx.x * gridDim.x + blockIdx.x] = h[threadIdx.x];
+}
+
+// Stable scatter of one tile: offs = exclusive scan of hist (digit-major), so the tile's entries with digit q go to
+// offs[q * tiles + tile] onwards, in their order inside the tile.  The tile is walked in rounds of 256 entries; inside a
+// round a warp ranks its lanes with __match_any_sync and the warps' counts are prefixed in warp order.
+__global__ void __launch_bounds__(kDetSortThreads)
+det_scatter_kernel(const uint32_t* __restrict__ keys, const int32_t* __restrict__ vals, int count, int shift,
+                   const int32_t* __restrict__ offs, uint32_t* __restrict__ okeys, int32_t* __restrict__ ovals) {
+  constexpr int W = kDetSortThreads / 32;
+  __shared__ int32_t wc[W][kDetRadix];
+  __shared__ int32_t run[kDetRadix];
+  __shared__ int32_t goff[kDetRadix];
+  const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
+  run[tid] = 0;
+  goff[tid] = offs[tid * gridDim.x + blockIdx.x];
+  const int lo = blockIdx.x * kDetSortTile, hi = min(count, lo + kDetSortTile);
+  for (int base = lo; base < hi; base += kDetSortThreads) {
+#pragma unroll
+    for (int w = 0; w < W; ++w) wc[w][tid] = 0;
+    __syncthreads();
+    const int i = base + tid;
+    const bool valid = i < hi;
+    const uint32_t k = valid ? keys[i] : 0u;
+    const int q = valid ? (int)((k >> shift) & (kDetRadix - 1)) : kDetRadix + lane;      // idle lanes match nobody
+    const unsigned peers = __match_any_sync(0xffffffffu, q);
+    const int rank = __popc(peers & ((1u << lane) - 1u));
+    if (valid && rank == 0) wc[warp][q] = __popc(peers);
+    __syncthreads();
+    {
+      int r = run[tid];
+#pragma unroll
+      for (int w = 0; w < W; ++w) { const int c = wc[w][tid]; wc[w][tid] = r; r += c; }
+      run[tid] = r;
+    }
+    __syncthreads();
+    if (valid) {
+      const int pos = goff[q] + wc[warp][q] + rank;
+      okeys[pos] = k;
+      ovals[pos] = vals[i];
+    }
+    __syncthreads();
+  }
+}
+
+// contribution of entry e to columns [4 c4, 4 c4 + 4) of its row in a train step: dX'[n, seg d + col] x dropout multiplier x
+// grad_scale, as scatter_dx_kernel (SIMT_ORDER false: g * (m * s)) or simt::ScatterDx (true: (g * m) * s) computes it
+template <bool SIMT_ORDER>
+struct DetStepContrib {
+  const float* dX;
+  Dropout dp;
+  float grad_scale;
+  int d;
+  __device__ __forceinline__ float4 operator()(int e, int c4) const {
+    const int n = e / 3, seg = e - 3 * n, j = seg * d + c4 * 4;
+    float4 g = *reinterpret_cast<const float4*>(dX + (size_t)n * 3 * d + j);
+    const float4 m = dropout_mult4(dp, n, j >> 2);
+    if (SIMT_ORDER) {
+      g.x = __fmul_rn(__fmul_rn(g.x, m.x), grad_scale); g.y = __fmul_rn(__fmul_rn(g.y, m.y), grad_scale);
+      g.z = __fmul_rn(__fmul_rn(g.z, m.z), grad_scale); g.w = __fmul_rn(__fmul_rn(g.w, m.w), grad_scale);
+    } else {
+      g.x = __fmul_rn(g.x, __fmul_rn(m.x, grad_scale)); g.y = __fmul_rn(g.y, __fmul_rn(m.y, grad_scale));
+      g.z = __fmul_rn(g.z, __fmul_rn(m.z, grad_scale)); g.w = __fmul_rn(g.w, __fmul_rn(m.w, grad_scale));
+    }
+    return g;
+  }
+};
+// c2v_selftest_row_sum: entry e contributes vals[e, :]
+struct DetListContrib {
+  const float* vals;
+  int d;
+  __device__ __forceinline__ float4 operator()(int e, int c4) const {
+    return *reinterpret_cast<const float4*>(vals + (size_t)e * d + c4 * 4);
+  }
+};
+
+// where key k's row lives: token table for k < T, path table otherwise (the tables are local: one shard at most)
+struct DetDest {
+  float* tok;
+  float* path;
+  int T, d;
+  __device__ __forceinline__ float* row(uint32_t k) const {
+    return (int)k < T ? tok + (size_t)k * d : path + (size_t)((int)k - T) * d;
+  }
+};
+
+__device__ __forceinline__ float4 add4_rn(float4 a, const float4& b) {
+  a.x = __fadd_rn(a.x, b.x); a.y = __fadd_rn(a.y, b.y); a.z = __fadd_rn(a.z, b.z); a.w = __fadd_rn(a.w, b.w);
+  return a;
+}
+
+// slot of the partial of the chunk starting at sorted position i (first: it is its row's first chunk).  Rows with more
+// than one chunk are longer than K, so a window [aK, aK + K) holds at most one first and one later chunk of such rows.
+__device__ __forceinline__ size_t det_slot(int i, bool first) { return 2 * (size_t)(i / kDetChunk) + (first ? 1 : 0); }
+
+// Pass 1: one warp per 32 sorted positions; every position that starts a chunk (its offset from its row's first entry is a
+// multiple of K) is summed by the warp.  A row of one chunk is stored; otherwise the chunk sum goes to its partial slot.
+template <class Contrib>
+__global__ void __launch_bounds__(256)
+det_chunk_kernel(const uint32_t* __restrict__ keys, const int32_t* __restrict__ vals, int count, uint32_t nkeys,
+                 const __grid_constant__ Contrib contrib, const __grid_constant__ DetDest dst, float* __restrict__ part) {
+  const int lane = threadIdx.x & 31;
+  const int i = blockIdx.x * 256 + threadIdx.x;
+  bool start = false;
+  int first = i;
+  uint32_t k = nkeys;
+  if (i < count) {
+    k = keys[i];
+    if (k < nkeys && i > 0 && keys[i - 1] == k) {        // inside a row: find the row's first entry (lower bound)
+      int lo = 0, hi = i - 1;
+      while (lo < hi) {
+        const int mid = (lo + hi) >> 1;
+        if (keys[mid] < k) lo = mid + 1; else hi = mid;
+      }
+      first = lo;
+    }
+    start = k < nkeys && (i - first) % kDetChunk == 0;
+  }
+  unsigned todo = __ballot_sync(0xffffffffu, start);
+  const int d4 = dst.d / 4;
+  while (todo) {
+    const int b = __ffs(todo) - 1;
+    todo &= todo - 1;
+    const int p = __shfl_sync(0xffffffffu, i, b);
+    const int f = __shfl_sync(0xffffffffu, first, b);
+    const uint32_t kk = __shfl_sync(0xffffffffu, k, b);
+    int end = p + 1;
+    while (end < count && end < p + kDetChunk && keys[end] == kk) ++end;
+    const bool single = p == f && !(end < count && keys[end] == kk);
+    for (int c4 = lane; c4 < d4; c4 += 32) {
+      float4 acc = make_float4(0.f, 0.f, 0.f, 0.f);
+      for (int j = p; j < end; ++j) acc = add4_rn(acc, contrib(vals[j], c4));
+      float* out = single ? dst.row(kk) : part + det_slot(p, p == f) * dst.d;
+      reinterpret_cast<float4*>(out)[c4] = acc;
+    }
+  }
+}
+
+// Pass 2: the first position of every row with more than one chunk adds the row's chunk sums in order and stores the row.
+__global__ void __launch_bounds__(256)
+det_combine_kernel(const uint32_t* __restrict__ keys, int count, uint32_t nkeys, const __grid_constant__ DetDest dst,
+                   const float* __restrict__ part) {
+  const int lane = threadIdx.x & 31;
+  const int i = blockIdx.x * 256 + threadIdx.x;
+  bool lead = false;
+  uint32_t k = nkeys;
+  if (i < count) {
+    k = keys[i];
+    lead = k < nkeys && (i == 0 || keys[i - 1] != k) && i + kDetChunk < count && keys[i + kDetChunk] == k;
+  }
+  unsigned todo = __ballot_sync(0xffffffffu, lead);
+  const int d4 = dst.d / 4;
+  while (todo) {
+    const int b = __ffs(todo) - 1;
+    todo &= todo - 1;
+    const int f = __shfl_sync(0xffffffffu, i, b);
+    const uint32_t kk = __shfl_sync(0xffffffffu, k, b);
+    for (int c4 = lane; c4 < d4; c4 += 32) {
+      float4 acc = make_float4(0.f, 0.f, 0.f, 0.f);
+      for (int p = f; p < count && keys[p] == kk; p += kDetChunk)
+        acc = add4_rn(acc, reinterpret_cast<const float4*>(part + det_slot(p, p == f) * dst.d)[c4]);
+      reinterpret_cast<float4*>(dst.row(kk))[c4] = acc;
+    }
+  }
+}
+
+// Deterministic sampled-softmax target gradient.  The B + S row ids are read as one list L = (target[0..B), sampled[0..S));
+// block j owns row L[j] if j is that row's first occurrence in L, and stores
+//   sum over L in order: true terms dl[b,0] v_b (one product each), then sampled terms, each the chunk sums of
+//   sampled_softmax_bwd_kernel (b in chunks of kSampledChunk, accumulated as there) added chunk by chunk
+// -- every addition left to right from +0.0f.  The gradient rows are zero before the step (cleared or caught up).
+__global__ void __launch_bounds__(kSampledThreads)
+sampled_softmax_bwd_det_kernel(const float* __restrict__ v, const float* __restrict__ dl, const int32_t* __restrict__ target,
+                               const int32_t* __restrict__ sampled, int B, int S, int D, float* __restrict__ g_tgt) {
+  const int j = blockIdx.x;
+  const int row = j < B ? target[j] : sampled[j - B];
+  for (int q = 0; q < j; ++q)
+    if ((q < B ? target[q] : sampled[q - B]) == row) return;          // not the first occurrence
+  for (int i = threadIdx.x; i < D; i += kSampledThreads) {
+    float acc = 0.f;
+    for (int b = j < B ? j : B; b < B; ++b)
+      if (target[b] == row) acc = __fadd_rn(acc, __fmul_rn(dl[(size_t)b * (S + 1)], v[(size_t)b * D + i]));
+    for (int s = 0; s < S; ++s) {
+      if (sampled[s] != row) continue;
+      for (int b0 = 0; b0 < B; b0 += kSampledChunk) {
+        const int b1 = min(B, b0 + kSampledChunk);
+        float c = 0.f;
+        for (int b = b0; b < b1; ++b) c += dl[(size_t)b * (S + 1) + 1 + s] * v[(size_t)b * D + i];
+        acc = __fadd_rn(acc, c);
+      }
+    }
+    g_tgt[(size_t)row * D + i] = acc;
+  }
+}
+
 }  // namespace c2v

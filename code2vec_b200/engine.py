@@ -89,6 +89,7 @@ _SIGNATURES = {
     "c2v_selftest_gemm3": (C.c_int, [_P, _I32, _I32, _I32, _I32, _I32, _I32, _I32, _P, _P, C.c_size_t, _P, _P, C.c_size_t,
                                      _P, C.c_size_t, _P]),
     "c2v_selftest_split": (C.c_int, [_P, _P, _P, _P, C.c_size_t, _P]),
+    "c2v_selftest_row_sum": (C.c_int, [_P, _I32, _P, _P, _I32, _P, _P]),
     "c2v_set_event": (C.c_int, [_P, C.c_char_p, _P]),
     "c2v_sync_tables": (C.c_int, [_P, _P]),
     "c2v_context_forward": (C.c_int, [_P, _P, _P, _P, _P, _I32, C.c_float, C.c_uint64, C.c_uint64, _P, _P, _P]),
@@ -305,6 +306,19 @@ class PathAttentionEngine:
         if rc < 0:
             self._check(rc)
         return out[:rc].sum(dim=0)
+
+    def selftest_row_sum(self, table_id: int, rows, vals):
+        """Test hook for option "deterministic" (c2v_selftest_row_sum): a zeroed copy of table `table_id` (0 = token,
+        1 = path) into which row rows[i] receives vals[i] (device int32 [count], float32 [count, embed_dim]), summed by the
+        train step's sort + chunked reduce in its documented order.  Returns the table as a device tensor."""
+        torch = self.torch
+        rows = rows.to(device=self.dev, dtype=torch.int32).contiguous()
+        vals = vals.to(device=self.dev, dtype=torch.float32).contiguous()
+        n_rows = self.dims.token_vocab if table_id == 0 else self.dims.path_vocab
+        out = torch.zeros((n_rows, self.dims.embed_dim), dtype=torch.float32, device=self.dev)
+        self._check(self.lib.c2v_selftest_row_sum(self.h, int(table_id), rows.data_ptr(), vals.data_ptr(), int(rows.numel()),
+                                                  out.data_ptr(), self._stream()))
+        return out
 
     def phase_stats(self, reset: bool = False) -> Dict[str, Tuple[float, int]]:
         """{phase name: (total device ms, number of timed occurrences)} since the last reset

@@ -128,6 +128,19 @@ def make_fully_sharded_engine(dims, local_batch: int, device: int, group=None, t
     return eng
 
 
+def deterministic_refusal(schedule: str, world: int, push_grads: bool) -> Optional[str]:
+    """Why `schedule` on `world` ranks cannot run with the engine option "deterministic", or None if it can.  The option
+    fixes the order of every reduction into tables the engine holds itself; row-sharded tables over several ranks take
+    order-free cross-rank red.adds (or inbox folds).  NCCL's own reduction order (allreduce / sharded) is outside it."""
+    if schedule in ("table_sharded", "fully_sharded") and world > 1:
+        if push_grads:
+            return ("deterministic training is not available with the %s schedule on %d ranks: peers push embedding "
+                    "gradients into a scatter inbox that is folded with atomics" % (schedule, world))
+        return ("deterministic training is not available with the %s schedule on %d ranks: the embedding tables are "
+                "row-sharded and peers red.add into them in no fixed order" % (schedule, world))
+    return None
+
+
 def shard_bounds(n: int, rank: int, world: int):
     """Contiguous slice [lo, hi) of n items owned by `rank` (sizes differ by at most 1)."""
     base, rem = divmod(n, world)
@@ -138,7 +151,8 @@ def shard_bounds(n: int, rank: int, world: int):
 class Trainer:
     def __init__(self, engine: PathAttentionEngine, keep_prob: float = 0.75, seed: int = 0, group=None,
                  adam: Optional[dict] = None, schedule: str = "table_sharded", lazy_adam: bool = True,
-                 fuse_target_adam: bool = True, push_grads: bool = False, allow_single_rank: bool = False):
+                 fuse_target_adam: bool = True, push_grads: bool = False, allow_single_rank: bool = False,
+                 deterministic: bool = False):
         self.e = engine
         self.keep = float(keep_prob)
         self.seed = int(seed)
@@ -155,6 +169,12 @@ class Trainer:
         self.schedule = schedule if self.multi else "single"
         if self.schedule in ("table_sharded", "fully_sharded") and self.world not in (1, 2, 4, 8):
             self.schedule = "sharded"
+        # deterministic: every step's results depend only on its inputs, seeds and options (engine option "deterministic")
+        self.deterministic = bool(deterministic)
+        if self.deterministic:
+            why = deterministic_refusal(self.schedule, self.world, push_grads)
+            if why:
+                raise ValueError(why)
         if self.schedule == "fully_sharded":
             if not hasattr(engine, "target_row0"):
                 raise ValueError("the fully_sharded schedule needs an engine from make_fully_sharded_engine()")
@@ -218,6 +238,7 @@ class Trainer:
             # dY (+ the target table's Adam step) straight after dv: on one GPU it is HBM-bound like the scatter-add
             # it would otherwise share the memory system with (dy_late 0/1/2 all measure within 1 %)
             engine.set_option("dy_late", 0)
+        engine.set_option("deterministic", 1 if self.deterministic else 0)
         self._loss_host = torch.zeros(1, dtype=torch.float32).pin_memory()
 
     # ---- inputs already resident on the device ----------------------------------------------

@@ -103,8 +103,20 @@ int c2v_bind_params(c2v_engine* e, const c2v_tensors* theta);         /* tf.get_
 int c2v_bind_grads(c2v_engine* e, const c2v_tensors* grads);          /* autodiff outputs of minimize(), :232   */
 int c2v_bind_adam_state(c2v_engine* e, const c2v_tensors* m, const c2v_tensors* v);  /* Adam slots, :232       */
 
-/* Options: "math_mode" (c2v_math_mode), "deterministic" (reserved: only 0 is accepted -- the
- * embedding scatter-add uses float atomics; every other reduction is fixed-order), "cta_pair"
+/* Options: "math_mode" (c2v_math_mode), "deterministic" (0/1, default 0, may change between steps: with 1 a train step's
+ * results depend only on its inputs, seeds and options -- not on scheduling, streams or the run -- on the same build and
+ * device type.  Every other reduction of a step is fixed-order already; this option replaces the two that use float
+ * atomics.  Embedding gradients: for a gradient row, the unmasked entries e = 3 n + seg that reference it (token table:
+ * seg 0 = source, 2 = target; path table: seg 1) are listed in increasing e; entry e contributes exactly what the atomic
+ * scatter adds (dX'[n, seg d : (seg+1) d] x dropout multiplier x grad scale); the list is cut into consecutive chunks of
+ * K = 32 entries starting at the row's first entry, each chunk is summed left to right from +0.0f, and the chunk sums are
+ * added left to right from +0.0f.  Sampled softmax (c2v_sampled_train_step): a target row's gradient is, from +0.0f and
+ * left to right, its true-row terms dl[b,0] v_b in b order, then for each sampled position s holding the row (in s order)
+ * the sums over b of dl[b,1+s] v_b in chunks of 64 examples, chunk by chunk.  Refused (C2V_ERR_UNSUPPORTED) while the
+ * embedding tables are row-sharded over more than one rank (c2v_bind_table_shards, world > 1; a scatter inbox can only be
+ * bound on top of that) -- their cross-rank red.adds and inbox folds stay order-free -- and binding such shards while it
+ * is set fails the same way.  The order in which NCCL reduces
+ * the gradients of data-parallel schedules is outside this guarantee), "cta_pair"
  * (0, 1 or 2, default 2: accepted for ABI compatibility
  * (it once selected CTA-pair GEMMs); the sm_90a GEMM has no CTA-pair form and ignores it), "dy_late" (where the target-table gradient GEMM dY = P^T.v -- with the
  * target table's Adam step in its epilogue when armed -- runs: 0 = right after dv on the caller's
@@ -360,6 +372,14 @@ int c2v_selftest_gemm3(c2v_engine* e, int32_t a_mn, int32_t b_mn, int32_t bn, in
                        const float* B, const float* B_lo, size_t ldb, float* C, size_t ldc,
                        void* stream);
 int c2v_selftest_split(c2v_engine* e, const float* x, float* hi, float* lo, size_t count, void* stream);
+
+/* Test hook for option "deterministic": the sort + chunked reduce of a train step's embedding-gradient scatter, on
+ * `count` caller-given contributions instead of dX' (no dropout, no scaling): row rows[i] of table table_id (0 = token
+ * table [T, d], 1 = path table [P, d]; d = embed_dim) receives vals[i, 0:d], summed in the order the option documents,
+ * and is stored into out (the table, zero on entry: unreferenced rows are not written).  count <= 3 * max_batch *
+ * max_contexts; rows must be in range; vals and out are 16-byte aligned device pointers. */
+int c2v_selftest_row_sum(c2v_engine* e, int32_t table_id, const int32_t* rows, const float* vals, int32_t count,
+                         float* out, void* stream);
 
 /* Introspection for tests and bench: number of kernels the engine has launched so far. */
 int64_t c2v_launch_count(const c2v_engine* e);
