@@ -33,6 +33,7 @@ constexpr int kSplitDw = 48;   // split-K slices for dW = X'^T . dU  (K = B*C)
 struct Workspace {
   size_t H, Xg, dXg, alpha, v, dv, S, loss_b, lse, loss, part, da_part, lse_part, dl;
   size_t Xg_lo, H_lo, S_lo, tgt_hi, tgt_lo, W_hi, W_lo, v_hi, v_lo;     // 3xTF32 operand splits
+  size_t WT, WT_lo, vT, vT_lo, tgtT, tgtT_lo;     // K-major copies of W, v, Ytab for ctx_fwd, dY, dv (3xTF32: hi^T, lo^T)
   size_t true_logit, rscale, v_scaled, slab_flag;                  // exp_slab schedule: row factors, scaled code vectors, {range flag, fallback count}
   size_t st_src, st_pth, st_tgt, st_mask, st_target, st_topk_idx, st_topk_val, st_code, st_attn;
   size_t nx_src, nx_pth, nx_tgt;                                  // indices of the hinted NEXT batch (host entry point)
@@ -43,6 +44,7 @@ struct Workspace {
   size_t det_keys[2], det_vals[2], det_hist, det_offs, det_starts, det_part;  // deterministic embedding-gradient sort + reduce
   size_t total;
   size_t ldS;
+  size_t ldB;     // row pitch of vT: the batch rounded up to 16 bytes, as TMA requires
 };
 
 bool dims_ok(const c2v_dims* d, std::string* why) {
@@ -62,6 +64,7 @@ Workspace carve(const c2v_dims& d) {
   Workspace w{};
   const size_t N = (size_t)d.max_batch * d.max_contexts, D = d.code_dim, B = d.max_batch, X = 3 * (size_t)d.embed_dim;
   w.ldS = align_up((size_t)d.target_vocab, 64);
+  w.ldB = align_up(B, 4);
   size_t off = 0;
   auto take = [&](size_t bytes) { size_t o = off; off = align_up(off + bytes); return o; };
   w.H = take(N * D * 4);
@@ -123,6 +126,14 @@ Workspace carve(const c2v_dims& d) {
   w.W_lo = take(X * D * 4);
   w.v_hi = take(B * D * 4);
   w.v_lo = take(B * D * 4);
+  // K-major (transposed) copies of the operands the engine stores MN-major: W^T [D, 3d] for ctx_fwd, v^T [D, ldB] for dY,
+  // Ytab^T [D, ldS] for dv; in 3xTF32 they hold the high parts and the *_lo regions the residuals
+  w.WT = take(X * D * 4);
+  w.WT_lo = take(X * D * 4);
+  w.vT = take(D * w.ldB * 4);
+  w.vT_lo = take(D * w.ldB * 4);
+  w.tgtT = take(D * w.ldS * 4);
+  w.tgtT_lo = take(D * w.ldS * 4);
   // option "deterministic": ping-pong keys / values of the 3 N entries, per-tile digit histograms and their scan, and two
   // chunk-partial slots of d floats per K entries (det_slot)
   const size_t M = 3 * N, tiles = (M + kDetSortTile - 1) / kDetSortTile;
@@ -196,7 +207,7 @@ struct c2v_engine {
   int64_t full_flush_t = 0;             // step count as of which every row was last known to be current
   int rest_shortcut = 1;                // option "adam_rest_shortcut": replay_row may stop dividing once theta rests
   bool tgt_lazy = false;                // the target table's rows are updated lazily too (sampled softmax steps)
-  bool tgt_split_valid = false;         // 3xTF32: ws.tgt_hi / tgt_lo hold the split of the current target table
+  bool tgt_t_valid = false;             // ws.tgtT (3xTF32: tgtT / tgtT_lo, as the split) holds the current target table transposed
   bool lazy_grads_pending = false;  // a train step's embedding gradients are in the tables and c2v_adam_step has not followed
   int64_t adam_t_done = 0;   // Adam steps applied so far
   int32_t mark_epoch = 0;
@@ -589,6 +600,36 @@ int split_small(c2v_engine* e, cudaStream_t st, const float* x, size_t n, size_t
   return C2V_OK;
 }
 
+// K-major copy [cols, ldT] (workspace region off_t) of a row-major operand x [rows, cols] that a GEMM reads MN-major.  split
+// (3xTF32): the transposed tf32 split goes to off_t / off_lo, and the untransposed one to hi / lo when they are given.
+int transpose_operand(c2v_engine* e, cudaStream_t st, const float* x, int rows, int cols, size_t ldT, size_t off_t, bool split,
+                      size_t off_lo = 0, float* hi = nullptr, float* lo = nullptr) {
+  const dim3 grid((unsigned)((rows + 31) / 32), (unsigned)((cols + 31) / 32));
+  if (split)
+    C2V_LAUNCH(e, (transpose_kernel<true><<<grid, 256, 0, st>>>(x, rows, cols, wsp<float>(e, off_t), wsp<float>(e, off_lo), ldT, hi, lo)));
+  else
+    C2V_LAUNCH(e, (transpose_kernel<false><<<grid, 256, 0, st>>>(x, rows, cols, wsp<float>(e, off_t), nullptr, ldT, nullptr, nullptr)));
+  return C2V_OK;
+}
+
+// Ytab^T for dv, from the current target table (every row must be current: callers run end_target_lazy first).  3xTF32: as
+// its transposed split, and with with_split also the untransposed split into tgt_hi / tgt_lo that the logits GEMM reads.
+int transpose_table(c2v_engine* e, cudaStream_t st, bool with_split) {
+  const int Y = e->dims.target_vocab, D = e->dims.code_dim;
+  int rc;
+  if (is_3x(e)) {
+    PhaseTimer pt(e, PH_SPLIT, st);
+    rc = transpose_operand(e, st, e->theta.tgt, Y, D, e->ws.ldS, e->ws.tgtT, true, e->ws.tgtT_lo,
+                           with_split ? wsp<float>(e, e->ws.tgt_hi) : nullptr, with_split ? wsp<float>(e, e->ws.tgt_lo) : nullptr);
+  } else {
+    PhaseTimer pt(e, PH_DV, st);
+    rc = transpose_operand(e, st, e->theta.tgt, Y, D, e->ws.ldS, e->ws.tgtT, false);
+  }
+  if (rc) return rc;
+  e->tgt_t_valid = true;
+  return C2V_OK;
+}
+
 // Sharded tables: bucket the batch's 3 B C context entries by (owner rank, 2 MB page of the owner's shard) into ws.perm.
 // Returns false when the plan does not apply (tables not sharded, option off, too many buckets).
 bool plan_buckets(c2v_engine* e, BucketPlan* bp, bool force = false) {
@@ -720,16 +761,23 @@ int run_ctx_fwd(c2v_engine* e, cudaStream_t st, const ContextSource& cs, const D
       } else if (x3) C2V_LAUNCH(e, (gather_ctx_kernel<true><<<gather_blocks(e, cs.rows, true), 256, 0, st>>>(cs, dp, Xg, wsp<float>(e, e->ws.Xg_lo))));
       else C2V_LAUNCH(e, (gather_ctx_kernel<false><<<gather_blocks(e, cs.rows, false), 256, 0, st>>>(cs, dp, Xg, nullptr)));
     }
-    if (x3) { int rcs = split_small(e, st, e->theta.W, (size_t)K * D, e->ws.W_hi, e->ws.W_lo); if (rcs) return rcs; }
+    // B = W^T, K-major.  3xTF32: one pass writes its split and the split of W itself, which dx_gemm reads
+    if (x3) {
+      PhaseTimer pt(e, PH_SPLIT, st);
+      int rcs = transpose_operand(e, st, e->theta.W, K, D, (size_t)K, e->ws.WT, true, e->ws.WT_lo, wsp<float>(e, e->ws.W_hi),
+                                  wsp<float>(e, e->ws.W_lo));
+      if (rcs) return rcs;
+    }
     PhaseTimer pt(e, PH_CTX_FWD, st);
+    if (!x3) { int rcs = transpose_operand(e, st, e->theta.W, K, D, (size_t)K, e->ws.WT, false); if (rcs) return rcs; }
     umma::Operand opA{Xg, (size_t)K, false, x3 ? wsp<float>(e, e->ws.Xg_lo) : nullptr};
-    umma::Operand opB{x3 ? wsp<float>(e, e->ws.W_hi) : e->theta.W, (size_t)D, true, x3 ? wsp<float>(e, e->ws.W_lo) : nullptr};
+    umma::Operand opB{wsp<float>(e, e->ws.WT), (size_t)K, false, x3 ? wsp<float>(e, e->ws.WT_lo) : nullptr};
     if (x3) {
       umma::EpiTanhStorePrecise ep{H, (size_t)D};
-      C2V_LAUNCH(e, C2V_CUDA(e, (umma::launch_cfg<false, true, umma::EpiTanhStorePrecise>(st, cs.rows, D, K, 1, opA, opB, ep, e->num_sms))));
+      C2V_LAUNCH(e, C2V_CUDA(e, (umma::launch_cfg<false, false, umma::EpiTanhStorePrecise>(st, cs.rows, D, K, 1, opA, opB, ep, e->num_sms))));
     } else {
       umma::EpiTanhStore ep{H, (size_t)D};
-      C2V_LAUNCH(e, C2V_CUDA(e, (umma::launch_cfg<false, true, umma::EpiTanhStore>(st, cs.rows, D, K, 1, opA, opB, ep, e->num_sms))));
+      C2V_LAUNCH(e, C2V_CUDA(e, (umma::launch_cfg<false, false, umma::EpiTanhStore>(st, cs.rows, D, K, 1, opA, opB, ep, e->num_sms))));
     }
     return C2V_OK;
   }
@@ -757,20 +805,24 @@ struct LogitsArgs {
   umma::SoftmaxGradArgs sg;
 };
 
+// for_dv: a dv GEMM of this step follows, so Ytab^T is made here (transpose_table), before the GEMM and from the same table
 template <bool X3>
-int launch_logits(c2v_engine* e, cudaStream_t st, const float* v, int B, LogitsOut out, const LogitsArgs& a) {
+int launch_logits(c2v_engine* e, cudaStream_t st, const float* v, int B, LogitsOut out, const LogitsArgs& a, bool for_dv) {
   const int D = e->dims.code_dim, Y = e->dims.target_vocab;
   umma::Operand opA{v, (size_t)D, false};
   umma::Operand opB{e->theta.tgt, (size_t)D, false};
+  int rcs;
   if (X3) {      // fp32-faithful: both operands as tf32 (hi, lo) pairs; the gated fallback reuses the previous pass's splits
-    int rcs;
     if (out != LOGITS_STORE_LSE_GATED) {
       if ((rcs = split_small(e, st, v, (size_t)B * D, e->ws.v_hi, e->ws.v_lo))) return rcs;
-      if ((rcs = split_small(e, st, e->theta.tgt, (size_t)Y * D, e->ws.tgt_hi, e->ws.tgt_lo))) return rcs;
+      if (for_dv) rcs = transpose_table(e, st, true);
+      else rcs = split_small(e, st, e->theta.tgt, (size_t)Y * D, e->ws.tgt_hi, e->ws.tgt_lo);
+      if (rcs) return rcs;
     }
-    e->tgt_split_valid = true;
     opA.base = wsp<float>(e, e->ws.v_hi); opA.lo = wsp<float>(e, e->ws.v_lo);
     opB.base = wsp<float>(e, e->ws.tgt_hi); opB.lo = wsp<float>(e, e->ws.tgt_lo);
+  } else if (for_dv && (rcs = transpose_table(e, st, false))) {
+    return rcs;
   }
   PhaseTimer pt(e, PH_LOGITS, st);
   float* S = wsp<float>(e, e->ws.S);
@@ -793,9 +845,10 @@ int launch_logits(c2v_engine* e, cudaStream_t st, const float* v, int B, LogitsO
   return C2V_OK;
 }
 
-int run_logits(c2v_engine* e, cudaStream_t st, const float* v, int B, LogitsOut out, const LogitsArgs& a = {}) {
+int run_logits(c2v_engine* e, cudaStream_t st, const float* v, int B, LogitsOut out, const LogitsArgs& a = {}, bool for_dv = false) {
   { int rcl = end_target_lazy(e, st); if (rcl) return rcl; }      // a pass over the whole table needs every row current
-  if (is_tc(e) && aligned16(v)) return is_3x(e) ? launch_logits<true>(e, st, v, B, out, a) : launch_logits<false>(e, st, v, B, out, a);
+  if (is_tc(e) && aligned16(v))
+    return is_3x(e) ? launch_logits<true>(e, st, v, B, out, a, for_dv) : launch_logits<false>(e, st, v, B, out, a, for_dv);
   const int D = e->dims.code_dim;
   PhaseTimer pt(e, PH_LOGITS, st);
   simt::RowsK al{v, (size_t)D};
@@ -971,16 +1024,14 @@ int run_dv(c2v_engine* e, cudaStream_t st, int B, float* dv, const SlabDesc& sla
   float* part = wsp<float>(e, e->ws.part);
   PhaseTimer pt(e, PH_DV, st);
   if (is_tc(e)) {
+    // B = Ytab^T, K-major, made by this step's logits pass (3xTF32: as the table's split; P was written as its split by
+    // softmax_grad_kernel)
+    if (!e->tgt_t_valid) { int rct = transpose_table(e, st, false); if (rct) return rct; }
     umma::Operand opA{S, e->ws.ldS, false};
-    umma::Operand opB{e->theta.tgt, (size_t)D, true};
-    if (is_3x(e)) {      // P was written as its split by softmax_grad_kernel; the table's split dates from the logits pass
-      if (!e->tgt_split_valid) {
-        int rcs = split_small(e, st, e->theta.tgt, (size_t)Y * D, e->ws.tgt_hi, e->ws.tgt_lo);
-        if (rcs) return rcs;
-        e->tgt_split_valid = true;
-      }
+    umma::Operand opB{wsp<float>(e, e->ws.tgtT), e->ws.ldS, false};
+    if (is_3x(e)) {
       opA.lo = wsp<float>(e, e->ws.S_lo);
-      opB.base = wsp<float>(e, e->ws.tgt_hi); opB.lo = wsp<float>(e, e->ws.tgt_lo);
+      opB.lo = wsp<float>(e, e->ws.tgtT_lo);
     }
     // enough split-K slices to fill the SMs about twice; few when the batch already gives many tiles
     const int tiles = ((B + umma::BM - 1) / umma::BM) * ((D + umma::BN - 1) / umma::BN);
@@ -990,7 +1041,7 @@ int run_dv(c2v_engine* e, cudaStream_t st, int B, float* dv, const SlabDesc& sla
     umma::EpiStore ep{part, (size_t)D, (size_t)B * D};
     if (slab.loaders) {       // A = the logits slab, turned into dL/dlogits by the GEMM's loaders
       umma::AXSoftmaxGrad<true> ax{slab.sg};
-      C2V_LAUNCH(e, C2V_CUDA(e, (umma::launch_cfg<false, true, umma::EpiStore, umma::AXSoftmaxGrad<true>>(st, B, D, Y, want, opA, opB, ep,
+      C2V_LAUNCH(e, C2V_CUDA(e, (umma::launch_cfg<false, false, umma::EpiStore, umma::AXSoftmaxGrad<true>>(st, B, D, Y, want, opA, opB, ep,
                                                                                                             e->num_sms, ax))));
     } else {
       C2V_LAUNCH(e, C2V_CUDA(e, (umma::launch(st, B, D, Y, want, opA, opB, ep, e->num_sms))));
@@ -1014,20 +1065,24 @@ int run_dy(c2v_engine* e, cudaStream_t st, const float* v, int B, const SlabDesc
     if (is_3x(e) && !aligned16(v))
       return fail(e, C2V_ERR_INVALID, "3xTF32: the code vectors must be 16-byte aligned");
     if (is_tc(e) && aligned16(v)) {
-      umma::Operand opA{S, e->ws.ldS, true};
-      umma::Operand opB{v, (size_t)D, true};
+      // A = S^T stays MN-major (a transposed copy of the slab would cost a write of its own size); B = v^T, K-major
+      const size_t ldB = align_up((size_t)B, 4);
+      int rcs;
       if (is_3x(e)) {
-        int rcs = split_small(e, st, v, (size_t)B * D, e->ws.v_hi, e->ws.v_lo);
-        if (rcs) return rcs;
-        opA.lo = wsp<float>(e, e->ws.S_lo);
-        opB.base = wsp<float>(e, e->ws.v_hi); opB.lo = wsp<float>(e, e->ws.v_lo);
+        PhaseTimer pts(e, PH_SPLIT, st);
+        rcs = transpose_operand(e, st, v, B, D, ldB, e->ws.vT, true, e->ws.vT_lo);
+      } else {
+        rcs = transpose_operand(e, st, v, B, D, ldB, e->ws.vT, false);
       }
+      if (rcs) return rcs;
+      umma::Operand opA{S, e->ws.ldS, true, is_3x(e) ? wsp<float>(e, e->ws.S_lo) : nullptr};
+      umma::Operand opB{wsp<float>(e, e->ws.vT), ldB, false, is_3x(e) ? wsp<float>(e, e->ws.vT_lo) : nullptr};
       auto go = [&](auto ep) -> int {
         if (slab.loaders)       // A = the logits slab, turned into dL/dlogits by the GEMM's loaders
-          C2V_LAUNCH(e, C2V_CUDA(e, (umma::launch_cfg<true, true, decltype(ep), umma::AXSoftmaxGrad<false>>(
+          C2V_LAUNCH(e, C2V_CUDA(e, (umma::launch_cfg<true, false, decltype(ep), umma::AXSoftmaxGrad<false>>(
                                         st, Y, D, B, 1, opA, opB, ep, e->num_sms, umma::AXSoftmaxGrad<false>{slab.sg}))));
         else
-          C2V_LAUNCH(e, C2V_CUDA(e, (umma::launch_cfg<true, true, decltype(ep)>(st, Y, D, B, 1, opA, opB, ep, e->num_sms))));
+          C2V_LAUNCH(e, C2V_CUDA(e, (umma::launch_cfg<true, false, decltype(ep)>(st, Y, D, B, 1, opA, opB, ep, e->num_sms))));
         return C2V_OK;
       };
       int rc;
@@ -1040,7 +1095,7 @@ int run_dy(c2v_engine* e, cudaStream_t st, const float* v, int B, const SlabDesc
           return rc;
         e->tgt_armed = false;
         e->tgt_fused_t = e->tgt_t;
-        e->tgt_split_valid = false;
+        e->tgt_t_valid = false;
       } else if ((rc = go(umma::EpiStore{e->grad.tgt, (size_t)D, 0}))) {
         return rc;
       }
@@ -1136,7 +1191,7 @@ int exp_slab_logits(c2v_engine* e, cudaStream_t st, const float* v, int B, const
                                                                   B, tl, flag)));
     if (tl_out) C2V_CUDA(e, cudaMemcpyAsync(tl_out, tl, (size_t)B * 4, cudaMemcpyDeviceToDevice, st));
   }
-  if ((rc = run_logits(e, st, v, B, LOGITS_EXP_SUM, LogitsArgs{tl}))) return rc;
+  if ((rc = run_logits(e, st, v, B, LOGITS_EXP_SUM, LogitsArgs{tl}, true))) return rc;
   {
     PhaseTimer pt(e, PH_XENT, st);
     if ((rc = combine())) return rc;
@@ -1172,7 +1227,7 @@ int train_step_impl(c2v_engine* e, cudaStream_t st, const int32_t* src, const in
   if (hs == HEAD_RECOMPUTE) {
     // the slab is written ONCE, as dL/dlogits: pass 1 of the logits GEMM leaves only log-sum-exp partials, the true-class
     // logit comes from a B-row dot product, pass 2 repeats the product and its epilogue writes (softmax - onehot) / B
-    if ((rc = run_logits(e, st, v, B, LOGITS_LSE_ONLY))) return rc;
+    if ((rc = run_logits(e, st, v, B, LOGITS_LSE_ONLY, {}, true))) return rc;
     float* tl = wsp<float>(e, e->ws.true_logit);
     {
       PhaseTimer pt(e, PH_XENT, st);
@@ -1202,7 +1257,7 @@ int train_step_impl(c2v_engine* e, cudaStream_t st, const int32_t* src, const in
       C2V_LAUNCH(e, (loss_reduce_kernel<<<1, 256, 0, st>>>(loss_b, B, invB, loss_out)));
     }
   } else {
-    if ((rc = run_logits(e, st, v, B, hs == HEAD_SIMT ? LOGITS_STORE : LOGITS_STORE_LSE))) return rc;
+    if ((rc = run_logits(e, st, v, B, hs == HEAD_SIMT ? LOGITS_STORE : LOGITS_STORE_LSE, {}, true))) return rc;
     PhaseTimer pt(e, PH_XENT, st);
     if (hs == HEAD_SIMT) {
       C2V_LAUNCH(e, (xent_kernel<<<B, kXentThreads, 0, st>>>(S, e->ws.ldS, target, Y, invB, loss_b, lse, 1)));
@@ -1327,7 +1382,7 @@ int adam_impl(c2v_engine* e, cudaStream_t st, float lr, float b1, float b2, floa
     first_dense = 2;
   }
   e->adam_t_done = t;
-  e->tgt_split_valid = false;
+  e->tgt_t_valid = false;
   if (e->lazy) { int rcs = sweep_rows(e, st, t); if (rcs) return rcs; }
   for (int i = first_dense; i < 5; ++i) {
     if (i == 2 && (skip_tgt || e->tgt_lazy)) continue;     // lazy target rows: deferred like the embedding rows
@@ -1471,6 +1526,7 @@ int c2v_set_option(c2v_engine* e, const char* key, int64_t value) {
     if (value != C2V_MATH_FP32 && !umma::get_encode_fn())
       return fail(e, C2V_ERR_UNSUPPORTED, "cuTensorMapEncodeTiled not available from the driver");
     e->math_mode = (int)value;
+    e->tgt_t_valid = false;      // ws.tgtT holds the table (tf32) or its high parts (3xTF32)
     return C2V_OK;
   }
   if (!strcmp(key, "deterministic")) {
@@ -1859,7 +1915,7 @@ int c2v_target_forward(c2v_engine* e, const float* code_all, int32_t Bt, const i
     return C2V_OK;
   }
   const bool fused = hs == HEAD_TWO_PASS;
-  if ((rc = run_logits(e, st, code_all, Bt, fused ? LOGITS_STORE_LSE : LOGITS_STORE))) return rc;
+  if ((rc = run_logits(e, st, code_all, Bt, fused ? LOGITS_STORE_LSE : LOGITS_STORE, {}, true))) return rc;
   PhaseTimer pt(e, PH_XENT, st);
   C2V_LAUNCH(e, (row_maxsum_kernel<<<Bt, 256, 0, st>>>(fused ? part : nullptr, n_tiles, S, e->ws.ldS, Y, target, row_offset, row_max,
                                                        row_sum, true_logit)));
@@ -2084,6 +2140,18 @@ int c2v_selftest_split(c2v_engine* e, const float* x, float* hi, float* lo, size
   if (blocks > (size_t)e->num_sms * 16) blocks = (size_t)e->num_sms * 16;
   if (blocks < 1) blocks = 1;
   C2V_LAUNCH(e, (split_tf32_kernel<<<(unsigned)blocks, 256, 0, (cudaStream_t)stream>>>(x, hi, lo, count / 4)));
+  return C2V_OK;
+}
+
+int c2v_selftest_transpose(c2v_engine* e, const float* x, int32_t rows, int32_t cols, float* xT, float* xT_lo, size_t ldT,
+                           void* stream) {
+  if (!e || !x || !xT) return C2V_ERR_INVALID;
+  if (rows < 1 || cols < 1 || ldT < (size_t)rows || cols > 65535 * 32) return fail(e, C2V_ERR_INVALID, "bad size");
+  C2V_CUDA(e, cudaSetDevice(e->device));
+  const dim3 grid((unsigned)((rows + 31) / 32), (unsigned)((cols + 31) / 32));
+  cudaStream_t st = (cudaStream_t)stream;
+  if (xT_lo) C2V_LAUNCH(e, (transpose_kernel<true><<<grid, 256, 0, st>>>(x, rows, cols, xT, xT_lo, ldT, nullptr, nullptr)));
+  else C2V_LAUNCH(e, (transpose_kernel<false><<<grid, 256, 0, st>>>(x, rows, cols, xT, nullptr, ldT, nullptr, nullptr)));
   return C2V_OK;
 }
 

@@ -473,6 +473,46 @@ split_tf32_kernel(const float* __restrict__ x, float* __restrict__ hi, float* __
   }
 }
 
+// xT[c, r] = x[r, c]: x is [rows, cols] row-major (pitch cols), xT is [cols, ldT].  Makes the K-major copy of a GEMM operand
+// that is stored MN-major (TRANSFORM, the code vectors, the target table), so the GEMM reads it by TMA without transposing it in
+// shared memory once per work item.  SPLIT (3xTF32): xT / xT_lo receive the transposed tf32 split, and hi / lo, when given, the
+// untransposed one (x's layout, as split_tf32_kernel writes it).  Columns [rows, ldT) of xT are not written.  32 x 32 tiles,
+// grid (ceil(rows / 32), ceil(cols / 32)).
+template <bool SPLIT>
+__global__ void __launch_bounds__(256)
+transpose_kernel(const float* __restrict__ x, int rows, int cols, float* __restrict__ xT, float* __restrict__ xT_lo, size_t ldT,
+                 float* __restrict__ hi, float* __restrict__ lo) {
+  __shared__ float th[32][33];
+  __shared__ float tl[SPLIT ? 32 : 1][33];
+  const int r0 = blockIdx.x * 32, c0 = blockIdx.y * 32;
+  const int tx = threadIdx.x & 31, ty = threadIdx.x >> 5;
+#pragma unroll
+  for (int i = ty; i < 32; i += 8) {
+    const int r = r0 + i, c = c0 + tx;
+    if (r >= rows || c >= cols) continue;
+    const size_t at = (size_t)r * cols + c;
+    const float v = x[at];
+    if constexpr (SPLIT) {
+      float h, l;
+      split_tf32(v, h, l);
+      if (hi) { hi[at] = h; lo[at] = l; }
+      th[i][tx] = h;
+      tl[i][tx] = l;
+    } else {
+      th[i][tx] = v;
+    }
+  }
+  __syncthreads();
+#pragma unroll
+  for (int i = ty; i < 32; i += 8) {
+    const int c = c0 + i, r = r0 + tx;
+    if (r >= rows || c >= cols) continue;
+    const size_t at = (size_t)c * ldT + r;
+    xT[at] = th[tx][i];
+    if constexpr (SPLIT) xT_lo[at] = tl[tx][i];
+  }
+}
+
 // ---------------------------------------------------------------------------------------------
 // Sampled softmax (BASELINE config 3; NOT in the reference, definition in DESIGN.md section 5 after
 // tf.nn.sampled_softmax_loss): logits over {target_b} U sampled[0..S) minus log expected counts,

@@ -89,6 +89,7 @@ _SIGNATURES = {
     "c2v_selftest_gemm3": (C.c_int, [_P, _I32, _I32, _I32, _I32, _I32, _I32, _I32, _P, _P, C.c_size_t, _P, _P, C.c_size_t,
                                      _P, C.c_size_t, _P]),
     "c2v_selftest_split": (C.c_int, [_P, _P, _P, _P, C.c_size_t, _P]),
+    "c2v_selftest_transpose": (C.c_int, [_P, _P, _I32, _I32, _P, _P, C.c_size_t, _P]),
     "c2v_selftest_row_sum": (C.c_int, [_P, _I32, _P, _P, _I32, _P, _P]),
     "c2v_set_event": (C.c_int, [_P, C.c_char_p, _P]),
     "c2v_sync_tables": (C.c_int, [_P, _P]),
@@ -287,6 +288,15 @@ class PathAttentionEngine:
         hi, lo = self.torch.empty_like(x), self.torch.empty_like(x)
         self._check(self.lib.c2v_selftest_split(self.h, x.data_ptr(), hi.data_ptr(), lo.data_ptr(), x.numel(), self._stream()))
         return hi, lo
+
+    def selftest_transpose(self, x, ld_t: int, split: bool = False):
+        """Test hook: the K-major copy [cols, ld_t] the engine makes of a row-major [rows, cols] operand (c2v_selftest_transpose);
+        with split, the transposed 3xTF32 split -> (hi, lo).  Columns rows .. ld_t-1 are left as torch.empty made them."""
+        rows, cols = x.shape
+        out = [self.torch.empty((cols, ld_t), dtype=x.dtype, device=x.device) for _ in range(2 if split else 1)]
+        self._check(self.lib.c2v_selftest_transpose(self.h, x.data_ptr(), rows, cols, out[0].data_ptr(),
+                                                    out[1].data_ptr() if split else None, ld_t, self._stream()))
+        return tuple(out) if split else out[0]
 
     def selftest_gemm(self, A, B, a_mn: bool, b_mn: bool, M: int, N: int, K: int, bn: int = 192, splits: int = 1,
                       three: bool = False):

@@ -373,6 +373,12 @@ int c2v_selftest_gemm3(c2v_engine* e, int32_t a_mn, int32_t b_mn, int32_t bn, in
                        void* stream);
 int c2v_selftest_split(c2v_engine* e, const float* x, float* hi, float* lo, size_t count, void* stream);
 
+/* Test hook for the K-major copies the engine makes of its MN-major GEMM operands: xT[c, r] = x[r, c] for a row-major
+ * x [rows, cols] (pitch cols) into xT [cols, ldT] (ldT >= rows; columns rows .. ldT-1 are not written).  With xT_lo
+ * non-NULL, xT / xT_lo receive the transposed 3xTF32 split of x instead.  Device pointers. */
+int c2v_selftest_transpose(c2v_engine* e, const float* x, int32_t rows, int32_t cols, float* xT, float* xT_lo, size_t ldT,
+                           void* stream);
+
 /* Test hook for option "deterministic": the sort + chunked reduce of a train step's embedding-gradient scatter, on
  * `count` caller-given contributions instead of dX' (no dropout, no scaling): row rows[i] of table table_id (0 = token
  * table [T, d], 1 = path table [P, d]; d = embed_dim) receives vals[i, 0:d], summed in the order the option documents,
