@@ -1837,6 +1837,9 @@ int c2v_apply_scatter_inbox(c2v_engine* e, void* stream) {
   PhaseTimer pt(e, PH_INBOX_APPLY, st);
   C2V_LAUNCH(e, (inbox_apply_kernel<<<e->num_sms * 8, 256, 0, st>>>(e->inbox, e->dims.embed_dim, e->gr_tok.base[e->inbox.rank],
                                                                     e->gr_path.base[e->inbox.rank])));
+  // the fold consumes the rows: a step that pushes nothing (the fp32 scatter red.adds straight into the shards) leaves
+  // zero counts, so the next fold cannot add the previous step's rows a second time
+  C2V_CUDA(e, cudaMemsetAsync(e->inbox.base[e->inbox.rank], 0, (size_t)e->inbox.world * 2 * 4, st));
   return C2V_OK;
 }
 

@@ -121,8 +121,15 @@ def make_fully_sharded_engine(dims, local_batch: int, device: int, group=None, t
     from dataclasses import replace
     dist = _dist()
     world, rank = dist.get_world_size(group), dist.get_rank(group)
+    # the last rank's block is the smallest: when it is empty, some rank has no target rows, and an engine needs at
+    # least one, whose logit would then enter every example's normaliser.  Every rank refuses alike.
+    last0, last1 = target_row_block(dims.target_vocab, world - 1, world)
+    if last1 <= last0:
+        per = (dims.target_vocab + world - 1) // world
+        raise ValueError("fully_sharded: %d target rows in blocks of %d leave ranks %d..%d of %d without a row"
+                         % (dims.target_vocab, per, -(-dims.target_vocab // per), world - 1, world))
     row0, row1 = target_row_block(dims.target_vocab, rank, world)
-    local = replace(dims, target_vocab=max(row1 - row0, 1), max_batch=local_batch * world)
+    local = replace(dims, target_vocab=row1 - row0, max_batch=local_batch * world)
     eng = PathAttentionEngine(local, device=device, training=training)
     eng.global_target_vocab, eng.target_row0, eng.local_batch = dims.target_vocab, row0, local_batch
     return eng

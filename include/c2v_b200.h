@@ -307,7 +307,8 @@ int c2v_bind_table_shards(c2v_engine* e, const c2v_table_shards* params, const c
  * the backward pass no longer issues 16-byte red.global.add over NVLink: it sorts its 3 B C gradient rows by owning
  * rank and writes each owner's rows -- (local row id, d floats) -- DENSELY into its region of that owner's inbox with
  * plain coalesced stores; after the caller's cross-rank barrier (the same one that ordered the remote red.adds before)
- * each owner folds its inbox into its own gradient shards with local atomics (c2v_apply_scatter_inbox).
+ * each owner folds its inbox into its own gradient shards with local atomics (c2v_apply_scatter_inbox).  The fold
+ * consumes the inbox: a step that pushed nothing (fp32 red.adds straight into the shards) then folds nothing.
  * inbox[r] = rank r's inbox as mapped into this process (r == rank: the local allocation). */
 size_t c2v_scatter_inbox_bytes(const c2v_dims* dims, int32_t world);
 int c2v_bind_scatter_inbox(c2v_engine* e, void* const* inbox, int32_t world, int32_t rank);
