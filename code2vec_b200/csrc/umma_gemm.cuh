@@ -1,7 +1,7 @@
 // Hopper (sm_90a) tensor-core GEMM:  C[M,N] = A[M,K] . B[K,N],  fp32 storage, tf32 operands (10-bit
 // mantissa), fp32 accumulation in registers  (C2V_MATH_TF32; C2V_MATH_3XTF32 issues three products).
 //
-// Persistent, warp-specialised, one CTA of three warpgroups per SM:
+// Persistent, warp-specialised, one CTA of four warpgroups per SM:
 //   warpgroup 0     : producer -- fills a 4-stage shared-memory ring.  Operands arrive by TMA
 //                     (cp.async.bulk.tensor, 128-byte swizzle, issued by one thread).  wgmma takes 32-bit
 //                     (tf32) operands K-major only, so an MN-major operand lands as four 32 x 32 boxes that
@@ -10,10 +10,17 @@
 //                     tile (softmax gradient of a logits tile, embedding gather).
 //   warpgroups 1, 2 : consumers -- each owns 64 rows of the 128-row tile and issues
 //                     wgmma.mma_async m64n128k8 (tf32) into a 64-register accumulator per thread;
-//                     then the fused epilogue (store / tanh / log-sum-exp partials / split-K slice / Adam).
+//                     then writes the accumulator to its shared-memory staging blocks and goes on to its
+//                     next tile.
+//   warpgroup 3     : epilogue -- drains each staged tile through the fused epilogue (store / tanh /
+//                     log-sum-exp partials / split-K slice / Adam) while the consumers run the next tile's
+//                     MMAs, so a tile costs the longer of the two rather than their sum.
 // Every stage is published by an mbarrier (K-major TMA transaction bytes + one arrival per producer thread;
 // MN-major boxes report to a second, per-stage "landed" barrier that the transposing warps wait on) and
-// released by one arrival per consumer warp once the wgmma group that read it has retired.
+// released by one arrival per consumer warp once the wgmma group that read it has retired.  The staging
+// blocks are handed over by two more: epi_full (every consumer thread has written its accumulator) and
+// epi_empty (every epilogue thread is done with the blocks).  setmaxnreg moves registers from the producer,
+// which holds no accumulator, to the epilogue (not for the plain store, which does not need them).
 // Out-of-range rows / K-tail are zero-filled (by TMA or by the loaders), so any M, N, K work; split-K
 // over blockIdx-independent work items.  Every operand needs a 16-byte aligned base and a row pitch that is a
 // multiple of 4 floats (operand_ok).
@@ -32,7 +39,14 @@ constexpr int BN = 128;          // columns of a tile: wgmma N
 constexpr int BK = 32;           // fp32 elements per stage along K = one 128-byte swizzle row
 constexpr int WG_K = 8;          // K per wgmma for 32-bit operands (32 bytes)
 constexpr int STAGES = 4;
-constexpr int kThreads = 3 * 128;
+constexpr int kThreads = 4 * 128;
+// Registers per thread of each role.  The CTA starts with 128 per thread (64 K for 512 threads, the whole register
+// file); the producer then gives some up to the epilogue, 1 x kRegsProducer + 2 x kRegsConsumer + 1 x kRegsEpilogue
+// = 4 x 128, unless the epilogue functor sets kMoveRegs = false (EpiStore).
+constexpr int kRegsProducer = 72;
+constexpr int kRegsConsumer = 128;
+constexpr int kRegsEpilogue = 184;
+static_assert(kRegsProducer + 2 * kRegsConsumer + kRegsEpilogue == 4 * 128, "the roles share the CTA's registers");
 
 // fast transcendental forms for the tensor-core path (operands are already tf32-rounded):
 // exp via ex2.approx (rel. error 2^-22), tanh(x) = 1 - 2 / (exp(2x) + 1) (abs. error ~1e-7).
@@ -67,16 +81,23 @@ __device__ __forceinline__ bool mbar_try_wait(uint64_t* bar, uint32_t parity) {
       : "=r"(ok) : "r"(smem_u32(bar)), "r"(parity) : "memory");
   return ok != 0;
 }
-// Bounded wait: a pipeline bug traps (reported as a CUDA error) instead of hanging the GPU.
+// Bounded wait: a pipeline bug traps (reported as a CUDA error) instead of hanging the GPU.  SLEEP: between polls the
+// warp sleeps, 32 ns at first and at most 256 ns -- for waits that can last a whole main loop (the epilogue warpgroup's
+// on epi_full), so that the polling warps take no issue slots from the warps doing the work.
+template <bool SLEEP = false>
 __device__ __forceinline__ void mbar_wait(uint64_t* bar, uint32_t parity) {
   if (mbar_try_wait(bar, parity)) return;
   const long long t0 = clock64();
+  uint32_t ns = 32;
   while (!mbar_try_wait(bar, parity)) {
+    if (SLEEP) {
+      __nanosleep(ns);
+      if (ns < 256) ns *= 2;
+    }
     if (clock64() - t0 > 20000000000LL) __trap();     // ~10 s at 2 GHz
   }
 }
 __device__ __forceinline__ void fence_proxy_async_smem() { asm volatile("fence.proxy.async.shared::cta;" ::: "memory"); }
-__device__ __forceinline__ void wg_bar_sync(int id) { asm volatile("bar.sync %0, 128;" ::"r"(id) : "memory"); }
 
 // ---- TMA ----------------------------------------------------------------------------------------
 __device__ __forceinline__ void tma_load_2d(void* smem_dst, const CUtensorMap* map, uint64_t* bar, int c0, int c1) {
@@ -98,6 +119,11 @@ __device__ __forceinline__ void wg_fence() { asm volatile("wgmma.fence.sync.alig
 __device__ __forceinline__ void wg_commit() { asm volatile("wgmma.commit_group.sync.aligned;" ::: "memory"); }
 template <int N>
 __device__ __forceinline__ void wg_wait() { asm volatile("wgmma.wait_group.sync.aligned %0;" ::"n"(N) : "memory"); }
+// per-thread register budget of the executing warpgroup (all 128 threads): release / acquire down / up to R
+template <int R>
+__device__ __forceinline__ void wg_regs_dec() { asm volatile("setmaxnreg.dec.sync.aligned.u32 %0;" ::"n"(R)); }
+template <int R>
+__device__ __forceinline__ void wg_regs_inc() { asm volatile("setmaxnreg.inc.sync.aligned.u32 %0;" ::"n"(R)); }
 // D[64 x 128] (+)= A[64 x 8] . B[8 x 128]; thread (warp w, lane l) holds rows 16w + l/4 (+8), columns 8j + 2(l%4) (+1)
 // in d[4j + 2i + c] (row + 8i, column + c)
 __device__ __forceinline__ void wgmma_tf32(float (&d)[64], uint64_t da, uint64_t db, uint32_t accumulate) {
@@ -146,6 +172,9 @@ struct EpiStore {
   __device__ __forceinline__ float* out(int split) const { return C + (size_t)split * split_stride; }
   using Pre = EpiNoState;
   static constexpr int kRowBatch = 8;
+  // A plain store needs no more than the 128 registers every role starts with; moving registers to the epilogue
+  // warpgroup (setmaxnreg) made the long-K GEMM that uses this epilogue (dv: 743 K blocks per work item) 15 % slower.
+  static constexpr bool kMoveRegs = false;
   __device__ __forceinline__ void prefetch(const float*, size_t, Pre&) const {}
   __device__ __forceinline__ void store4(float* c, size_t off, float4 v, const Pre&) const { *reinterpret_cast<float4*>(c + off) = v; }
   __device__ __forceinline__ void store1(float* c, size_t off, float x) const { c[off] = x; }
@@ -411,7 +440,9 @@ struct EpiAdam {
     }
   }
   struct Pre { float4 p, m, v; };
-  static constexpr int kRowBatch = 2;            // more rows in flight spill registers at the 168-register cap of the GEMM
+  // rows whose (theta, m, v) loads are in flight together per thread; the epilogue warpgroup's kRegsEpilogue registers
+  // hold them without spilling
+  static constexpr int kRowBatch = 4;
   __device__ __forceinline__ void prefetch(const float* c, size_t off, Pre& q) const {
     q.p = *reinterpret_cast<const float4*>(c + off);
     q.m = *reinterpret_cast<const float4*>(Mo + off);
@@ -454,6 +485,10 @@ __device__ __forceinline__ auto epi_prefetch_tile(const Epi& epi, int m, int n0,
 template <class Epi>
 __device__ __forceinline__ void epi_prefetch_tile(const Epi&, int, int, int, int, int, long) {}
 template <class Epi>
+constexpr bool epi_move_regs(...) { return true; }
+template <class Epi, bool V = Epi::kMoveRegs>
+constexpr bool epi_move_regs(int) { return V; }
+template <class Epi>
 constexpr bool epi_stores(...) { return true; }
 template <class Epi, bool V = Epi::kStores>
 constexpr bool epi_stores(int) { return V; }
@@ -473,6 +508,7 @@ __device__ __forceinline__ void store_chunk(const Epi& epi, const typename Epi::
   const int gn = n + col4 * 4;
   // two passes per batch of rows so that a read-modify-write epilogue has kBatch rows' loads in flight
   constexpr int kBatch = Epi::kRowBatch;
+  static_assert(8 % kBatch == 0, "the batches tile the chunk's 8 row groups: a remainder would reach into the next block");
 #pragma unroll
   for (int it0 = 0; it0 < 8; it0 += kBatch) {
     float4 v[kBatch];
@@ -670,8 +706,9 @@ struct SmemLayout {
   static constexpr int kEpiOffset = STAGES * kStageBytes;                     // per consumer warpgroup: 64 x BN fp32
   static constexpr int kEpiBytes = 64 * BN * 4;
   static constexpr int kBarOffset = kEpiOffset + 2 * kEpiBytes;
-  static constexpr int kTotal = kBarOffset + 256 + 1024;   // barriers (full, empty, landed per stage), + slack for 1024-B alignment
-  static_assert(3 * STAGES * 8 <= 256, "the barriers fit their block");
+  // barriers (full, empty, landed per stage; epi_full, epi_empty), + slack for 1024-B alignment
+  static constexpr int kTotal = kBarOffset + 256 + 1024;
+  static_assert((3 * STAGES + 2) * 8 <= 256, "the barriers fit their block");
   static_assert(kTotal <= 232448, "exceeds the 227 KB of shared memory a CTA can opt into");
 };
 
@@ -697,6 +734,8 @@ umma_gemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant_
   uint64_t* full_bar = reinterpret_cast<uint64_t*>(smem + L::kBarOffset);     // the stage is ready for the MMA
   uint64_t* empty_bar = full_bar + STAGES;                                     // the MMA has read the stage
   uint64_t* landed_bar = empty_bar + STAGES;                                   // the MN-major boxes have landed
+  uint64_t* epi_full = landed_bar + STAGES;                                    // the staging blocks hold a tile
+  uint64_t* epi_empty = epi_full + 1;                                          // the epilogue is done with them
 
   const int wg = threadIdx.x >> 7, warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
   const int total_items = gs.m_tiles * gs.n_tiles * gs.splits;
@@ -704,6 +743,8 @@ umma_gemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant_
 
   if (threadIdx.x == 0) {
     for (int s = 0; s < STAGES; ++s) { mbar_init(&full_bar[s], 128); mbar_init(&empty_bar[s], 8); mbar_init(&landed_bar[s], 1); }
+    mbar_init(epi_full, 256);
+    mbar_init(epi_empty, 128);
     asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
   }
   __syncthreads();
@@ -724,6 +765,7 @@ umma_gemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant_
 
   if (wg == 0) {
     // ===================== producer warpgroup =====================
+    if constexpr (epi_move_regs<Epi>(0)) wg_regs_dec<kRegsProducer>();
     const int t = threadIdx.x;
     // The step sequence the consumers run: work items; per item, 3xTF32's three passes -- the two small cross terms
     // (A_lo.B_hi, A_hi.B_lo) over the whole K range first, then A_hi.B_hi (while only the 2^-11-sized cross terms have
@@ -818,24 +860,19 @@ umma_gemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant_
         if (ahead > kLag || !more) { complete(tr); next(tr); --ahead; }
       }
     }
-  } else {
+  } else if (wg <= 2) {
     // ===================== consumer warpgroups: rows 64 (wg - 1) .. of the tile =====================
     const int cw = wg - 1, wl = warp & 3;
-    float* stg = reinterpret_cast<float*>(smem + L::kEpiOffset + cw * L::kEpiBytes);    // 8 blocks of 32 x 32
+    const int g = lane >> 2;      // this thread's rows of the accumulator: 16 wl + g (+ 8); columns 8 j + 2 (lane % 4) (+ 1)
+    // staging: 8 blocks of 32 x 32 fp32 (row half, column quarter), 1024-byte aligned
+    const uint32_t stg_row = smem_u32(smem + L::kEpiOffset + cw * L::kEpiBytes) + (wl >> 1) * 4096 + (16 * (wl & 1) + g) * 128 +
+                             ((g ^ ((lane >> 1) & 1)) << 4) + 8 * (lane & 1);
     int stage = 0;
-    uint32_t phase = 0;
+    uint32_t phase = 0, epi_phase = 0;
     float acc[64];
-    auto prefetch_item = [&](int it) {            // read-modify-write epilogues: warm L2 with the tile's destination lines
-      if (it >= total_items || (wl >> 1)) return;
-      int mt2, nt2, sp2;
-      decode(it, mt2, nt2, sp2);
-      epi_prefetch_tile(epi, mt2 * BM + 64 * cw + 32 * (wl & 1) + lane, nt2 * BN, BN, gs.M, gs.N, 0);
-    };
-    prefetch_item(blockIdx.x);
-    for (int item = blockIdx.x; item < total_items; item += gridDim.x) {
+    for (int item = blockIdx.x; item < total_items; item += gridDim.x, epi_phase ^= 1) {
       int mt, nt, sp;
       decode(item, mt, nt, sp);
-      prefetch_item(item + gridDim.x);
       const int kb0 = sp * gs.kblocks_per_split;
       const int kb1 = min(total_kblocks, kb0 + gs.kblocks_per_split);
       const int n_steps = (kb1 - kb0) * gs.terms;          // 3xTF32: three passes over the K range (see the producer)
@@ -857,45 +894,73 @@ umma_gemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant_
       wg_wait<0>();
       if (n_steps > 0 && lane == 0) mbar_arrive(&empty_bar[prev]);
 
-      // Epilogue.  The accumulator goes through shared memory (8 XOR-swizzled 32 x 32 blocks per warpgroup:
-      // block (row half, column quarter)) so that each thread then holds one row's 32 consecutive columns, the
-      // layout the functors' row-wise math and store_chunk's coalesced stores work on.  Warp wl drains row half
-      // wl & 1, column quarters wl >> 1 and (wl >> 1) + 2.
-      wg_bar_sync(1 + cw);                                  // the previous tile's epilogue has read its blocks
+      // Hand the tile to the epilogue warpgroup and go on to the next one.  The accumulator goes through shared
+      // memory (8 XOR-swizzled 32 x 32 blocks per consumer: block (row half, column quarter)) so that an epilogue
+      // thread then holds one row's 32 consecutive columns, the layout the functors' row-wise math and
+      // store_chunk's coalesced stores work on.  The epilogue of this tile runs next to the MMAs of the next
+      // one, which is only sound because no GEMM reads in its main loop what its epilogue writes: dY reads S and
+      // v^T and updates (theta, m, v) of the target table, logits reads Ytab (or its tf32 split) and writes the
+      // slab and the partials, and the other GEMMs write outputs that are none of their operands.
+      // Element (row r, column cc) goes to block (r / 32, cc / 32), row r % 32, 16-byte chunk (cc % 32 / 4) ^ (r % 8).
+      // For this thread's rows 16 wl + lane / 4 (+ 8 i) and columns 8 j + 2 (lane % 4) that is byte
+      // (stg_row ^ ((j % 4) << 5)) + 8192 (j / 4) + 1024 i: written so, the 32 stores need four addresses, not 32
+      // loop-invariant ones.
+      mbar_wait(epi_empty, epi_phase ^ 1);                  // the epilogue is done with the previous tile's blocks
 #pragma unroll
       for (int j = 0; j < BN / 8; ++j) {
 #pragma unroll
-        for (int i = 0; i < 2; ++i) {
-          const int r = 16 * wl + (lane >> 2) + 8 * i, cc = 8 * j + 2 * (lane & 3);
-          const int b = (r >> 5) | ((cc >> 5) << 1), rr = r & 31, c32 = cc & 31;
-          *reinterpret_cast<float2*>(stg + b * 1024 + rr * 32 + (((c32 >> 2) ^ (rr & 7)) << 2) + (c32 & 3)) =
-              make_float2(acc[4 * j + 2 * i], acc[4 * j + 2 * i + 1]);
-        }
+        for (int i = 0; i < 2; ++i)
+          asm volatile("st.shared.v2.f32 [%0], {%1, %2};" ::"r"((stg_row ^ ((j & 3) << 5)) + 8192 * (j >> 2) + 1024 * i),
+                       "f"(acc[4 * j + 2 * i]), "f"(acc[4 * j + 2 * i + 1]) : "memory");
       }
-      wg_bar_sync(1 + cw);
-      const int m_base = mt * BM + 64 * cw + 32 * (wl & 1), m = m_base + lane;
+      mbar_arrive(epi_full);
+    }
+  } else {
+    // ===================== epilogue warpgroup: warp w drains rows 32w .. 32w+31 of the tile =====================
+    // i.e. row half w & 1 of consumer w >> 1, all four column quarters.  The (max, sum) partial of slot 2 nt + p
+    // takes column quarters p and p + 2, in that order.
+    if constexpr (epi_move_regs<Epi>(0)) wg_regs_inc<kRegsEpilogue>();
+    const int w = warp & 3;
+    float* stg = reinterpret_cast<float*>(smem + L::kEpiOffset + (w >> 1) * L::kEpiBytes);
+    auto prefetch_item = [&](int it) {            // read-modify-write epilogues: warm L2 with the tile's destination lines
+      if (it >= total_items) return;
+      int mt2, nt2, sp2;
+      decode(it, mt2, nt2, sp2);
+      epi_prefetch_tile(epi, mt2 * BM + 32 * w + lane, nt2 * BN, BN, gs.M, gs.N, 0);
+    };
+    prefetch_item(blockIdx.x);
+    uint32_t epi_phase = 0;
+    for (int item = blockIdx.x; item < total_items; item += gridDim.x, epi_phase ^= 1) {
+      int mt, nt, sp;
+      decode(item, mt, nt, sp);
+      prefetch_item(item + gridDim.x);
+      mbar_wait<true>(epi_full, epi_phase);
+      const int m_base = mt * BM + 32 * w, m = m_base + lane;
       float* cbase = epi.out(sp);
-      typename Epi::State est;
-      epi.begin(est);
 #pragma unroll 1
-      for (int qq = 0; qq < 2; ++qq) {
-        const int q = (wl >> 1) + 2 * qq;
-        float* blk = stg + ((wl & 1) | (q << 1)) * 1024;
-        uint32_t r[32];
+      for (int p = 0; p < 2; ++p) {
+        typename Epi::State est;
+        epi.begin(est);
+#pragma unroll 1
+        for (int q = p; q < 4; q += 2) {
+          float* blk = stg + ((w & 1) | (q << 1)) * 1024;
+          uint32_t r[32];
 #pragma unroll
-        for (int c4 = 0; c4 < 8; ++c4) {
-          const float4 x = *reinterpret_cast<const float4*>(blk + lane * 32 + ((c4 ^ (lane & 7)) << 2));
-          r[4 * c4] = __float_as_uint(x.x); r[4 * c4 + 1] = __float_as_uint(x.y);
-          r[4 * c4 + 2] = __float_as_uint(x.z); r[4 * c4 + 3] = __float_as_uint(x.w);
+          for (int c4 = 0; c4 < 8; ++c4) {
+            const float4 x = *reinterpret_cast<const float4*>(blk + lane * 32 + ((c4 ^ (lane & 7)) << 2));
+            r[4 * c4] = __float_as_uint(x.x); r[4 * c4 + 1] = __float_as_uint(x.y);
+            r[4 * c4 + 2] = __float_as_uint(x.z); r[4 * c4 + 3] = __float_as_uint(x.w);
+          }
+          __syncwarp();
+          const int n = nt * BN + 32 * q;
+          if (n < gs.N) {
+            if (m < gs.M) epi.observe(m, n, r, gs.N - n, est);
+            if (epi_stores<Epi>(0)) store_chunk(epi, est, r, blk, lane, m_base, n, gs.M, gs.N, cbase, epi.ldc);
+          }
         }
-        __syncwarp();
-        const int n = nt * BN + 32 * q;
-        if (n < gs.N) {
-          if (m < gs.M) epi.observe(m, n, r, gs.N - n, est);
-          if (epi_stores<Epi>(0)) store_chunk(epi, est, r, blk, lane, m_base, n, gs.M, gs.N, cbase, epi.ldc);
-        }
+        epi.end(m, 2 * nt + p, sp, m < gs.M, est);
       }
-      epi.end(m, 2 * nt + (wl >> 1), sp, m < gs.M, est);
+      mbar_arrive(epi_empty);
     }
   }
 }
@@ -1027,7 +1092,7 @@ inline int effective_splits(int K, int splits) {
   return (total_kblocks + per - 1) / per;
 }
 
-// (max, sum exp) partial slots per logits row: one per (row, tile, column parity of the draining warps)
+// (max, sum exp) partial slots per logits row: one per (row, tile, parity of the tile's 32-column quarter)
 inline int lse_slots(int n) { return 2 * ((n + BN - 1) / BN); }
 
 // Runtime dispatch over operand majors.
