@@ -798,12 +798,27 @@ enum LogitsOut {
   LOGITS_SOFTMAX_GRAD,     // dL/dlogits = (softmax - onehot) * inv_batch, from the log-sum-exp in LogitsArgs::sg
   LOGITS_EXP_SUM,          // U = exp(s - LogitsArgs::exp_offset[row]) and (max U, sum U) partials
   LOGITS_STORE_LSE_GATED,  // as LOGITS_STORE_LSE while *LogitsArgs::gate != 0, else nothing (the exp_slab fallback)
+  LOGITS_TOPK,             // nothing: each (row, partial slot)'s best LogitsArgs::topk_k candidates (topk_candidates)
+  LOGITS_TOPK_LSE,         // the candidates and the partials
 };
 struct LogitsArgs {
   const float* exp_offset;
   const int* gate;
   umma::SoftmaxGradArgs sg;
+  int topk_k;
+  int row0;                // first global class of this engine's table (candidate ids)
 };
+
+// Candidate lists of the top-k epilogue in ws.S: values [B, lse_slots(Y), k], then the ids.  For k <= kTopkEpiMax that is
+// 2 x 4 x 16 x 2 ceil(Y / 128) <= 4 ldS bytes per row: the slab region holds them, and the workspace is unchanged.
+struct TopkCandidates {
+  float* val;
+  int32_t* idx;
+};
+inline TopkCandidates topk_candidates(c2v_engine* e, int B, int k) {
+  float* S = wsp<float>(e, e->ws.S);
+  return {S, reinterpret_cast<int32_t*>(S + (size_t)B * umma::lse_slots(e->dims.target_vocab) * k)};
+}
 
 // for_dv: a dv GEMM of this step follows, so Ytab^T is made here (transpose_table), before the GEMM and from the same table
 template <bool X3>
@@ -841,6 +856,12 @@ int launch_logits(c2v_engine* e, cudaStream_t st, const float* v, int B, LogitsO
       return go(umma::EpiSoftmaxGradT<X3, X3>{S, S_lo, ld, a.sg.lse, a.sg.target, a.sg.row0, a.sg.inv_batch, B});
     case LOGITS_EXP_SUM: return go(umma::EpiExpSumT<X3, X3>{S, S_lo, ld, a.exp_offset, lse.partial, lse.slots});
     case LOGITS_STORE_LSE_GATED: return go(umma::EpiStoreLseGatedT<X3>{lse, a.gate});
+    case LOGITS_TOPK:
+    case LOGITS_TOPK_LSE: {
+      const TopkCandidates c = topk_candidates(e, B, a.topk_k);
+      if (out == LOGITS_TOPK_LSE) return go(umma::EpiTopkT<X3, true>{lse, c.val, c.idx, a.topk_k, a.row0});
+      return go(umma::EpiTopkT<X3, false>{lse, c.val, c.idx, a.topk_k, a.row0});
+    }
   }
   return C2V_OK;
 }
@@ -883,6 +904,40 @@ int topk_impl(c2v_engine* e, cudaStream_t st, const float* code_vec, int B, int3
   else
     C2V_LAUNCH(e, (topk_iter_kernel<<<B, kTopkThreads, 0, st>>>(S, e->ws.ldS, Y, k, normalize, idx, val)));
   if (normalize == 2) C2V_LAUNCH(e, (topk_full_softmax_kernel<<<B, 256, 0, st>>>(S, e->ws.ldS, Y, k, val)));
+  return C2V_OK;
+}
+
+// This engine's best k rows (global ids row0 + local row) per example, raw logits, padded with (-inf, INT_MAX); with row_max /
+// row_sum, the (max, sum exp) of each example's logits over the local rows.  Tensor cores and k <= kTopkEpiMax: the logits
+// epilogue keeps per-(row, slot) candidate lists and topk_merge_kernel merges a row's slots, so no logit is stored.  fp32
+// (SIMT logits) and larger k: the logits slab, scanned by the kernels of c2v_topk.
+int topk_partial_impl(c2v_engine* e, cudaStream_t st, const float* code_all, int Bt, int row0, int k, int32_t* idx, float* val,
+                      float* row_max, float* row_sum) {
+  const int Y = e->dims.target_vocab;
+  const int slots = umma::lse_slots(Y);
+  float* S = wsp<float>(e, e->ws.S);
+  float2* part = wsp<float2>(e, e->ws.lse_part);
+  const bool stats = row_max != nullptr;
+  int rc;
+  if (is_tc(e) && aligned16(code_all) && k <= umma::kTopkEpiMax) {
+    LogitsArgs la{};
+    la.topk_k = k;
+    la.row0 = row0;
+    if ((rc = run_logits(e, st, code_all, Bt, stats ? LOGITS_TOPK_LSE : LOGITS_TOPK, la))) return rc;
+    PhaseTimer pt(e, PH_TOPK, st);
+    const TopkCandidates c = topk_candidates(e, Bt, k);
+    const TopkMergeArgs ma{c.idx, c.val, slots, (size_t)slots * k, (size_t)k, k, 0, nullptr, nullptr, 1, Bt, 0, idx, val};
+    C2V_LAUNCH(e, (topk_merge_kernel<umma::kTopkEpiMax><<<Bt, kTopkThreads, 0, st>>>(ma)));
+    if (stats) C2V_LAUNCH(e, (row_maxsum_kernel<<<Bt, 256, 0, st>>>(part, slots, S, e->ws.ldS, Y, nullptr, 0, row_max, row_sum, nullptr)));
+    return C2V_OK;
+  }
+  if ((rc = run_logits(e, st, code_all, Bt, LOGITS_STORE))) return rc;
+  PhaseTimer pt(e, PH_TOPK, st);
+  if (k <= 16)
+    C2V_LAUNCH(e, (topk_kernel<16><<<Bt, kTopkThreads, 0, st>>>(S, e->ws.ldS, Y, k, 0, idx, val, row0)));
+  else
+    C2V_LAUNCH(e, (topk_iter_kernel<<<Bt, kTopkThreads, 0, st>>>(S, e->ws.ldS, Y, k, 0, idx, val, row0)));
+  if (stats) C2V_LAUNCH(e, (row_maxsum_kernel<<<Bt, 256, 0, st>>>(nullptr, 0, S, e->ws.ldS, Y, nullptr, 0, row_max, row_sum, nullptr)));
   return C2V_OK;
 }
 
@@ -1684,6 +1739,39 @@ int c2v_topk(c2v_engine* e, const float* code_vec, int32_t B, int32_t* idx, floa
   if (!code_vec || !idx || !val) return fail(e, C2V_ERR_INVALID, "NULL argument");
   C2V_CUDA(e, cudaSetDevice(e->device));
   return topk_impl(e, (cudaStream_t)stream, code_vec, B, idx, val, normalize);
+}
+
+int c2v_topk_partial(c2v_engine* e, const float* code_all, int32_t Bt, int32_t row_offset, int32_t k, int32_t* idx, float* val,
+                     float* row_max, float* row_sum, void* stream) {
+  int rc = check_batch(e, Bt);
+  if (rc) return rc;
+  if (!code_all || !idx || !val) return fail(e, C2V_ERR_INVALID, "NULL argument");
+  if ((row_max == nullptr) != (row_sum == nullptr)) return fail(e, C2V_ERR_INVALID, "row_max and row_sum: both or neither");
+  if (k < 1 || k > e->dims.top_k) return fail(e, C2V_ERR_INVALID, "k must be in [1, top_k]");
+  if (row_offset < 0) return fail(e, C2V_ERR_INVALID, "row_offset must be >= 0");
+  C2V_CUDA(e, cudaSetDevice(e->device));
+  return topk_partial_impl(e, (cudaStream_t)stream, code_all, Bt, row_offset, k, idx, val, row_max, row_sum);
+}
+
+int c2v_topk_merge(c2v_engine* e, const int32_t* idx, const float* val, const float* maxes, const float* sums, int32_t world,
+                   int32_t Bt, int32_t k, int32_t row0, int32_t rows, int32_t normalize, int32_t* idx_out, float* val_out,
+                   void* stream) {
+  if (!e) return C2V_ERR_INVALID;
+  if (!idx || !val || !idx_out || !val_out) return fail(e, C2V_ERR_INVALID, "NULL argument");
+  if (normalize < 0 || normalize > 2) return fail(e, C2V_ERR_INVALID, "normalize must be 0 (logits), 1 (softmax over k) or 2 (full softmax)");
+  if (normalize == 2 && (!maxes || !sums)) return fail(e, C2V_ERR_INVALID, "normalize 2 needs maxes and sums");
+  if (world < 1 || Bt < 1 || k < 1 || k > e->dims.top_k) return fail(e, C2V_ERR_INVALID, "bad size");
+  if (rows < 1 || row0 < 0 || row0 > Bt - rows) return fail(e, C2V_ERR_INVALID, "rows [row0, row0 + rows) must lie in [0, Bt)");
+  C2V_CUDA(e, cudaSetDevice(e->device));
+  cudaStream_t st = (cudaStream_t)stream;
+  PhaseTimer pt(e, PH_TOPK, st);
+  // list r of row b: idx[r, b, :]
+  const TopkMergeArgs ma{idx, val, world, (size_t)k, (size_t)Bt * k, k, normalize, maxes, sums, world, Bt, row0, idx_out, val_out};
+  if (k <= 16)
+    C2V_LAUNCH(e, (topk_merge_kernel<16><<<rows, kTopkThreads, 0, st>>>(ma)));
+  else
+    C2V_LAUNCH(e, (topk_merge_iter_kernel<<<rows, kTopkThreads, 0, st>>>(ma)));
+  return C2V_OK;
 }
 
 int c2v_loss(c2v_engine* e, const float* code_vec, const int32_t* target, int32_t B, float* loss_out, void* stream) {

@@ -635,8 +635,10 @@ row_maxsum_kernel(const float2* __restrict__ partial, int slots, const float* __
   if (threadIdx.x == 0) {
     row_max[b] = m;
     row_sum[b] = s;
-    const int t = target[b] - row0;                  // local row of the example's target, if it lives here
-    if (!have_true_logit) true_logit[b] = (t >= 0 && t < Y) ? row[t] : 0.f;
+    if (target && !have_true_logit) {                // target == nullptr: the statistics only (c2v_topk_partial)
+      const int t = target[b] - row0;                // local row of the example's target, if it lives here
+      true_logit[b] = (t >= 0 && t < Y) ? row[t] : 0.f;
+    }
   }
 }
 
@@ -757,11 +759,15 @@ __device__ __forceinline__ void topk_finish(float* vals, int k, int normalize, f
   }
 }
 
+// Column j of a row-sharded slab whose first column is global class row_offset (c2v_topk_partial); the padding id INT_MAX
+// stays INT_MAX
+__device__ __forceinline__ int topk_global_id(int j, int row_offset) { return j == INT_MAX ? INT_MAX : j + row_offset; }
+
 // Fast path, k <= K: per-thread sorted register list, then k rounds of block arg-best over the heads.
 template <int K>
 __global__ void __launch_bounds__(kTopkThreads)
 topk_kernel(const float* __restrict__ S, size_t ldS, int Y, int k, int normalize, int32_t* __restrict__ idx_out,
-            float* __restrict__ val_out) {
+            float* __restrict__ val_out, int row_offset = 0) {
   __shared__ ValIdx red[32];
   __shared__ float cv[kTopkThreads * K];
   __shared__ int ci[kTopkThreads * K];
@@ -798,7 +804,7 @@ topk_kernel(const float* __restrict__ S, size_t ldS, int Y, int k, int normalize
     const int hi = (head < K) ? ci[tid * K + head] : INT_MAX;
     const ValIdx w = block_argbest(hv, hi, red);
     if (w.i == hi && hi != INT_MAX) ++head;
-    if (tid == 0) { idx_out[(size_t)blockIdx.x * k + r] = w.i; outv[r] = w.v; }
+    if (tid == 0) { idx_out[(size_t)blockIdx.x * k + r] = topk_global_id(w.i, row_offset); outv[r] = w.v; }
   }
   if (tid == 0) topk_finish(outv, k, normalize, val_out + (size_t)blockIdx.x * k);
 }
@@ -807,7 +813,7 @@ topk_kernel(const float* __restrict__ S, size_t ldS, int Y, int k, int normalize
 // the previous pick.
 __global__ void __launch_bounds__(kTopkThreads)
 topk_iter_kernel(const float* __restrict__ S, size_t ldS, int Y, int k, int normalize, int32_t* __restrict__ idx_out,
-                 float* __restrict__ val_out) {
+                 float* __restrict__ val_out, int row_offset = 0) {
   __shared__ ValIdx red[32];
   __shared__ float outv[64];
   const float* row = S + (size_t)blockIdx.x * ldS;
@@ -824,7 +830,7 @@ topk_iter_kernel(const float* __restrict__ S, size_t ldS, int Y, int k, int norm
     }
     const ValIdx w = block_argbest(bv, bi, red);
     pv = w.v; pi = w.i;
-    if (tid == 0) { idx_out[(size_t)blockIdx.x * k + r] = w.i; outv[r] = w.v; }
+    if (tid == 0) { idx_out[(size_t)blockIdx.x * k + r] = topk_global_id(w.i, row_offset); outv[r] = w.v; }
   }
   if (tid == 0) topk_finish(outv, k, normalize, val_out + (size_t)blockIdx.x * k);
 }
@@ -845,6 +851,112 @@ topk_full_softmax_kernel(const float* __restrict__ S, size_t ldS, int Y, int k, 
     float* v = val + (size_t)blockIdx.x * k + threadIdx.x;
     *v = expf(*v - m) / s;
   }
+}
+
+// ---------------------------------------------------------------------------------------------
+// Merge of sorted candidate lists (c2v_topk_partial over a rank's partial slots, c2v_topk_merge across ranks).  Output
+// row b takes input row row0 + b: L lists of k (value, global id) pairs, list l at (row0 + b) * row_stride + l * list_stride,
+// each sorted by `better` with its padding (-inf, INT_MAX) last, and keeps the best k of their union in the same order.
+// Every element of a row's top k is in the top k of the list that holds it, so the result is the top k of the whole row
+// under tf.nn.top_k's order.  normalize 0 / 1: topk_finish; 2: exp(v - M) / S, (M, S) the combine of the ranks'
+// (max, sum exp) pairs maxes / sums [world, Bt] as in lse_combine_kernel.
+// ---------------------------------------------------------------------------------------------
+struct TopkMergeArgs {
+  const int32_t* idx;
+  const float* val;
+  int L;
+  size_t row_stride, list_stride;
+  int k, normalize;
+  const float* maxes;       // normalize 2: [world, Bt]
+  const float* sums;
+  int world, Bt, row0;
+  int32_t* idx_out;         // [rows, k]
+  float* val_out;
+};
+
+__device__ __forceinline__ void topk_merge_finish(const TopkMergeArgs& a, float* vals) {
+  // thread 0 only
+  const int row = a.row0 + blockIdx.x;
+  float* out = a.val_out + (size_t)blockIdx.x * a.k;
+  if (a.normalize != 2) { topk_finish(vals, a.k, a.normalize, out); return; }
+  float m = -INFINITY;
+  for (int r = 0; r < a.world; ++r) m = fmaxf(m, a.maxes[(size_t)r * a.Bt + row]);
+  float s = 0.f;
+  for (int r = 0; r < a.world; ++r) {
+    const float mr = a.maxes[(size_t)r * a.Bt + row];
+    if (mr > -INFINITY) s += a.sums[(size_t)r * a.Bt + row] * expf(mr - m);
+  }
+  for (int q = 0; q < a.k; ++q) out[q] = expf(vals[q] - m) / s;
+}
+
+// k <= K: each thread keeps a sorted register list of the best K entries of its lists (a list is read only while its
+// entries still enter), then k rounds of block arg-best over the threads' heads, as topk_kernel.
+template <int K>
+__global__ void __launch_bounds__(kTopkThreads) topk_merge_kernel(TopkMergeArgs a) {
+  __shared__ ValIdx red[32];
+  __shared__ float cv[kTopkThreads * K];
+  __shared__ int ci[kTopkThreads * K];
+  __shared__ float outv[K];
+  const int tid = threadIdx.x;
+  const size_t row = (size_t)(a.row0 + blockIdx.x) * a.row_stride;
+  float tv[K];
+  int ti[K];
+#pragma unroll
+  for (int q = 0; q < K; ++q) { tv[q] = -INFINITY; ti[q] = INT_MAX; }
+  for (int l = tid; l < a.L; l += kTopkThreads) {
+    const float* lv = a.val + row + (size_t)l * a.list_stride;
+    const int32_t* li = a.idx + row + (size_t)l * a.list_stride;
+    for (int q = 0; q < a.k; ++q) {
+      const float x = lv[q];
+      const int j = li[q];
+      if (!better(x, j, tv[K - 1], ti[K - 1])) break;      // the list is sorted: none of its later entries enters either
+      tv[K - 1] = x; ti[K - 1] = j;
+#pragma unroll
+      for (int p = K - 1; p > 0; --p) {
+        if (better(tv[p], ti[p], tv[p - 1], ti[p - 1])) {
+          const float fv = tv[p]; tv[p] = tv[p - 1]; tv[p - 1] = fv;
+          const int fi = ti[p]; ti[p] = ti[p - 1]; ti[p - 1] = fi;
+        }
+      }
+    }
+  }
+#pragma unroll
+  for (int q = 0; q < K; ++q) { cv[tid * K + q] = tv[q]; ci[tid * K + q] = ti[q]; }
+  int head = 0;
+  for (int r = 0; r < a.k; ++r) {
+    const float hv = (head < K) ? cv[tid * K + head] : -INFINITY;
+    const int hi = (head < K) ? ci[tid * K + head] : INT_MAX;
+    const ValIdx w = block_argbest(hv, hi, red);
+    if (w.i == hi && hi != INT_MAX) ++head;
+    if (tid == 0) { a.idx_out[(size_t)blockIdx.x * a.k + r] = w.i; outv[r] = w.v; }
+  }
+  if (tid == 0) topk_merge_finish(a, outv);
+}
+
+// Any k <= 64 (the slab route's k > 16, L = world): k rounds, each a block arg-best over the entries ordered after the
+// previous pick, as topk_iter_kernel.
+__global__ void __launch_bounds__(kTopkThreads) topk_merge_iter_kernel(TopkMergeArgs a) {
+  __shared__ ValIdx red[32];
+  __shared__ float outv[64];
+  const int tid = threadIdx.x;
+  const size_t row = (size_t)(a.row0 + blockIdx.x) * a.row_stride;
+  const int n = a.L * a.k;
+  float pv = INFINITY;
+  int pi = -1;
+  for (int r = 0; r < a.k; ++r) {
+    float bv = -INFINITY;
+    int bi = INT_MAX;
+    for (int e = tid; e < n; e += kTopkThreads) {
+      const size_t off = row + (size_t)(e / a.k) * a.list_stride + e % a.k;
+      const float x = a.val[off];
+      const int j = a.idx[off];
+      if (better(pv, pi, x, j) && better(x, j, bv, bi)) { bv = x; bi = j; }
+    }
+    const ValIdx w = block_argbest(bv, bi, red);
+    pv = w.v; pi = w.i;
+    if (tid == 0) { a.idx_out[(size_t)blockIdx.x * a.k + r] = w.i; outv[r] = w.v; }
+  }
+  if (tid == 0) topk_merge_finish(a, outv);
 }
 
 // ---------------------------------------------------------------------------------------------

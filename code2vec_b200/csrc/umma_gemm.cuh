@@ -27,6 +27,7 @@
 #pragma once
 #include <cuda.h>
 #include <cuda_runtime.h>
+#include <limits.h>
 #include <stdint.h>
 
 #include "common.cuh"
@@ -260,6 +261,83 @@ struct EpiStoreLseT {
 template <bool PRECISE>
 struct EpiLseOnlyT : EpiStoreLseT<PRECISE> {
   static constexpr bool kStores = false;
+};
+// Candidate epilogue of the row-sharded prediction (c2v_topk_partial): nothing is stored.  Each (row, partial slot) keeps
+// the best k (value, column) pairs of its 64 columns in registers, value descending, ties to the lower column: an element
+// enters only if it is strictly greater than the list's k-th value, the rule of topk_kernel, so NaN never enters and
+// empty entries stay (-inf, INT_MAX).  A slot's columns arrive in increasing order (quarter p, then p + 2), which is what
+// makes the strict rule put ties in index order.  end() writes the list to cand_val / cand_idx [M, slots, k] with global
+// columns (local + row0).  LSE: the (max, sum exp) partials of EpiStoreLseT as well (normalize 2).
+// The list is kTopkEpiMax registers long; for k < kTopkEpiMax its first kTopkEpiMax - k entries hold +inf, which no
+// element passes, so the k-th value is always the last register.
+constexpr int kTopkEpiMax = 16;
+template <bool PRECISE, bool LSE>
+struct EpiTopkT : EpiStoreLseT<PRECISE> {
+  using Lse = EpiStoreLseT<PRECISE>;
+  struct State {
+    float v[kTopkEpiMax];
+    int i[kTopkEpiMax];
+    typename Lse::State ls;
+  };
+  float* cand_val;
+  int32_t* cand_idx;
+  int k;
+  int row0;
+  static constexpr bool kStores = false;
+  __device__ __forceinline__ void begin(State& st) const {
+#pragma unroll
+    for (int q = 0; q < kTopkEpiMax; ++q) {
+      st.v[q] = q < kTopkEpiMax - k ? INFINITY : -INFINITY;
+      st.i[q] = INT_MAX;
+    }
+    if (LSE) Lse::begin(st.ls);
+  }
+  // x (column col) into the sorted list: c[q] = x > v[q] is monotone in q, so x lands before the first entry it beats and
+  // the entries from there shift down one place; x <= v[K - 1] changes nothing.  Branch-free, so the 32 lanes run it in step.
+  __device__ __forceinline__ void insert(float x, int col, State& st) const {
+#pragma unroll
+    for (int q = kTopkEpiMax - 1; q > 0; --q) {
+      const bool here = x > st.v[q], above = x > st.v[q - 1];
+      st.v[q] = above ? st.v[q - 1] : (here ? x : st.v[q]);
+      st.i[q] = above ? st.i[q - 1] : (here ? col : st.i[q]);
+    }
+    if (x > st.v[0]) { st.v[0] = x; st.i[0] = col; }
+  }
+  // The chunk is screened against the list's k-th value as it stands (it only grows, so nothing screened out could
+  // enter), then each lane inserts its survivors in column order: one rolled loop, so the epilogue's code stays small
+  // enough for the instruction cache (fully unrolled, the 32 insertions made the kernel 35 K instructions long and the
+  // product 7 times slower).  The loop reads the lane's next survivor at a per-lane index, which registers cannot serve:
+  // from a copy of the chunk in local memory (128 bytes per thread, L1-resident).
+  __device__ __forceinline__ void observe(int m, int n, const uint32_t (&r)[32], int nvalid, State& st) const {
+    if (LSE) Lse::observe(m, n, r, nvalid, st.ls);
+    const float kth = st.v[kTopkEpiMax - 1];
+    float x[32];
+    uint32_t todo = 0;
+#pragma unroll
+    for (int j = 0; j < 32; ++j) {
+      x[j] = __uint_as_float(r[j]);
+      if (j < nvalid && x[j] > kth) todo |= 1u << j;
+    }
+#pragma unroll 1
+    while (todo) {
+      const int j = __ffs(todo) - 1;
+      todo &= todo - 1;
+      insert(x[j], n + j, st);
+    }
+  }
+  __device__ __forceinline__ void end(int m, int slot, int sp, bool row_ok, State& st) const {
+    if (!row_ok) return;
+    if (LSE) Lse::end(m, slot, sp, row_ok, st.ls);
+    const size_t base = ((size_t)m * this->slots + slot) * k;
+#pragma unroll
+    for (int q = 0; q < kTopkEpiMax; ++q) {
+      const int p = q - (kTopkEpiMax - k);
+      if (p >= 0) {
+        cand_val[base + p] = st.v[q];
+        cand_idx[base + p] = st.i[q] == INT_MAX ? INT_MAX : st.i[q] + row0;
+      }
+    }
+  }
 };
 // Logits pass 2: the same product again, and the epilogue writes dL/dlogits = (softmax - onehot) / B straight from the
 // accumulator, given each row's log-sum-exp from pass 1: the slab is written once, as the gradient, and never read back

@@ -98,6 +98,8 @@ _SIGNATURES = {
     "c2v_lse_combine": (C.c_int, [_P, _P, _P, _I32, _I32, _P, C.c_float, _P, _P, _P]),
     "c2v_target_backward": (C.c_int, [_P, _P, _I32, _P, _P, _I32, C.c_float, _P, _P]),
     "c2v_context_backward": (C.c_int, [_P, _P, _P, _P, _P, _I32, C.c_float, C.c_uint64, C.c_uint64, _P, _P, _P]),
+    "c2v_topk_partial": (C.c_int, [_P, _P, _I32, _I32, _I32, _P, _P, _P, _P, _P]),
+    "c2v_topk_merge": (C.c_int, [_P, _P, _P, _P, _P, _I32, _I32, _I32, _I32, _I32, _I32, _P, _P, _P]),
     "c2v_launch_count": (C.c_int64, [_P]),
     "c2v_phase_count": (C.c_int, []),
     "c2v_phase_name": (C.c_char_p, [C.c_int]),
@@ -400,11 +402,12 @@ class PathAttentionEngine:
         return torch.from_numpy(np.ascontiguousarray(arr)).to(device=self.dev, dtype=dtype)
 
     # ---- device-pointer entry points ---------------------------------------------------------
-    def forward(self, src, path, tgt, mask, want_attention: bool = True):
-        """c2v_forward: (code_vectors [B, D], attention [B, C] or None) as device tensors."""
+    def forward(self, src, path, tgt, mask, want_attention: bool = True, code_out=None):
+        """c2v_forward: (code_vectors [B, D], attention [B, C] or None) as device tensors; code_out: an existing
+        [B, D] tensor to write the code vectors into."""
         torch = self.torch
         B, Cn = src.shape
-        code = torch.empty((B, self.dims.code_dim), dtype=torch.float32, device=self.dev)
+        code = torch.empty((B, self.dims.code_dim), dtype=torch.float32, device=self.dev) if code_out is None else code_out
         attn = torch.empty((B, Cn), dtype=torch.float32, device=self.dev) if want_attention else None
         self._check(self.lib.c2v_forward(self.h, src.data_ptr(), path.data_ptr(), tgt.data_ptr(), mask.data_ptr(),
                                          B, code.data_ptr(), _ptr(attn), self._stream()))
@@ -500,6 +503,22 @@ class PathAttentionEngine:
         self._check(self.lib.c2v_context_backward(self.h, src.data_ptr(), path.data_ptr(), tgt.data_ptr(), mask.data_ptr(),
                                                   src.shape[0], float(keep), int(seed), int(step), _ptr(dropout_mask),
                                                   dv.data_ptr(), self._stream()))
+
+    # ---- prediction against a row-sharded target table (fully sharded schedule) ------------------------
+    def topk_partial(self, code_all, row_offset, k, idx, val, row_max=None, row_sum=None):
+        """c2v_topk_partial: this engine's best k target rows for each of the Bt examples of code_all [Bt, D], with global
+        ids (local row + row_offset) and raw logits, into idx [Bt, k] (int32) / val [Bt, k]; with row_max / row_sum [Bt],
+        the (max, sum exp) of each example's local logits as well (for normalize 2)."""
+        self._check(self.lib.c2v_topk_partial(self.h, code_all.data_ptr(), code_all.shape[0], int(row_offset), int(k),
+                                              idx.data_ptr(), val.data_ptr(), _ptr(row_max), _ptr(row_sum), self._stream()))
+
+    def topk_merge(self, idx, val, maxes, sums, row0, rows, normalize, idx_out, val_out):
+        """c2v_topk_merge: the ranks' candidates idx / val [world, Bt, k] (and maxes / sums [world, Bt], or None unless
+        normalize == 2) -> the top k of examples [row0, row0 + rows) into idx_out / val_out [rows, k]."""
+        world, Bt, k = idx.shape
+        self._check(self.lib.c2v_topk_merge(self.h, idx.data_ptr(), val.data_ptr(), _ptr(maxes), _ptr(sums), world, Bt, k,
+                                            int(row0), int(rows), int(normalize), idx_out.data_ptr(), val_out.data_ptr(),
+                                            self._stream()))
 
     # ---- row-sharded embedding tables over peer memory (data-parallel runs) ----------------------
     def apply_scatter_inbox(self):

@@ -194,6 +194,10 @@ class Trainer:
             self._fs = dict(v_local=z((Bl, D)), v_all=z((Bt, D)), tgt_all=z((Bt,), i32), rmax=z((Bt,)), rsum=z((Bt,)),
                             tlogit=z((Bt,)), maxes=z((self.world, Bt)), sums=z((self.world, Bt)), lse=z((Bt,)),
                             dv_part=z((Bt, D)), dv_local=z((Bl, D)), loss=z((1,)), token=z((1,)))
+            # predict(): this rank's candidates, every rank's (all-gathered), and the merged rows of its own examples
+            W, k = self.world, min(engine.dims.top_k, engine.global_target_vocab)
+            self._pred = dict(idx=z((Bt, k), i32), val=z((Bt, k)), idx_all=z((W, Bt, k), i32), val_all=z((W, Bt, k)),
+                              idx_out=z((Bl, k), i32), val_out=z((Bl, k)))
             layout, total = engine.flat_layout()
             small0 = [off for k, off, n in layout if k == "W"][0]
             self._small = (small0, total)
@@ -293,6 +297,38 @@ class Trainer:
                                     seed=self.seed, step=t)
         e.adam_step(t=t, **self.adam)
         return loss
+
+    def predict(self, src, path, tgt, mask, normalize: int = 0):
+        """Top-k prediction of this rank's examples: (idx [B, k], val [B, k], code_vec [B, D]) as device tensors, the
+        result of forward + topk on one engine holding the whole model (normalize as c2v_topk).  No training state is
+        touched, so it runs between training steps and on engines made with training=False.
+        fully_sharded: the rank's engine holds one block of target rows, so the code vectors are all-gathered, every
+        rank ranks its block for the whole global batch (c2v_topk_partial), the [Bt, k] candidates (and for normalize 2
+        the per-row (max, sum exp)) are all-gathered, and each rank merges the rows of its own examples
+        (c2v_topk_merge).  The returned tensors are buffers the next predict() call overwrites."""
+        e = self.e
+        if self.schedule != "fully_sharded":
+            code, _ = e.forward(src, path, tgt, mask, want_attention=False)
+            idx, val = e.topk(code, normalize)
+            return idx, val, code
+        dist, fs, pr = _dist(), self._fs, self._pred
+        if int(src.shape[0]) != e.local_batch:
+            raise ValueError("fully_sharded needs the same local batch (%d) on every rank" % e.local_batch)
+        full = normalize == 2
+        e.forward(src, path, tgt, mask, want_attention=False, code_out=fs["v_local"])
+        dist.all_gather_into_tensor(fs["v_all"], fs["v_local"], group=self.group)
+        k = pr["idx"].shape[1]
+        e.topk_partial(fs["v_all"], e.target_row0, k, pr["idx"], pr["val"], fs["rmax"] if full else None,
+                       fs["rsum"] if full else None)
+        dist.all_gather_into_tensor(pr["idx_all"].view(-1), pr["idx"].view(-1), group=self.group)
+        dist.all_gather_into_tensor(pr["val_all"].view(-1), pr["val"].view(-1), group=self.group)
+        if full:
+            dist.all_gather_into_tensor(fs["maxes"].view(-1), fs["rmax"], group=self.group)
+            dist.all_gather_into_tensor(fs["sums"].view(-1), fs["rsum"], group=self.group)
+        Bl = e.local_batch
+        e.topk_merge(pr["idx_all"], pr["val_all"], fs["maxes"] if full else None, fs["sums"] if full else None,
+                     self.rank * Bl, Bl, normalize, pr["idx_out"], pr["val_out"])
+        return pr["idx_out"], pr["val_out"], fs["v_local"]
 
     def _fully_sharded_step(self, src, path, tgt, mask, target):
         e, dist, fs = self.e, _dist(), self._fs

@@ -272,6 +272,31 @@ int c2v_context_backward(c2v_engine* e, const int32_t* src, const int32_t* path,
                          const float* mask, int32_t B, float keep_prob, uint64_t seed, uint64_t step,
                          const float* dropout_mask, const float* dv, void* stream);
 
+/* ---- Prediction against a row-sharded target table (the fully sharded schedule) -----------------------
+ * The same engine as the phase-split step (target_vocab = LOCAL rows, max_batch = GLOBAL batch Bt).
+ * Each rank ranks its own block, the ranks all-gather [Bt, k] candidates, and each rank merges the
+ * rows of its own examples; the result is c2v_topk's over the whole target vocabulary: idx equal, val
+ * equal for normalize 0 and 1 and equal up to summation order for normalize 2.
+ *   c2v_topk_partial : k <= top_k (pass min(top_k, global target vocabulary)).  idx / val [Bt, k] =
+ *                      this engine's best k rows for each of the Bt examples, sorted as tf.nn.top_k
+ *                      (value descending, ties to the lower id), with GLOBAL ids (local row +
+ *                      row_offset) and raw logits, padded with (-inf, INT_MAX) where the block has
+ *                      fewer than k rows.  row_max / row_sum [Bt] (both or neither; needed for
+ *                      normalize 2) = max and sum exp(. - max) of the example's logits over the
+ *                      local rows.  As c2v_topk, lazily updated target rows are brought up to date
+ *                      first and 3xTF32 splits the table.  In the tensor-core modes with k <= 16 no
+ *                      logit is stored: the logits GEMM's epilogue keeps candidate lists.
+ *   c2v_topk_merge   : idx / val [world, Bt, k] (the ranks' c2v_topk_partial results, all-gathered),
+ *                      maxes / sums [world, Bt] (their row_max / row_sum; only read for normalize 2)
+ *                      -> idx_out / val_out [rows, k] for examples [row0, row0 + rows): the best k of
+ *                      the world lists, padding ignored, with c2v_topk's normalize (0, 1, 2; 2 uses
+ *                      the global log-sum-exp combined from maxes / sums). */
+int c2v_topk_partial(c2v_engine* e, const float* code_all, int32_t Bt, int32_t row_offset, int32_t k,
+                     int32_t* idx, float* val, float* row_max, float* row_sum, void* stream);
+int c2v_topk_merge(c2v_engine* e, const int32_t* idx, const float* val, const float* maxes,
+                   const float* sums, int32_t world, int32_t Bt, int32_t k, int32_t row0, int32_t rows,
+                   int32_t normalize, int32_t* idx_out, float* val_out, void* stream);
+
 /* With "lazy_adam" on: replay all deferred updates so that the bound token / path tables (and their
  * Adam slots) hold exactly what the dense optimizer would hold after the steps applied so far.  Call
  * before reading the parameter tensors from outside the engine (export, checkpoint).  No-op otherwise. */
