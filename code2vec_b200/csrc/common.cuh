@@ -35,8 +35,13 @@ __device__ __forceinline__ float adam_move(float theta, float lr_t, float m, flo
 }
 // exp_slab schedule (umma::EpiExpSumT, expsum_combine_kernel): a row's largest U = exp(logit - c_row) must stay inside this
 // window for the deferred normalisation to be used; fp32 then still resolves elements e^-27 below the row's maximum and
-// a sum of 2^18 such terms cannot overflow.
+// a sum of 2^18 such terms cannot overflow.  Its factor r = 1 / (B Z) must also leave dY's operand r v_b normal where it
+// matters: r max_j |v_b[j]| >= kExpSlabMinOperand, 2^14 above FLT_MIN.  A subnormal operand loses the 13 bits the tf32
+// tensor cores (and each half of the 3xTF32 split) drop from the bottom of its field, 2^-136 absolutely; above this
+// limit that is below 2^-24 of the row's largest operand.  Z reaches 2.6e35 inside the U window (Y = 261,246), where r
+// falls below FLT_MIN at B = 1024.
 constexpr float kExpSlabMin = 1e-26f, kExpSlabMax = 1e30f;
+constexpr float kExpSlabMinOperand = 0x1p-112f;
 
 // The same move without the test, for dense gradients (the target table's update in the dY epilogue, adam_kernel): zero
 // numerators are rare there and the branch costs more than the occasional slow path.  Identical bits by the argument above.

@@ -872,6 +872,12 @@ int run_logits(c2v_engine* e, cudaStream_t st, const float* v, int B, LogitsOut 
     return is_3x(e) ? launch_logits<true>(e, st, v, B, out, a, for_dv) : launch_logits<false>(e, st, v, B, out, a, for_dv);
   const int D = e->dims.code_dim;
   PhaseTimer pt(e, PH_LOGITS, st);
+  if (!aligned16(v)) {        // the SIMT loaders read float4s: code vectors a caller passed unaligned go through a copy
+    float* va = wsp<float>(e, e->ws.v_scaled);
+    if (e->pending_dy.v == va) return fail(e, C2V_ERR_STATE, "a deferred dY still reads the exp_slab scaled code vectors");
+    C2V_CUDA(e, cudaMemcpyAsync(va, v, (size_t)B * D * 4, cudaMemcpyDeviceToDevice, st));
+    v = va;
+  }
   simt::RowsK al{v, (size_t)D};
   simt::RowsK bl{e->theta.tgt, (size_t)D};
   simt::StoreC ep{wsp<float>(e, e->ws.S), e->ws.ldS, 0};
@@ -1299,8 +1305,8 @@ int train_step_impl(c2v_engine* e, cudaStream_t st, const int32_t* src, const in
     int* flag = wsp<int>(e, e->ws.slab_flag);
     float* S_lo = is_3x(e) ? wsp<float>(e, e->ws.S_lo) : nullptr;
     rc = exp_slab_logits(e, st, v, B, target, 0, nullptr, [&]() -> int {
-      C2V_LAUNCH(e, (expsum_combine_kernel<<<B, 256, 0, st>>>(part, n_tiles, S, S_lo, e->ws.ldS, Y, target, tl, tl, invB, loss_b, lse,
-                                                              rscale, flag)));
+      C2V_LAUNCH(e, (expsum_combine_kernel<<<B, 256, 0, st>>>(part, n_tiles, S, S_lo, e->ws.ldS, Y, target, tl, tl, v, e->dims.code_dim,
+                                                              invB, loss_b, lse, rscale, flag)));
       return C2V_OK;
     });
     if (rc) return rc;

@@ -329,29 +329,35 @@ true_logit_kernel(const float* __restrict__ v, const float* __restrict__ Ytab, c
 // softmax - onehot = (U - Z [j == y_b]) / Z  -- so ONE element of the row is patched (U[b, y_b] -= Z) and the row's factor
 // 1 / (B Z) (rscale) is handed to the two gradient GEMMs: it scales dv's rows in the split-K reduction and the code vectors
 // that are dY's small operand (scale_rows_kernel).  A row whose largest U is outside [kExpSlabMin, kExpSlabMax] (or not a
-// number) raises *bad: the gated two-pass kernels that follow then redo the step's softmax the classic way.  One CTA per row.
+// number), or whose scaled code vector rscale v_b has its largest element below kExpSlabMinOperand (common.cuh: smaller,
+// and the tensor cores would read subnormal operands that keep only a few bits), raises *bad: the gated two-pass kernels
+// that follow then redo the step's softmax the classic way.  One CTA per row.
 __global__ void __launch_bounds__(256)
 expsum_combine_kernel(const float2* __restrict__ partial, int n_tiles, float* __restrict__ U, float* __restrict__ U_lo, size_t ldS, int Y,
                       const int32_t* __restrict__ target, const float* __restrict__ offset, const float* __restrict__ true_logit,
-                      float inv_batch, float* __restrict__ loss_b, float* __restrict__ lse_out, float* __restrict__ rscale,
-                      int* __restrict__ bad) {
+                      const float* __restrict__ v, int D, float inv_batch, float* __restrict__ loss_b, float* __restrict__ lse_out,
+                      float* __restrict__ rscale, int* __restrict__ bad) {
   __shared__ float red[32];
   const int b = blockIdx.x;
   const float2* p = partial + (size_t)b * n_tiles;
-  float m = 0.f, s = 0.f;
+  float m = 0.f, s = 0.f, a = 0.f;
   for (int i = threadIdx.x; i < n_tiles; i += 256) {
     const float2 q = p[i];
     m = fmaxf(m, q.x);
     s += q.y;
   }
+  for (int j = threadIdx.x; j < D; j += 256) a = fmaxf(a, fabsf(v[(size_t)b * D + j]));
   const float M = block_max(m, red);
+  const float A = block_max(a, red);
   s = block_sum(s, red);
   if (threadIdx.x == 0) {
+    const float r = inv_batch / s;
     if (!(M >= kExpSlabMin && M <= kExpSlabMax && s <= 3.0e38f)) *bad = 1;      // NaN fails every comparison
+    if (A > 0.f && !(r * A >= kExpSlabMinOperand)) *bad = 1;                     // a zero code vector loses nothing
     const float lz = logf(s);
     lse_out[b] = offset[b] + lz;
     loss_b[b] = (offset[b] - true_logit[b]) + lz;
-    rscale[b] = inv_batch / s;
+    rscale[b] = r;
     const int y = target[b];
     if (y >= 0 && y < Y) {
       const size_t at = (size_t)b * ldS + y;

@@ -150,7 +150,9 @@ int c2v_bind_adam_state(c2v_engine* e, const c2v_tensors* m, const c2v_tensors* 
  * train step): the logits GEMM's epilogue writes U = exp(logit - true-class logit) instead of the logits, one element
  * per row is patched and the softmax's 1 / sum is applied as a per-example factor by the two target-side gradient
  * GEMMs, so no pass re-reads the [B, Y] slab to normalise it; a step in which some row's largest U leaves the fp32
- * window [1e-26, 1e30] is redone on the device as the two-pass schedule (logits stored, then rewritten) -- read-only
+ * window [1e-26, 1e30], or some row's scaled code vector (the factor times v_b, dY's operand) has its largest
+ * element below 2^-112 (subnormal elements would lose most of their bits on the tensor cores), is redone on the
+ * device as the two-pass schedule (logits stored, then rewritten) -- read-only
  * "exp_slab_fallbacks" counts those steps (the read synchronises the device), "sort_peer_access" (row-sharded
  * tables over peer memory: 0 never, 1 = default: when a table exceeds 2 GB, 2 always -- the step's row indices are
  * counting-sorted by (owner, 2 MB page) before the peer gather / scatter-add).
@@ -179,7 +181,8 @@ int c2v_topk(c2v_engine* e, const float* code_vec, int32_t B, int32_t* idx, floa
              int32_t normalize, void* stream);
 
 /* Mean sparse-softmax cross entropy of code_vec against `target` without gradients
- * (tensorflow_model.py:226-230).  loss_out: device float[1]. */
+ * (tensorflow_model.py:226-230).  code_vec needs only float alignment: code vectors that are not 16-byte aligned
+ * take the fp32 SIMT logits through an aligned copy.  loss_out: device float[1]. */
 int c2v_loss(c2v_engine* e, const float* code_vec, const int32_t* target, int32_t B,
              float* loss_out, void* stream);
 

@@ -42,7 +42,8 @@ SLICE_TOL = {0: SLICE_TOL_FP32, 1: SLICE_TOL_TF32, 2: SLICE_TOL_FP32}     # by e
 @dataclass
 class Ref64:
     """Values (float64) and magnitudes of one step.  vals / mags hold v, alpha, dv and the five gradients; extra holds
-    the per-example log-sum-exp "lse" and, for the full softmax, the smallest probability "pmin"."""
+    the per-example log-sum-exp "lse" and, for the full softmax, the smallest probability "pmin", the loss magnitude
+    "loss_mag" and each row's largest log U = max_y s - s_true with its column ("log_umax", "umax_col")."""
     loss: float
     vals: Dict[str, np.ndarray]
     mags: Dict[str, np.ndarray]
@@ -145,24 +146,60 @@ def forward64(params, src, pth, tgt, mask, ex_block=128):
     return tuple(np.concatenate(out[k]) for k in ("v", "Mv", "alpha", "Malpha"))
 
 
-def _full_head(P, v, Mv, target, y_block, soft_factor=1.0):
-    """Full softmax over Y in row blocks: loss, dv, dY and magnitudes.  Two passes (log-sum-exp and max M(s) first)."""
-    Yt = P["tgt"]
+def _lse_pass(Yt, v, Mv, y_block):
+    """First pass over the target rows: log-sum-exp, max M(s), and each row's largest logit with its column."""
     B, Y = v.shape[0], Yt.shape[0]
-    av = np.abs(v)
     m = np.full(B, -np.inf)
+    col = np.zeros(B, dtype=np.int64)
     ssum = np.zeros(B)
     Msmax = np.zeros(B)
-    s_true = np.einsum("bd,bd->b", v, Yt[target])
     for y0 in range(0, Y, y_block):
         Yb = Yt[y0:y0 + y_block]
         s = v @ Yb.T
         Ms = Mv @ np.abs(Yb).T + np.abs(s)
         Msmax = np.maximum(Msmax, Ms.max(axis=1))
-        mn = np.maximum(m, s.max(axis=1))
+        bm, bi = s.max(axis=1), s.argmax(axis=1)
+        col = np.where(bm > m, y0 + bi, col)
+        mn = np.maximum(m, bm)
         ssum = ssum * np.exp(m - mn) + np.exp(s - mn[:, None]).sum(axis=1)
         m = mn
-    lse = m + np.log(ssum)
+    return m + np.log(ssum), Msmax, m, col
+
+
+def _loss_extra(lse, Mlse, s_true, Ms_true, smax, col):
+    """extra entries of the loss: "lse"; "loss_mag", the mean over b of M(lse_b) + M(s_true,b), so that a loss whose
+    logits are in the hundreds can be held to tau M rather than to a flat tolerance below its fp32 rounding; and per row
+    "log_umax" = max_y s - s_true (the log of the exp_slab schedule's largest U = exp(s - s_true)) and "umax_col", its
+    column."""
+    return dict(lse=lse, loss_mag=float(np.mean(Mlse + Ms_true)), log_umax=smax - s_true, umax_col=col)
+
+
+def head_loss64(params, v, target, Mv=None, y_block=16384):
+    """Loss of the full softmax from given code vectors [B, D] (exact float32 values unless Mv is given): (loss, extra)
+    with extra as _full_head's ("lse", "loss_mag", "log_umax", "umax_col")."""
+    Yt = np.asarray(params["tgt"], dtype=np.float64)
+    v = np.asarray(v, dtype=np.float64)
+    Mv = np.abs(v) if Mv is None else Mv
+    lse, _, smax, col = _lse_pass(Yt, v, Mv, y_block)
+    Mlse = np.abs(lse)
+    for y0 in range(0, Yt.shape[0], y_block):
+        Yb = Yt[y0:y0 + y_block]
+        s = v @ Yb.T
+        Mlse += (np.exp(s - lse[:, None]) * (Mv @ np.abs(Yb).T + np.abs(s))).sum(axis=1)
+    s_true = np.einsum("bd,bd->b", v, Yt[target])
+    Ms_true = np.einsum("bd,bd->b", Mv, np.abs(Yt[target])) + np.abs(s_true)
+    return float(np.mean(lse - s_true)), _loss_extra(lse, Mlse, s_true, Ms_true, smax, col)
+
+
+def _full_head(P, v, Mv, target, y_block, soft_factor=1.0):
+    """Full softmax over Y in row blocks: loss, dv, dY and magnitudes.  Two passes (log-sum-exp and max M(s) first)."""
+    Yt = P["tgt"]
+    B, Y = v.shape[0], Yt.shape[0]
+    av = np.abs(v)
+    s_true = np.einsum("bd,bd->b", v, Yt[target])
+    Ms_true = np.einsum("bd,bd->b", Mv, np.abs(Yt[target])) + np.abs(s_true)
+    lse, Msmax, smax, col = _lse_pass(Yt, v, Mv, y_block)
+    Mlse = np.abs(lse)
     loss = float(np.mean(lse - s_true))
     dv = np.zeros_like(v)
     Mdv = np.zeros_like(v)
@@ -177,6 +214,7 @@ def _full_head(P, v, Mv, target, y_block, soft_factor=1.0):
         Ms = Mv @ aYb.T + np.abs(s)
         p = np.exp(s - lse[:, None])
         pmin = min(pmin, float(p.min()))
+        Mlse += (p * Ms).sum(axis=1)
         Mp = p * (1.0 + Ms + Msmax[:, None])
         q = p * soft_factor
         hit = (target >= y0) & (target < y0 + Yb.shape[0])
@@ -190,7 +228,7 @@ def _full_head(P, v, Mv, target, y_block, soft_factor=1.0):
         dv += dl @ Yb
         Mdv += Mdl @ aYb
     Mdv += np.abs(dv)
-    return loss, dv, Mdv, gY, MgY, dict(pmin=pmin, lse=lse)
+    return loss, dv, Mdv, gY, MgY, dict(pmin=pmin, **_loss_extra(lse, Mlse, s_true, Ms_true, smax, col))
 
 
 def _sampled_head(P, v, Mv, target, sampled, logq_true, logq_sampled):
@@ -314,17 +352,98 @@ def topk64(params, v, Mv, k, y_block=16384):
     return dict(idx=idx, s=s, Ms=Ms, p=p, Mp=Mp)
 
 
+LOG_U_EDGE = float(np.log(5e29))     # just inside the exp_slab window's largest U, 1e30
+
+
+def _row_logits_max(Yt, v, exclude, y_block=16384):
+    """max_y v_b . Y_y over y != exclude[b], per row of v."""
+    out = np.full(v.shape[0], -np.inf)
+    rows = np.arange(v.shape[0])
+    for y0 in range(0, Yt.shape[0], y_block):
+        s = v @ Yt[y0:y0 + y_block].T
+        hit = (exclude >= y0) & (exclude < y0 + s.shape[1])
+        s[rows[hit], exclude[hit] - y0] = -np.inf
+        out = np.maximum(out, s.max(axis=1))
+    return out
+
+
+def _column_direction(v, b):
+    """u with v_b . u = 1 and the other code vectors as orthogonal to it as they can be (ridge least squares)."""
+    others = np.delete(v, b, axis=0)
+    G = others.T @ others
+    u = np.linalg.solve(G + 1e-3 * np.trace(G) / G.shape[0] * np.eye(G.shape[0]), v[b])
+    return u / (v[b] @ u)
+
+
+def quiet_row(v, candidates=64):
+    """The example among the first `candidates` whose raise_column direction the other code vectors overlap least."""
+    v = np.asarray(v, dtype=np.float64)
+    leak = [np.abs(np.delete(v, b, axis=0) @ _column_direction(v, b)).max() for b in range(min(candidates, len(v)))]
+    return int(np.argmin(leak))
+
+
+def raise_column(params, v, target, b, col, log_u):
+    """Copy of params in which example b's logit in column `col` exceeds its true-class logit by log_u, and the other
+    examples' logits there move as little as possible: target row `col` moves along u, the least-squares solution of
+    v_b . u = 1 with the other code vectors as orthogonal to u as they can be.  v: the step's code vectors [B, D] (after
+    dropout).  No example may have `col` as its class."""
+    assert not np.any(target == col), col
+    v = np.asarray(v, dtype=np.float64)
+    u = _column_direction(v, b)
+    Yt = np.asarray(params["tgt"], dtype=np.float64)
+    lam = log_u + v[b] @ Yt[target[b]] - v[b] @ Yt[col]
+    out = dict(params)
+    out["tgt"] = params["tgt"].copy()
+    out["tgt"][col] = (Yt[col] + lam * u).astype(np.float32)
+    return out
+
+
+def rows_to_lower(v, target, n, candidates=256):
+    """`n` examples for lower_true_rows: among the first `candidates` whose class no other example has, those whose
+    raise_column direction the other code vectors overlap least."""
+    v = np.asarray(v, dtype=np.float64)
+    own = np.flatnonzero(np.bincount(target)[target] == 1)[:candidates]
+    leak = [np.abs(np.delete(v, b, axis=0) @ _column_direction(v, b)).max() for b in own]
+    return np.sort(own[np.argsort(leak, kind="stable")[:n]])
+
+
+def lower_true_rows(params, v, target, rows, log_u, iters=4, y_block=16384):
+    """Copy of params in which each example b of `rows` has its largest exp(s - s_true) at exp(log_u): its true-class row
+    moves by -lambda_b u_b (u_b as in raise_column: v_b . u_b = 1, the other code vectors nearly orthogonal), which lowers
+    s_true,b by lambda_b and the other examples' logits in that column by little.  The classes of `rows` must be
+    distinct and no other example's, so no other true-class logit moves.  lambda is refined `iters` times, because
+    lowering one row's class can raise another chosen row's largest logit a little."""
+    rows = np.asarray(rows)
+    t = target[rows]
+    assert len(np.unique(t)) == len(rows) and not np.isin(np.delete(target, rows), t).any()
+    v = np.asarray(v, dtype=np.float64)
+    U = np.stack([_column_direction(v, b) for b in rows])
+    vr = v[rows]
+    Yt = np.asarray(params["tgt"], dtype=np.float64).copy()
+    for _ in range(iters):
+        gap = _row_logits_max(Yt, vr, t, y_block) - np.einsum("bd,bd->b", vr, Yt[t])
+        Yt[t] -= (log_u - gap)[:, None] * U
+    out = dict(params)
+    out["tgt"] = params["tgt"].copy()
+    out["tgt"][t] = Yt[t].astype(np.float32)
+    return out
+
+
 def tf32_truncate(a):
     """The tf32 operand the tensor cores read from an fp32 value: the low 13 mantissa bits dropped (truncation)."""
     u = np.ascontiguousarray(a, dtype=np.float32).view(np.uint32)
     return (u & np.uint32(0xFFFFE000)).view(np.float32).astype(np.float64)
 
 
-def tf32_model_loss(params, src, pth, tgt, mask, target, *, keep=1.0, dropout_mask=None, y_block=16384):
+def tf32_model_loss(params, src, pth, tgt, mask, target, *, keep=1.0, dropout_mask=None, y_block=16384,
+                    true_logit="fp32"):
     """Loss of a train step whose two loss-bearing GEMMs read tf32-truncated operands, everything else exact: the
-    context projection X.W and the logits v.Y^T; the true-class logit stays fp32, as the exp_slab schedule computes it.
-    Truncation biases every product toward zero, and a bias does not average out over the batch, so this is what tf32
-    converges to where the logits are large or have few terms; the float64 loss is what fp32 converges to."""
+    context projection X.W and the logits v.Y^T.  true_logit: "fp32" keeps the true-class logit exact, as the exp_slab
+    and recompute_logits schedules compute it (a separate fp32 dot product); "tf32" takes it from the truncated logits,
+    as the two-pass and loader schedules do (they read it from the tensor-core slab).  Truncation biases every product
+    toward zero, and a bias does not average out over the batch, so this is what tf32 converges to where the logits are
+    large or have few terms; the float64 loss is what fp32 converges to."""
+    assert true_logit in ("fp32", "tf32"), true_logit
     P = _f64(params)
     B, C = src.shape
     x = np.concatenate([P["tok"][src], P["path"][pth], P["tok"][tgt]], axis=-1).reshape(B * C, -1)
@@ -345,7 +464,10 @@ def tf32_model_loss(params, src, pth, tgt, mask, target, *, keep=1.0, dropout_ma
         mn = np.maximum(m, s.max(axis=1))
         ssum = ssum * np.exp(m - mn) + np.exp(s - mn[:, None]).sum(axis=1)
         m = mn
-    s_true = np.einsum("bd,bd->b", v, P["tgt"][target])
+    if true_logit == "tf32":
+        s_true = np.einsum("bd,bd->b", vt, tf32_truncate(P["tgt"][target]))
+    else:
+        s_true = np.einsum("bd,bd->b", v, P["tgt"][target])
     return float(np.mean(m + np.log(ssum) - s_true))
 
 

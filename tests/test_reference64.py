@@ -229,3 +229,99 @@ def test_sampled_head_matches_oracle_and_float32_passes():
     bad[sampled[5]] *= np.float32(1.01)
     with pytest.raises(AssertionError):
         R.check_step({"tgt": bad}, ref, R.TAU_FP32)
+
+
+# ---- the loss bound of logits in the hundreds, the truncation model's true-class logit, the window-edge recipes ----------
+
+ODD = O.Dims(777, 333, 1537, 20, 52, 13)
+
+
+def wide_logits_case(name):
+    """(params, batch): trained-scale logits (target table x 80, attention vector x 4), or logits up to +-400."""
+    if name == "trained":
+        dims = O.Dims(20011, 10007, 5003, 128, 384, 50)
+        params = O.init_params(dims, seed=4321)
+        params["tgt"] = (params["tgt"] * np.float32(80.0)).astype(np.float32)
+        params["a"] = (params["a"] * np.float32(4.0)).astype(np.float32)
+        return params, O.synthetic_batch(dims, 64, seed=90)
+    batch = O.synthetic_batch(ODD, 37, seed=81)
+    params = O.init_params(ODD, seed=9)
+    v, _, _ = O.forward(params, *batch[:4])
+    params["tgt"] = (params["tgt"] * np.float32(400.0 / np.abs(O.logits_of(params, v)).max())).astype(np.float32)
+    return params, batch
+
+
+@pytest.mark.parametrize("name", ["trained", "logits_400"])
+def test_float32_oracle_meets_the_loss_bound(name):
+    """The float32 oracle's loss is within TAU_FP32 M_loss of the float64 one, with no absolute floor."""
+    params, batch = wide_logits_case(name)
+    ref = R.train_step64(params, *batch)
+    loss, _, _ = O.train_loss_and_grads(params, *batch)
+    if name == "logits_400":
+        assert np.abs(ref.extra["log_umax"]).max() > 100
+    err, bound = abs(loss - ref.loss), R.TAU_FP32 * ref.extra["loss_mag"]
+    print(name, "loss %.6g err %.2e bound %.2e" % (ref.loss, err, bound))
+    assert err <= bound
+
+
+def tf32_emulated_loss(params, src, pth, tgt, mask, target, true_logit):
+    """tf32_model_loss's model in float32 numpy: truncated operands, float32 arithmetic everywhere else."""
+    f32 = lambda a: np.asarray(a, dtype=np.float32)
+    tr = lambda a: f32(R.tf32_truncate(a))
+    B, C = src.shape
+    x = np.concatenate([params["tok"][src], params["path"][pth], params["tok"][tgt]], axis=-1).reshape(B * C, -1)
+    h = np.tanh(tr(x) @ tr(params["W"]))
+    z = np.where(mask > 0, (h @ params["a"]).reshape(B, C), np.float32(-np.inf))
+    al = np.exp(z - z.max(axis=1, keepdims=True))
+    al /= al.sum(axis=1, keepdims=True)
+    v = np.einsum("bc,bcd->bd", al, h.reshape(B, C, -1))
+    s = tr(v) @ tr(params["tgt"]).T
+    m = s.max(axis=1)
+    lse = m + np.log(np.exp(s - m[:, None]).sum(axis=1))
+    st = s[np.arange(B), target] if true_logit == "tf32" else np.einsum("bd,bd->b", v, params["tgt"][target])
+    return float(np.mean(lse - st))
+
+
+@pytest.mark.parametrize("true_logit", ["fp32", "tf32"])
+def test_tf32_model_true_logit_variants_match_a_float32_emulation(true_logit):
+    params, batch = wide_logits_case("trained")
+    model = R.tf32_model_loss(params, *batch, true_logit=true_logit)
+    emulated = tf32_emulated_loss(params, *batch, true_logit)
+    other = R.tf32_model_loss(params, *batch, true_logit="tf32" if true_logit == "fp32" else "fp32")
+    print(true_logit, "model %.7g emulated %.7g other variant %.7g" % (model, emulated, other))
+    assert abs(model - emulated) < 1e-5
+    assert abs(model - other) > 1e-4                  # the choice matters at trained scale
+
+
+RECIPE = O.Dims(1001, 501, 5003, 128, 384, 20)
+
+
+@pytest.mark.parametrize("recipe", ["column_last", "column_first", "lowered"])
+def test_window_edge_recipes_put_the_largest_u_where_they_claim(recipe):
+    params = O.init_params(RECIPE, seed=4321)
+    src, pth, tgt, mask, target = O.synthetic_batch(RECIPE, 256, seed=7)
+    target = np.where(np.isin(target, [0, RECIPE.target_vocab - 1]), 1, target).astype(target.dtype)
+    v, Mv, _, _ = R.forward64(params, src, pth, tgt, mask)
+    if recipe == "lowered":
+        rows = R.rows_to_lower(v, target, 24)
+        crafted = R.lower_true_rows(params, v, target, rows, R.LOG_U_EDGE)
+        col = None
+    else:
+        rows = np.array([R.quiet_row(v)])
+        col = RECIPE.target_vocab - 1 if recipe == "column_last" else 0
+        crafted = R.raise_column(params, v, target, rows[0], col, R.LOG_U_EDGE)
+    _, ex = R.head_loss64(crafted, v, target, Mv=Mv)
+    log_u = ex["log_umax"]
+    others = np.setdiff1d(np.arange(len(target)), rows)
+    print(recipe, "rows %.4f..%.4f, others below %.2f" % (log_u[rows].min(), log_u[rows].max(), log_u[others].max()))
+    assert np.all(np.abs(log_u[rows] - R.LOG_U_EDGE) < 0.05)
+    assert np.all(log_u[rows] < np.log(1e30))
+    assert log_u[others].max() < 20.0
+    if col is not None:
+        assert ex["umax_col"][rows[0]] == col
+    else:
+        # the rows' true-class logits sit below every other class: U = exp(s - s_true) is large in every column
+        Yt = crafted["tgt"].astype(np.float64)
+        s = v[rows] @ Yt.T
+        s[np.arange(len(rows)), target[rows]] = np.inf
+        assert (s.min(axis=1) - np.einsum("bd,bd->b", v[rows], Yt[target[rows]])).min() > R.LOG_U_EDGE - 5.0
