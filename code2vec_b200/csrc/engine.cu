@@ -219,6 +219,8 @@ struct c2v_engine {
   const int32_t* sorted_src = nullptr;   // ws.perm / ws.bkt_starts hold the bucket order of THIS batch (set by the forward pass)
   int sorted_rows = 0;
   InboxSet inbox{};          // push-based gradient exchange (c2v_bind_scatter_inbox); world == 0: not bound
+  int ordered_exchange = 0;  // option "ordered_exchange": sharded tables take sorted per-row sums through the inbox, folded in rank order
+  bool exchange_pushed = false;   // ws.det_starts holds the bounds of an ordered push (option "ordered_exchange_rows")
   int sort_peer = 1;         // option "sort_peer_access": sharded tables are gathered / scattered in (owner, 2 MB page) order
   bool bkt_zeroed = false;   // the bucket counters have been cleared once (bucket_scan_kernel leaves them cleared)
   int recompute = 0;         // option "recompute_logits" (tensor-core modes, single-GPU step): the logits GEMM runs twice -- once for the
@@ -670,10 +672,9 @@ int sort_entries(c2v_engine* e, cudaStream_t st, const ContextSource& cs, const 
 // Option "deterministic": the sum of each referenced gradient row in the fixed order of DESIGN.md section 5.1 -- a stable radix
 // sort of the `count` entries by key (keys in [0, nkeys]; nkeys marks an entry that contributes nothing), then chunk sums and
 // their combine.  Every referenced row is stored (the rows are zero before); no atomics, so the result is the same on every run.
-template <class KeyFn, class Contrib>
-int det_row_sums(c2v_engine* e, cudaStream_t st, const KeyFn& key, int count, uint32_t nkeys, const Contrib& contrib,
-                 const DetDest& dst) {
-  if (count <= 0) return C2V_OK;
+// det_sort leaves the sorted keys / entries in ws.det_keys[*cur] / ws.det_vals[*cur]; the other pair is free afterwards.
+template <class KeyFn>
+int det_sort(c2v_engine* e, cudaStream_t st, const KeyFn& key, int count, uint32_t nkeys, int* cur_out) {
   int bits = 1;
   while (bits < 32 && (1ull << bits) <= nkeys) ++bits;
   uint32_t* keys[2] = {wsp<uint32_t>(e, e->ws.det_keys[0]), wsp<uint32_t>(e, e->ws.det_keys[1])};
@@ -691,11 +692,26 @@ int det_row_sums(c2v_engine* e, cudaStream_t st, const KeyFn& key, int count, ui
     C2V_LAUNCH(e, (det_scatter_kernel<<<tiles, kDetSortThreads, 0, st>>>(keys[cur], vals[cur], count, shift, offs, keys[cur ^ 1],
                                                                          vals[cur ^ 1])));
   }
+  *cur_out = cur;
+  return C2V_OK;
+}
+template <class Contrib, class Dest>
+int det_reduce(c2v_engine* e, cudaStream_t st, int cur, int count, uint32_t nkeys, const Contrib& contrib, const Dest& dst) {
+  const uint32_t* keys = wsp<uint32_t>(e, e->ws.det_keys[cur]);
   const unsigned grid = (unsigned)((count + 255) / 256);
   float* part = wsp<float>(e, e->ws.det_part);
-  C2V_LAUNCH(e, (det_chunk_kernel<Contrib><<<grid, 256, 0, st>>>(keys[cur], vals[cur], count, nkeys, contrib, dst, part)));
-  C2V_LAUNCH(e, (det_combine_kernel<<<grid, 256, 0, st>>>(keys[cur], count, nkeys, dst, part)));
+  C2V_LAUNCH(e, (det_chunk_kernel<Contrib, Dest><<<grid, 256, 0, st>>>(keys, wsp<int32_t>(e, e->ws.det_vals[cur]), count, nkeys, contrib,
+                                                                       dst, part)));
+  C2V_LAUNCH(e, (det_combine_kernel<Dest><<<grid, 256, 0, st>>>(keys, count, nkeys, dst, part)));
   return C2V_OK;
+}
+template <class KeyFn, class Contrib>
+int det_row_sums(c2v_engine* e, cudaStream_t st, const KeyFn& key, int count, uint32_t nkeys, const Contrib& contrib,
+                 const DetDest& dst) {
+  if (count <= 0) return C2V_OK;
+  int cur, rc;
+  if ((rc = det_sort(e, st, key, count, nkeys, &cur))) return rc;
+  return det_reduce(e, st, cur, count, nkeys, contrib, dst);
 }
 
 // The embedding-gradient scatter of a train step in deterministic mode, from dX' in dXg.  simt_order: the contributions are
@@ -708,6 +724,55 @@ int det_scatter(c2v_engine* e, cudaStream_t st, const ContextSource& cs, const f
   if (simt_order)
     return det_row_sums(e, st, key, 3 * cs.rows, key.nkeys, DetStepContrib<true>{dXg, dp, e->grad_scale, d.embed_dim}, dst);
   return det_row_sums(e, st, key, 3 * cs.rows, key.nkeys, DetStepContrib<false>{dXg, dp, e->grad_scale, d.embed_dim}, dst);
+}
+
+// Option "ordered_exchange" on row-sharded tables: is this engine's embedding-gradient scatter the ordered push?
+bool ordered_route(const c2v_engine* e) { return e->ordered_exchange && e->table_world > 1; }
+
+ExchangeKeyMap exchange_key_map(const c2v_engine* e) {
+  const int W = e->table_world, Tl = (e->dims.token_vocab + W - 1) / W, Pl = (e->dims.path_vocab + W - 1) / W;
+  return ExchangeKeyMap{e->gr_tok.shift, e->gr_tok.mask, Tl, Tl + Pl};
+}
+// the owner-major keys, W (Tl + Pl) for masked entries included, must sort as 31-bit numbers on any world size
+bool exchange_keys_fit(const c2v_dims& d) { return (int64_t)d.token_vocab + d.path_vocab + 2 * kMaxShards < INT32_MAX; }
+
+// The sender's half of the ordered exchange (DESIGN.md section 5.1): one fixed-order sum per distinct (owner, table, row) of
+// the `count` entries, stored densely and in key order into this rank's region of each owner's inbox, with the row ids and
+// the two counts.  The head ranks live in the sort's spare entry buffer, the per-tile head counts and their scan in its
+// histogram buffers, and the 2 W + 1 bounds in ws.det_starts: the workspace is that of option "deterministic".
+template <class KeyFn, class Contrib>
+int exchange_push(c2v_engine* e, cudaStream_t st, const KeyFn& key, int count, const Contrib& contrib) {
+  const ExchangeKeyMap map = exchange_key_map(e);
+  const uint32_t nkeys = (uint32_t)e->table_world * map.L;
+  int32_t* bounds = wsp<int32_t>(e, e->ws.det_starts);
+  e->exchange_pushed = true;
+  if (count <= 0) {            // nothing to push: zero counts in every owner's inbox
+    C2V_LAUNCH(e, (exchange_bounds_kernel<<<1, 32, 0, st>>>(nullptr, nullptr, 0, map, e->inbox, bounds)));
+    return C2V_OK;
+  }
+  int cur, rc;
+  if ((rc = det_sort(e, st, key, count, nkeys, &cur))) return rc;
+  const uint32_t* keys = wsp<uint32_t>(e, e->ws.det_keys[cur]);
+  int32_t* head_rank = wsp<int32_t>(e, e->ws.det_vals[cur ^ 1]);
+  int32_t* tile_heads = wsp<int32_t>(e, e->ws.det_hist);
+  int32_t* tile_base = wsp<int32_t>(e, e->ws.det_offs);
+  const int tiles = (count + kDetSortTile - 1) / kDetSortTile;
+  C2V_LAUNCH(e, (det_head_count_kernel<<<tiles, kDetSortThreads, 0, st>>>(keys, count, nkeys, tile_heads)));
+  C2V_LAUNCH(e, (bucket_scan_kernel<<<1, 1024, 0, st>>>(tile_heads, tile_base, bounds, tiles)));
+  C2V_LAUNCH(e, (det_head_rank_kernel<<<tiles, kDetSortThreads, 0, st>>>(keys, count, nkeys, tile_base, head_rank)));
+  C2V_LAUNCH(e, (exchange_bounds_kernel<<<1, 32, 0, st>>>(keys, head_rank, count, map, e->inbox, bounds)));
+  const DetInboxDest dst{e->inbox, head_rank, bounds, map.L, e->dims.embed_dim};
+  C2V_LAUNCH(e, (exchange_ids_kernel<<<(count + 255) / 256, 256, 0, st>>>(keys, count, map, dst)));
+  return det_reduce(e, st, cur, count, nkeys, contrib, dst);
+}
+
+// The embedding-gradient scatter of a train step on row-sharded tables under option "ordered_exchange", from dX' in dXg
+int exchange_scatter(c2v_engine* e, cudaStream_t st, const ContextSource& cs, const float* mask, const Dropout& dp, const float* dXg,
+                     bool simt_order) {
+  const int d = e->dims.embed_dim;
+  const ExchangeStepKeys key{cs.src, cs.pth, cs.tgt, mask, exchange_key_map(e)};
+  if (simt_order) return exchange_push(e, st, key, 3 * cs.rows, DetStepContrib<true>{dXg, dp, e->grad_scale, d});
+  return exchange_push(e, st, key, 3 * cs.rows, DetStepContrib<false>{dXg, dp, e->grad_scale, d});
 }
 
 // Grid of the gather: one wave of resident CTAs (8 warps each; a warp strides over the rows), never more CTAs than rows / 8.
@@ -744,7 +809,7 @@ int run_ctx_fwd(c2v_engine* e, cudaStream_t st, const ContextSource& cs, const D
       PhaseTimer pt(e, PH_GATHER, st);
       BucketPlan bp;
       e->sorted_src = nullptr;
-      if (e->inbox.world > 1 && plan_buckets(e, &bp, true) && !plan_buckets(e, &bp)) {
+      if (e->inbox.world > 1 && !ordered_route(e) && plan_buckets(e, &bp, true) && !plan_buckets(e, &bp)) {
         // the backward pass will push gradient rows owner by owner: bucket the batch now, while the SMs are free (in
         // the backward pass the same three small kernels would queue behind the persistent dW GEMM)
         int rcs = sort_entries(e, st, cs, bp);
@@ -967,6 +1032,9 @@ int context_backward(c2v_engine* e, cudaStream_t st, const ContextSource& cs, co
   float* da_part = wsp<float>(e, e->ws.da_part);
   float* part = wsp<float>(e, e->ws.part);
   int rc;
+  if (ordered_route(e) && e->inbox.world < 2)
+    return fail(e, C2V_ERR_STATE, "ordered_exchange: the gradient rows of row-sharded tables travel through the scatter inbox, "
+                                  "and none is bound (c2v_bind_scatter_inbox)");
   if (!is_tc(e) && (rc = run_pending_dy(e, st))) return rc;     // fp32 path: nothing to overlap with, run it first
   const bool x3 = is_tc(e) && is_3x(e);
   float* H_lo = x3 ? wsp<float>(e, e->ws.H_lo) : nullptr;
@@ -1000,7 +1068,10 @@ int context_backward(c2v_engine* e, cudaStream_t st, const ContextSource& cs, co
     {
       PhaseTimer pt(e, PH_DX_SCATTER, e->side);
       BucketPlan bp;
-      if (e->inbox.world > 1 && plan_buckets(e, &bp, true)) {
+      if (ordered_route(e)) {      // one fixed-order sum per distinct row into the owner's inbox; the owners fold in rank order
+        e->sorted_src = nullptr;
+        if ((rc = exchange_scatter(e, e->side, cs, mask, dp, dXg, false))) return rc;
+      } else if (e->inbox.world > 1 && plan_buckets(e, &bp, true)) {
         // push: every owner's rows go densely into this rank's region of the owner's inbox (plain coalesced stores over
         // NVLink); the owners fold them in with local atomics after the caller's barrier (c2v_apply_scatter_inbox)
         if (e->sorted_src != cs.src || e->sorted_rows != cs.rows) {     // not bucketed by this step's forward pass
@@ -1064,11 +1135,12 @@ int context_backward(c2v_engine* e, cudaStream_t st, const ContextSource& cs, co
     PhaseTimer pt(e, PH_DX_SCATTER, st);
     simt::RowsK al{H, (size_t)D};
     simt::RowsK bl{e->theta.W, (size_t)D};
-    if (e->deterministic) {        // dX' is stored, then summed row by row in a fixed order
+    if (e->deterministic || ordered_route(e)) {        // dX' is stored, then summed row by row in a fixed order
       float* dXg = wsp<float>(e, e->ws.dXg);
       simt::StoreC ep{dXg, (size_t)K3, 0};
       C2V_LAUNCH(e, C2V_CUDA(e, simt::launch(st, N, K3, D, 1, al, bl, ep)));
-      if ((rc = det_scatter(e, st, cs, mask, dp, dXg, true))) return rc;
+      if ((rc = ordered_route(e) ? exchange_scatter(e, st, cs, mask, dp, dXg, true) : det_scatter(e, st, cs, mask, dp, dXg, true)))
+        return rc;
     } else {
       simt::ScatterDx ep{cs, e->gr_tok, e->gr_path, mask, dp, e->grad_scale};
       C2V_LAUNCH(e, C2V_CUDA(e, simt::launch(st, N, K3, D, 1, al, bl, ep)));
@@ -1592,12 +1664,22 @@ int c2v_set_option(c2v_engine* e, const char* key, int64_t value) {
   }
   if (!strcmp(key, "deterministic")) {
     if (value != 0 && value != 1) return fail(e, C2V_ERR_INVALID, "deterministic must be 0 or 1");
-    if (value && e->table_world > 1)
+    if (value && e->table_world > 1 && !e->ordered_exchange)
       return fail(e, C2V_ERR_UNSUPPORTED, "deterministic: the embedding tables are row-sharded over more than one rank, and the "
                                           "cross-rank red.add scatter into them is order-free");
     if (value && (int64_t)e->dims.token_vocab + e->dims.path_vocab >= INT32_MAX)
       return fail(e, C2V_ERR_UNSUPPORTED, "deterministic: token_vocab + path_vocab must be below 2^31");
     e->deterministic = (int)value;
+    return C2V_OK;
+  }
+  if (!strcmp(key, "ordered_exchange")) {
+    if (value != 0 && value != 1) return fail(e, C2V_ERR_INVALID, "ordered_exchange must be 0 or 1");
+    if (!value && e->deterministic && e->table_world > 1)
+      return fail(e, C2V_ERR_UNSUPPORTED, "ordered_exchange: deterministic is set and the embedding tables are row-sharded over "
+                                          "more than one rank; the other exchanges are order-free (set deterministic to 0 first)");
+    if (value && !exchange_keys_fit(e->dims))
+      return fail(e, C2V_ERR_UNSUPPORTED, "ordered_exchange: the padded rows of both tables over all ranks must be below 2^31");
+    e->ordered_exchange = (int)value;
     return C2V_OK;
   }
   if (!strcmp(key, "profile")) { e->profile = value ? 1 : 0; return C2V_OK; }
@@ -1698,6 +1780,18 @@ int c2v_get_option(const c2v_engine* e, const char* key, int64_t* value) {
   if (!e || !key || !value) return C2V_ERR_INVALID;
   if (!strcmp(key, "math_mode")) { *value = e->math_mode; return C2V_OK; }
   if (!strcmp(key, "deterministic")) { *value = e->deterministic; return C2V_OK; }
+  if (!strcmp(key, "ordered_exchange")) { *value = e->ordered_exchange; return C2V_OK; }
+  if (!strcmp(key, "ordered_exchange_rows")) {    // (row, sum) records this rank pushed in its last step, over all owners (synchronises)
+    *value = 0;
+    if (e->wbase && e->exchange_pushed) {
+      int32_t n = 0;
+      if (cudaDeviceSynchronize() != cudaSuccess ||
+          cudaMemcpy(&n, e->wbase + e->ws.det_starts + (size_t)2 * e->table_world * 4, 4, cudaMemcpyDeviceToHost) != cudaSuccess)
+        return C2V_ERR_CUDA;
+      *value = n;
+    }
+    return C2V_OK;
+  }
   if (!strcmp(key, "profile")) { *value = e->profile; return C2V_OK; }
   if (!strcmp(key, "lazy_adam")) { *value = e->lazy; return C2V_OK; }
   if (!strcmp(key, "adam_sweep_period")) { *value = e->sweep_period; return C2V_OK; }
@@ -1880,7 +1974,7 @@ int c2v_bind_table_shards(c2v_engine* e, const c2v_table_shards* params, const c
   const int w = params->world;
   if (!(w == 1 || w == 2 || w == 4 || w == 8)) return fail(e, C2V_ERR_INVALID, "world must be 1, 2, 4 or 8");
   if (grads && grads->world != w) return fail(e, C2V_ERR_INVALID, "params / grads world mismatch");
-  if (e->deterministic && w > 1)
+  if (e->deterministic && w > 1 && !e->ordered_exchange)
     return fail(e, C2V_ERR_UNSUPPORTED, "deterministic is set: row-sharded tables over more than one rank take order-free "
                                         "cross-rank red.adds (set deterministic to 0 first)");
   int shift = 0;
@@ -1929,8 +2023,12 @@ int c2v_apply_scatter_inbox(c2v_engine* e, void* stream) {
   C2V_CUDA(e, cudaSetDevice(e->device));
   cudaStream_t st = (cudaStream_t)stream;
   PhaseTimer pt(e, PH_INBOX_APPLY, st);
-  C2V_LAUNCH(e, (inbox_apply_kernel<<<e->num_sms * 8, 256, 0, st>>>(e->inbox, e->dims.embed_dim, e->gr_tok.base[e->inbox.rank],
-                                                                    e->gr_path.base[e->inbox.rank])));
+  float* g_tok = e->gr_tok.base[e->inbox.rank];
+  float* g_path = e->gr_path.base[e->inbox.rank];
+  if (ordered_route(e))        // the senders' sorted row sums, added per row in sender order and stored
+    C2V_LAUNCH(e, (inbox_fold_ordered_kernel<<<e->num_sms * 8, 256, 0, st>>>(e->inbox, e->dims.embed_dim, g_tok, g_path)));
+  else
+    C2V_LAUNCH(e, (inbox_apply_kernel<<<e->num_sms * 8, 256, 0, st>>>(e->inbox, e->dims.embed_dim, g_tok, g_path)));
   // the fold consumes the rows: a step that pushes nothing (the fp32 scatter red.adds straight into the shards) leaves
   // zero counts, so the next fold cannot add the previous step's rows a second time
   C2V_CUDA(e, cudaMemsetAsync(e->inbox.base[e->inbox.rank], 0, (size_t)e->inbox.world * 2 * 4, st));
@@ -2267,6 +2365,27 @@ int c2v_selftest_row_sum(c2v_engine* e, int32_t table_id, const int32_t* rows, c
   const DetDest dst{out, out, d.token_vocab, d.embed_dim};
   return det_row_sums(e, (cudaStream_t)stream, DetListKeys{rows, table_id ? d.token_vocab : 0}, count,
                       (uint32_t)(d.token_vocab + d.path_vocab), DetListContrib{vals, d.embed_dim}, dst);
+}
+
+int c2v_selftest_exchange_push(c2v_engine* e, const int32_t* tok_rows, const float* tok_vals, int32_t n_tok,
+                               const int32_t* path_rows, const float* path_vals, int32_t n_path, void* stream) {
+  if (!e || n_tok < 0 || n_path < 0) return C2V_ERR_INVALID;
+  if ((n_tok && (!tok_rows || !tok_vals)) || (n_path && (!path_rows || !path_vals))) return fail(e, C2V_ERR_INVALID, "NULL list");
+  if (!e->wbase) return fail(e, C2V_ERR_STATE, "workspace not bound (c2v_bind_workspace)");
+  if (!ordered_route(e)) return fail(e, C2V_ERR_STATE, "set ordered_exchange and bind row-sharded tables over more than one rank first");
+  if (e->inbox.world < 2) return fail(e, C2V_ERR_STATE, "no scatter inbox bound (c2v_bind_scatter_inbox)");
+  if ((int64_t)n_tok + n_path > 3ll * e->dims.max_batch * e->dims.max_contexts)
+    return fail(e, C2V_ERR_INVALID, "n_tok + n_path must be at most 3 * max_batch * max_contexts");
+  if (((uintptr_t)tok_vals | (uintptr_t)path_vals) % 16) return fail(e, C2V_ERR_INVALID, "tok_vals and path_vals must be 16-byte aligned");
+  C2V_CUDA(e, cudaSetDevice(e->device));
+  cudaStream_t st = (cudaStream_t)stream;
+  // one [n_tok + n_path, d] list of contributions, in the dX' region (it holds 3 * max_batch * max_contexts rows of d)
+  const size_t d = (size_t)e->dims.embed_dim;
+  float* vals = wsp<float>(e, e->ws.dXg);
+  if (n_tok) C2V_CUDA(e, cudaMemcpyAsync(vals, tok_vals, n_tok * d * 4, cudaMemcpyDeviceToDevice, st));
+  if (n_path) C2V_CUDA(e, cudaMemcpyAsync(vals + n_tok * d, path_vals, n_path * d * 4, cudaMemcpyDeviceToDevice, st));
+  return exchange_push(e, st, ExchangeListKeys{tok_rows, path_rows, n_tok, exchange_key_map(e)}, n_tok + n_path,
+                       DetListContrib{vals, (int)d});
 }
 
 int64_t c2v_launch_count(const c2v_engine* e) { return e ? e->launches : 0; }

@@ -1615,12 +1615,13 @@ struct DetListContrib {
   }
 };
 
-// where key k's row lives: token table for k < T, path table otherwise (the tables are local: one shard at most)
+// Where the finished sum of key k's row goes (`first`: the sorted position of the row's first entry).
+// DetDest: into the row itself -- token table for k < T, path table otherwise (the tables are local: one shard at most)
 struct DetDest {
   float* tok;
   float* path;
   int T, d;
-  __device__ __forceinline__ float* row(uint32_t k) const {
+  __device__ __forceinline__ float* row(uint32_t k, int /*first*/) const {
     return (int)k < T ? tok + (size_t)k * d : path + (size_t)((int)k - T) * d;
   }
 };
@@ -1636,10 +1637,10 @@ __device__ __forceinline__ size_t det_slot(int i, bool first) { return 2 * (size
 
 // Pass 1: one warp per 32 sorted positions; every position that starts a chunk (its offset from its row's first entry is a
 // multiple of K) is summed by the warp.  A row of one chunk is stored; otherwise the chunk sum goes to its partial slot.
-template <class Contrib>
+template <class Contrib, class Dest>
 __global__ void __launch_bounds__(256)
 det_chunk_kernel(const uint32_t* __restrict__ keys, const int32_t* __restrict__ vals, int count, uint32_t nkeys,
-                 const __grid_constant__ Contrib contrib, const __grid_constant__ DetDest dst, float* __restrict__ part) {
+                 const __grid_constant__ Contrib contrib, const __grid_constant__ Dest dst, float* __restrict__ part) {
   const int lane = threadIdx.x & 31;
   const int i = blockIdx.x * 256 + threadIdx.x;
   bool start = false;
@@ -1671,15 +1672,16 @@ det_chunk_kernel(const uint32_t* __restrict__ keys, const int32_t* __restrict__ 
     for (int c4 = lane; c4 < d4; c4 += 32) {
       float4 acc = make_float4(0.f, 0.f, 0.f, 0.f);
       for (int j = p; j < end; ++j) acc = add4_rn(acc, contrib(vals[j], c4));
-      float* out = single ? dst.row(kk) : part + det_slot(p, p == f) * dst.d;
+      float* out = single ? dst.row(kk, f) : part + det_slot(p, p == f) * dst.d;
       reinterpret_cast<float4*>(out)[c4] = acc;
     }
   }
 }
 
 // Pass 2: the first position of every row with more than one chunk adds the row's chunk sums in order and stores the row.
+template <class Dest>
 __global__ void __launch_bounds__(256)
-det_combine_kernel(const uint32_t* __restrict__ keys, int count, uint32_t nkeys, const __grid_constant__ DetDest dst,
+det_combine_kernel(const uint32_t* __restrict__ keys, int count, uint32_t nkeys, const __grid_constant__ Dest dst,
                    const float* __restrict__ part) {
   const int lane = threadIdx.x & 31;
   const int i = blockIdx.x * 256 + threadIdx.x;
@@ -1696,11 +1698,205 @@ det_combine_kernel(const uint32_t* __restrict__ keys, int count, uint32_t nkeys,
     todo &= todo - 1;
     const int f = __shfl_sync(0xffffffffu, i, b);
     const uint32_t kk = __shfl_sync(0xffffffffu, k, b);
+    float4* out = reinterpret_cast<float4*>(dst.row(kk, f));
     for (int c4 = lane; c4 < d4; c4 += 32) {
       float4 acc = make_float4(0.f, 0.f, 0.f, 0.f);
       for (int p = f; p < count && keys[p] == kk; p += kDetChunk)
         acc = add4_rn(acc, reinterpret_cast<const float4*>(part + det_slot(p, p == f) * dst.d)[c4]);
-      reinterpret_cast<float4*>(dst.row(kk))[c4] = acc;
+      out[c4] = acc;
+    }
+  }
+}
+
+// ---------------------------------------------------------------------------------------------
+// Ordered gradient exchange for row-sharded tables (option "ordered_exchange", DESIGN.md section 5.1).
+//
+// Sender: the entries are keyed owner-major -- key = o L + (path table ? Tl + rho : rho) for global row r with owner
+// o = r % W and local row rho = r / W, Tl / Pl rows per token / path shard, L = Tl + Pl; W L for masked contexts -- and
+// sorted and reduced as above, so each distinct (owner, table, row) ends as ONE ordered sum.  The sums of owner o lie in key
+// order, token rows before path rows: the k-th of them goes into slot k of this rank's region of o's inbox (the layout of
+// the plain push: row ids, values, two counts per sender), where k is the row's head rank -- the exclusive scan of "sorted
+// position starts a row" -- minus the head rank at o's first position.
+// Owner: inbox_fold_ordered_kernel adds the senders' sums of a row in sender order and stores the row.
+// ---------------------------------------------------------------------------------------------
+struct ExchangeKeyMap {
+  int shift, mask;     // as ShardedTable: owner = r & mask, local row = r >> shift
+  int Tl, L;           // token rows per shard; token + path rows per shard
+  __device__ __forceinline__ uint32_t key(int r, bool path) const {
+    return (uint32_t)((r & mask) * L + (path ? Tl : 0) + (r >> shift));
+  }
+  __device__ __forceinline__ uint32_t nkeys() const { return (uint32_t)((mask + 1) * L); }
+};
+// key of entry e of a train step's batch
+struct ExchangeStepKeys {
+  const int32_t* src;
+  const int32_t* pth;
+  const int32_t* tgt;
+  const float* mask;
+  ExchangeKeyMap map;
+  __device__ __forceinline__ uint32_t operator()(int e) const {
+    const int n = e / 3, seg = e - 3 * n;
+    if (mask[n] == 0.f) return map.nkeys();
+    return map.key(seg == 0 ? src[n] : (seg == 1 ? pth[n] : tgt[n]), seg == 1);
+  }
+};
+// key of entry e of c2v_selftest_exchange_push: n_tok global token rows, then global path rows
+struct ExchangeListKeys {
+  const int32_t* tok_rows;
+  const int32_t* path_rows;
+  int n_tok;
+  ExchangeKeyMap map;
+  __device__ __forceinline__ uint32_t operator()(int e) const {
+    return e < n_tok ? map.key(tok_rows[e], false) : map.key(path_rows[e - n_tok], true);
+  }
+};
+
+__device__ __forceinline__ bool det_is_head(const uint32_t* __restrict__ keys, int i, uint32_t nkeys) {
+  const uint32_t k = keys[i];
+  return k < nkeys && (i == 0 || keys[i - 1] != k);
+}
+
+// tile_heads[tile] = rows that start inside the tile of kDetSortTile sorted positions
+__global__ void __launch_bounds__(kDetSortThreads)
+det_head_count_kernel(const uint32_t* __restrict__ keys, int count, uint32_t nkeys, int32_t* __restrict__ tile_heads) {
+  const int lo = blockIdx.x * kDetSortTile, hi = min(count, lo + kDetSortTile);
+  int n = 0;
+  for (int i = lo + threadIdx.x; i < hi; i += kDetSortThreads) n += det_is_head(keys, i, nkeys) ? 1 : 0;
+  __shared__ int32_t total;
+  if (threadIdx.x == 0) total = 0;
+  __syncthreads();
+  n = __reduce_add_sync(0xffffffffu, n);
+  if ((threadIdx.x & 31) == 0 && n) atomicAdd(&total, n);
+  __syncthreads();
+  if (threadIdx.x == 0) tile_heads[blockIdx.x] = total;
+}
+
+// head_rank[i] = rows that start before sorted position i (tile_base = exclusive scan of tile_heads)
+__global__ void __launch_bounds__(kDetSortThreads)
+det_head_rank_kernel(const uint32_t* __restrict__ keys, int count, uint32_t nkeys, const int32_t* __restrict__ tile_base,
+                     int32_t* __restrict__ head_rank) {
+  constexpr int W = kDetSortThreads / 32;
+  __shared__ int32_t wc[W];
+  const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+  const int lo = blockIdx.x * kDetSortTile, hi = min(count, lo + kDetSortTile);
+  int run = tile_base[blockIdx.x];
+  for (int base = lo; base < hi; base += kDetSortThreads) {
+    const int i = base + threadIdx.x;
+    const bool head = i < hi && det_is_head(keys, i, nkeys);
+    const unsigned heads = __ballot_sync(0xffffffffu, head);
+    if (lane == 0) wc[warp] = __popc(heads);
+    __syncthreads();
+    int before = 0, all = 0;
+#pragma unroll
+    for (int w = 0; w < W; ++w) { before += w < warp ? wc[w] : 0; all += wc[w]; }
+    if (i < hi) head_rank[i] = run + before + __popc(heads & ((1u << lane) - 1u));
+    run += all;
+    __syncthreads();
+  }
+}
+
+// rows that start before the first sorted position whose key is >= k
+__device__ __forceinline__ int exchange_heads_below(const uint32_t* __restrict__ keys, const int32_t* __restrict__ head_rank,
+                                                    int count, uint32_t nkeys, uint32_t k) {
+  if (count == 0) return 0;
+  int lo = 0, hi = count;
+  while (lo < hi) {
+    const int mid = (lo + hi) >> 1;
+    if (keys[mid] < k) lo = mid + 1; else hi = mid;
+  }
+  if (lo < count) return head_rank[lo];
+  return head_rank[count - 1] + (det_is_head(keys, count - 1, nkeys) ? 1 : 0);
+}
+
+// bounds[2 o] / bounds[2 o + 1] = head rank at the first token / path key of owner o, bounds[2 W] = distinct rows in all;
+// the two counts of this sender go into every owner's inbox
+__global__ void exchange_bounds_kernel(const uint32_t* __restrict__ keys, const int32_t* __restrict__ head_rank, int count,
+                                       const __grid_constant__ ExchangeKeyMap map, const __grid_constant__ InboxSet inbox,
+                                       int32_t* __restrict__ bounds) {
+  __shared__ int32_t b[2 * kMaxShards + 1];
+  const int j = threadIdx.x, W = map.mask + 1;
+  if (j <= 2 * W) {
+    b[j] = exchange_heads_below(keys, head_rank, count, map.nkeys(), (uint32_t)((j >> 1) * map.L + (j & 1) * map.Tl));
+    bounds[j] = b[j];
+  }
+  __syncthreads();
+  if (j < W) {
+    InboxView v = inbox_of(inbox, j);
+    v.cnt[2 * inbox.rank] = b[2 * j + 1] - b[2 * j];
+    v.cnt[2 * inbox.rank + 1] = b[2 * j + 2] - b[2 * j + 1];
+  }
+}
+
+// the inbox slot of key k's row, from the sorted position of the row's first entry
+struct DetInboxDest {
+  InboxSet inbox;
+  const int32_t* head_rank;
+  const int32_t* bounds;
+  int L, d;
+  __device__ __forceinline__ size_t slot(uint32_t k, int first) const {
+    return (size_t)inbox.rank * inbox.cap + (size_t)(head_rank[first] - bounds[2 * (k / (uint32_t)L)]);
+  }
+  __device__ __forceinline__ float* row(uint32_t k, int first) const {
+    return inbox_of(inbox, (int)(k / (uint32_t)L)).val + slot(k, first) * d;
+  }
+};
+
+// ids[slot] = local row, for every row this sender pushes
+__global__ void __launch_bounds__(256)
+exchange_ids_kernel(const uint32_t* __restrict__ keys, int count, const __grid_constant__ ExchangeKeyMap map,
+                    const __grid_constant__ DetInboxDest dst) {
+  const int i = blockIdx.x * 256 + threadIdx.x;
+  if (i >= count || !det_is_head(keys, i, map.nkeys())) return;
+  const uint32_t k = keys[i];
+  const int o = (int)(k / (uint32_t)map.L), rem = (int)(k - (uint32_t)o * map.L);
+  inbox_of(dst.inbox, o).ids[dst.slot(k, i)] = rem < map.Tl ? rem : rem - map.Tl;
+}
+
+// position of `row` in the strictly increasing list ids[0, n), or -1
+__device__ __forceinline__ int exchange_find(const int32_t* __restrict__ ids, int n, int row) {
+  int lo = 0, hi = n;
+  while (lo < hi) {
+    const int mid = (lo + hi) >> 1;
+    if (ids[mid] < row) lo = mid + 1; else hi = mid;
+  }
+  return (lo < n && ids[lo] == row) ? lo : -1;
+}
+
+// The owner's half: one warp per (sender s, slot k) of this rank's inbox.  The warp of the lowest sender that lists a row
+// leads it: from +0.0f it adds the row's sums of senders s, s + 1, ... in that order (each sender lists a row at most once,
+// in increasing row order per table: binary search) and stores the row.  No atomics; persistent grid.
+__global__ void __launch_bounds__(256)
+inbox_fold_ordered_kernel(const __grid_constant__ InboxSet inbox, int d, float* __restrict__ g_tok, float* __restrict__ g_path) {
+  const int lane = threadIdx.x & 31;
+  const int warp_global = (blockIdx.x * 256 + threadIdx.x) >> 5, total_warps = (gridDim.x * 256) >> 5;
+  const InboxView v = inbox_of(inbox, inbox.rank);
+  for (int s = 0; s < inbox.world; ++s) {
+    const int n_tok = v.cnt[2 * s], n_all = n_tok + v.cnt[2 * s + 1];
+    for (int k = warp_global; k < n_all; k += total_warps) {
+      const bool path = k >= n_tok;
+      const int row = v.ids[(size_t)s * inbox.cap + k];
+      // the list of the row's table in sender t's region: [begin, begin + n)
+      auto find = [&](int t) {
+        const int t_tok = v.cnt[2 * t];
+        const size_t begin = (size_t)t * inbox.cap + (path ? t_tok : 0);
+        const int q = exchange_find(v.ids + begin, path ? v.cnt[2 * t + 1] : t_tok, row);
+        return q < 0 ? (size_t)-1 : begin + q;
+      };
+      bool lead = true;
+      for (int t = 0; t < s && lead; ++t) lead = find(t) == (size_t)-1;
+      if (!lead) continue;
+      size_t at[kMaxShards];
+#pragma unroll
+      for (int t = 0; t < kMaxShards; ++t)
+        at[t] = t == s ? (size_t)s * inbox.cap + k : ((t > s && t < inbox.world) ? find(t) : (size_t)-1);
+      float* dst = (path ? g_path : g_tok) + (size_t)row * d;
+      for (int j = lane * 4; j < d; j += 128) {
+        float4 acc = make_float4(0.f, 0.f, 0.f, 0.f);
+#pragma unroll
+        for (int t = 0; t < kMaxShards; ++t)
+          if (at[t] != (size_t)-1) acc = add4_rn(acc, *reinterpret_cast<const float4*>(v.val + at[t] * d + j));
+        *reinterpret_cast<float4*>(dst + j) = acc;
+      }
     }
   }
 }

@@ -91,6 +91,7 @@ _SIGNATURES = {
     "c2v_selftest_split": (C.c_int, [_P, _P, _P, _P, C.c_size_t, _P]),
     "c2v_selftest_transpose": (C.c_int, [_P, _P, _I32, _I32, _P, _P, C.c_size_t, _P]),
     "c2v_selftest_row_sum": (C.c_int, [_P, _I32, _P, _P, _I32, _P, _P]),
+    "c2v_selftest_exchange_push": (C.c_int, [_P, _P, _P, _I32, _P, _P, _I32, _P]),
     "c2v_set_event": (C.c_int, [_P, C.c_char_p, _P]),
     "c2v_sync_tables": (C.c_int, [_P, _P]),
     "c2v_context_forward": (C.c_int, [_P, _P, _P, _P, _P, _I32, C.c_float, C.c_uint64, C.c_uint64, _P, _P, _P]),
@@ -332,6 +333,18 @@ class PathAttentionEngine:
                                                   out.data_ptr(), self._stream()))
         return out
 
+    def selftest_exchange_push(self, tok_rows, tok_vals, path_rows, path_vals):
+        """Test hook for option "ordered_exchange" (c2v_selftest_exchange_push): this rank pushes tok_vals[i] for GLOBAL token
+        row tok_rows[i] and path_vals[i] for global path row path_rows[i] (int32 [n], float32 [n, embed_dim]) into the
+        owners' inboxes, one ordered sum per distinct row.  Barrier, then apply_scatter_inbox() on every rank."""
+        torch = self.torch
+        i32 = lambda t: torch.as_tensor(t).to(device=self.dev, dtype=torch.int32).contiguous()
+        f32 = lambda t: torch.as_tensor(t).to(device=self.dev, dtype=torch.float32).contiguous()
+        tr, tv, pr, pv = i32(tok_rows), f32(tok_vals), i32(path_rows), f32(path_vals)
+        self._check(self.lib.c2v_selftest_exchange_push(self.h, _ptr(tr), _ptr(tv), int(tr.numel()), _ptr(pr), _ptr(pv),
+                                                        int(pr.numel()), self._stream()))
+        torch.cuda.current_stream(self.dev).synchronize()       # the lists above may be freed on return
+
     def phase_stats(self, reset: bool = False) -> Dict[str, Tuple[float, int]]:
         """{phase name: (total device ms, number of timed occurrences)} since the last reset
         (needs set_option("profile", 1)).  Synchronises the device."""
@@ -526,12 +539,14 @@ class PathAttentionEngine:
         the cross-rank barrier that follows every rank's backward pass)."""
         self._check(self.lib.c2v_apply_scatter_inbox(self.h, self._stream()))
 
-    def enable_table_sharding(self, group=None, push_grads: bool = False):
+    def enable_table_sharding(self, group=None, push_grads: bool = False, ordered_exchange: bool = False):
         """Re-homes WORDS_VOCAB / PATHS_VOCAB (+ gradients, Adam slots) as row-interleaved shards: global
         row r -> rank r % world, local row r // world.  Parameter and gradient shards live in
         cudaMalloc'ed memory whose CUDA-IPC handles are exchanged once, so every rank's kernels can
         load rows from, and red.add gradients into, every other rank's shard over NVLink.  The current
-        contents of the replicated tables are carried over."""
+        contents of the replicated tables are carried over.  push_grads: gradient rows go through a per-rank inbox instead
+        of red.adds; ordered_exchange: through the inbox as sorted per-row sums that the owners fold in rank order (engine
+        option "ordered_exchange"), which is what option "deterministic" needs on sharded tables."""
         import torch.distributed as dist
         torch = self.torch
         world, rank = dist.get_world_size(group), dist.get_rank(group)
@@ -542,7 +557,11 @@ class PathAttentionEngine:
         d = self.dims.embed_dim
         rows = {"tok": (self.dims.token_vocab + world - 1) // world, "path": (self.dims.path_vocab + world - 1) // world}
         own, handles = {}, {}
-        self.push_grads = bool(push_grads) and self.training and world > 1
+        self.ordered_exchange = bool(ordered_exchange) and self.training and world > 1
+        if self.ordered_exchange:
+            self.set_option("ordered_exchange", 1)
+        # push_grads also says "an inbox is bound: fold it after the step's barrier", which holds for both routes
+        self.push_grads = (bool(push_grads) and self.training and world > 1) or self.ordered_exchange
         if self.push_grads:          # one inbox per rank for the embedding-gradient rows its peers push (c2v_bind_scatter_inbox)
             cd = self.dims.to_c()
             nbytes = self.lib.c2v_scatter_inbox_bytes(C.byref(cd), world)

@@ -135,11 +135,12 @@ def make_fully_sharded_engine(dims, local_batch: int, device: int, group=None, t
     return eng
 
 
-def deterministic_refusal(schedule: str, world: int, push_grads: bool) -> Optional[str]:
+def deterministic_refusal(schedule: str, world: int, push_grads: bool, ordered_exchange: bool = False) -> Optional[str]:
     """Why `schedule` on `world` ranks cannot run with the engine option "deterministic", or None if it can.  The option
     fixes the order of every reduction into tables the engine holds itself; row-sharded tables over several ranks take
-    order-free cross-rank red.adds (or inbox folds).  NCCL's own reduction order (allreduce / sharded) is outside it."""
-    if schedule in ("table_sharded", "fully_sharded") and world > 1:
+    order-free cross-rank red.adds (or inbox folds) unless ordered_exchange sends sorted per-row sums that the owners
+    fold in rank order.  NCCL's own reduction order (allreduce / sharded) is outside it."""
+    if schedule in ("table_sharded", "fully_sharded") and world > 1 and not ordered_exchange:
         if push_grads:
             return ("deterministic training is not available with the %s schedule on %d ranks: peers push embedding "
                     "gradients into a scatter inbox that is folded with atomics" % (schedule, world))
@@ -159,7 +160,7 @@ class Trainer:
     def __init__(self, engine: PathAttentionEngine, keep_prob: float = 0.75, seed: int = 0, group=None,
                  adam: Optional[dict] = None, schedule: str = "table_sharded", lazy_adam: bool = True,
                  fuse_target_adam: bool = True, push_grads: bool = False, allow_single_rank: bool = False,
-                 deterministic: bool = False):
+                 deterministic: bool = False, ordered_exchange: bool = False):
         self.e = engine
         self.keep = float(keep_prob)
         self.seed = int(seed)
@@ -177,16 +178,18 @@ class Trainer:
         if self.schedule in ("table_sharded", "fully_sharded") and self.world not in (1, 2, 4, 8):
             self.schedule = "sharded"
         # deterministic: every step's results depend only on its inputs, seeds and options (engine option "deterministic")
+        # ordered_exchange: the row-sharded schedules send embedding gradients as sorted per-row sums through the scatter
+        # inbox and the owners fold them in rank order (engine option "ordered_exchange"); deterministic needs it there
         self.deterministic = bool(deterministic)
         if self.deterministic:
-            why = deterministic_refusal(self.schedule, self.world, push_grads)
+            why = deterministic_refusal(self.schedule, self.world, push_grads, ordered_exchange)
             if why:
-                raise ValueError(why)
+                raise ValueError(why + "; pass ordered_exchange=True")
         if self.schedule == "fully_sharded":
             if not hasattr(engine, "target_row0"):
                 raise ValueError("the fully_sharded schedule needs an engine from make_fully_sharded_engine()")
             with torch.cuda.device(engine.dev):
-                engine.enable_table_sharding(group, push_grads=push_grads)
+                engine.enable_table_sharding(group, push_grads=push_grads, ordered_exchange=ordered_exchange)
             engine.set_option("grad_scale_inverse", 1)     # dv already carries the 1/global-batch factor
             Bl, Bt, D = engine.local_batch, engine.local_batch * self.world, engine.dims.code_dim
             f32, i32, dev = torch.float32, torch.int32, engine.dev
@@ -212,7 +215,7 @@ class Trainer:
                              target=torch.empty((B,), dtype=i32, device=engine.dev))
         if self.schedule == "table_sharded":
             with torch.cuda.device(engine.dev):
-                engine.enable_table_sharding(group, push_grads=push_grads)
+                engine.enable_table_sharding(group, push_grads=push_grads, ordered_exchange=ordered_exchange)
             (a0, a1), _ = engine.bucket_bounds()
             layout, total = engine.flat_layout()
             small0 = [off for k, off, n in layout if k == "W"][0]         # W, a: the tail of the flat buffer

@@ -115,8 +115,18 @@ int c2v_bind_adam_state(c2v_engine* e, const c2v_tensors* m, const c2v_tensors* 
  * the sums over b of dl[b,1+s] v_b in chunks of 64 examples, chunk by chunk.  Refused (C2V_ERR_UNSUPPORTED) while the
  * embedding tables are row-sharded over more than one rank (c2v_bind_table_shards, world > 1; a scatter inbox can only be
  * bound on top of that) -- their cross-rank red.adds and inbox folds stay order-free -- and binding such shards while it
- * is set fails the same way.  The order in which NCCL reduces
- * the gradients of data-parallel schedules is outside this guarantee), "cta_pair"
+ * is set fails the same way -- unless "ordered_exchange" is set.  The order in which NCCL reduces
+ * the gradients of data-parallel schedules is outside this guarantee), "ordered_exchange" (0/1, default 0; no effect on
+ * one rank.  With 1, a train step or c2v_context_backward on tables row-sharded over W > 1 ranks sends embedding gradients
+ * through the scatter inbox in a fixed order, in every math mode, and "deterministic" is accepted on such tables: each
+ * sender s reduces its own entries of a row to ONE sum R_s in the order "deterministic" documents and pushes one (local
+ * row, R_s) record per distinct row, sorted by row, and c2v_apply_scatter_inbox stores G, where G = +0.0f and then
+ * G = fl(G + R_s) for s = 0 .. W-1, skipping senders without an entry for the row (the shard's gradient rows must be zero
+ * before the step; rows nobody references are not written).  Same inputs, seeds, options, build and world size then give
+ * the same bits; a single engine on the global batch associates differently.  Needs c2v_bind_scatter_inbox: a backward
+ * pass without one fails with C2V_ERR_STATE.  Cannot be cleared (C2V_ERR_UNSUPPORTED) while "deterministic" is set on
+ * tables sharded over more than one rank; refused unless token_vocab + path_vocab + 16 < 2^31), "ordered_exchange_rows"
+ * (read-only: the records this rank pushed in its last ordered exchange, summed over owners; synchronises), "cta_pair"
  * (0, 1 or 2, default 2: accepted for ABI compatibility
  * (it once selected CTA-pair GEMMs); the sm_90a GEMM has no CTA-pair form and ignores it), "dy_late" (where the target-table gradient GEMM dY = P^T.v -- with the
  * target table's Adam step in its epilogue when armed -- runs: 0 = right after dv on the caller's
@@ -337,6 +347,9 @@ int c2v_bind_table_shards(c2v_engine* e, const c2v_table_shards* params, const c
  * plain coalesced stores; after the caller's cross-rank barrier (the same one that ordered the remote red.adds before)
  * each owner folds its inbox into its own gradient shards with local atomics (c2v_apply_scatter_inbox).  The fold
  * consumes the inbox: a step that pushed nothing (fp32 red.adds straight into the shards) then folds nothing.
+ * With option "ordered_exchange" the same inbox carries one fixed-order sum per distinct (owner, table, row) of each
+ * sender, token rows then path rows, each list strictly increasing in the local row id, and the fold adds the senders'
+ * sums of a row in sender-rank order without atomics and stores the row (see the option).
  * inbox[r] = rank r's inbox as mapped into this process (r == rank: the local allocation). */
 size_t c2v_scatter_inbox_bytes(const c2v_dims* dims, int32_t world);
 int c2v_bind_scatter_inbox(c2v_engine* e, void* const* inbox, int32_t world, int32_t rank);
@@ -415,6 +428,15 @@ int c2v_selftest_transpose(c2v_engine* e, const float* x, int32_t rows, int32_t 
  * max_contexts; rows must be in range; vals and out are 16-byte aligned device pointers. */
 int c2v_selftest_row_sum(c2v_engine* e, int32_t table_id, const int32_t* rows, const float* vals, int32_t count,
                          float* out, void* stream);
+
+/* Test hook for option "ordered_exchange": the sender's half of the exchange on caller-given contributions instead of
+ * dX' (no dropout, no scaling).  GLOBAL token row tok_rows[i] receives tok_vals[i, 0:d] and global path row path_rows[i]
+ * receives path_vals[i, 0:d]; per distinct row the contributions are summed in list order as "deterministic" documents
+ * and pushed into the owners' inboxes.  The caller then barriers and calls c2v_apply_scatter_inbox on every rank.  Needs
+ * the option set, shards bound over more than one rank and an inbox bound; n_tok + n_path <= 3 * max_batch *
+ * max_contexts; rows in range; 16-byte aligned device pointers (a list of length 0 may be NULL). */
+int c2v_selftest_exchange_push(c2v_engine* e, const int32_t* tok_rows, const float* tok_vals, int32_t n_tok,
+                               const int32_t* path_rows, const float* path_vals, int32_t n_path, void* stream);
 
 /* Introspection for tests and bench: number of kernels the engine has launched so far. */
 int64_t c2v_launch_count(const c2v_engine* e);
