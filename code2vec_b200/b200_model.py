@@ -7,9 +7,13 @@ Where the reference's TensorFlow backend (tensorflow_model.py:18-447) builds a g
     predict()  : c2v_predict_batch_host, batch of 1, normalised scores + attention           (:331-335)
 Host-side bookkeeping (logging cadence, save/evaluate cadence, log.txt, .vectors, metrics) follows
 the reference method by method; the citations are on each method.
+Under torch.distributed.run with WORLD_SIZE = 2, 4 or 8, train() and evaluate() run the fully sharded schedule: every
+rank takes its slice of each global batch, rank 0 logs and writes the files, and the checkpoint is written and read by
+all ranks in the one-GPU format (multi_rank.py, DESIGN.md §6c).
 """
 from __future__ import annotations
 
+import contextlib
 import json
 import os
 import struct
@@ -25,8 +29,16 @@ from .config import Config
 from .engine import PARAM_NAMES, EngineDims, PathAttentionEngine
 from .model_base import Code2VecModelBase, ModelEvaluationResults, ModelPredictionResults
 from .path_context_reader import EstimatorAction, ModelInputTensorsFormer, PathContextReader, ReaderInputTensors
-from .trainer import Trainer
+from .multi_rank import (CKPT_MAGIC, CKPT_SUFFIX, batch_split, check_checkpoint_dims, check_multi_rank_run,
+                         checkpoint_header, create_checkpoint_file, read_checkpoint_header, read_checkpoint_part, run_world,
+                         write_checkpoint, write_checkpoint_part)
+from .trainer import Trainer, make_fully_sharded_engine
 from .vocabularies import VocabType
+
+
+def _barrier():
+    import torch.distributed as dist
+    dist.barrier()
 
 def _prefetch(iterable, depth: int = 8):
     """Runs `iterable` (the reader) in a background thread, `depth` batches ahead: the native
@@ -107,8 +119,8 @@ def run_determinism(environ, now=time.time):
     return deterministic, seed
 
 
-_CKPT_MAGIC = b"C2VB200\0"
-_CKPT_SUFFIX = ".c2v_b200"
+_CKPT_MAGIC = CKPT_MAGIC
+_CKPT_SUFFIX = CKPT_SUFFIX
 
 
 class Code2VecModel(Code2VecModelBase):
@@ -123,7 +135,57 @@ class Code2VecModel(Code2VecModelBase):
         self.vocab_type_to_tf_variable_name_mapping: Dict[VocabType, str] = {
             VocabType.Token: "WORDS_VOCAB", VocabType.Target: "TARGET_WORDS_VOCAB", VocabType.Path: "PATHS_VOCAB"}
         self._param_of_vocab = {VocabType.Token: "tok", VocabType.Target: "tgt", VocabType.Path: "path"}
+        # WORLD_SIZE > 1 (torch.distributed.run): one rank per GPU on the fully sharded schedule (DESIGN.md §6c)
+        self.world, self.local_rank = run_world(os.environ)
+        self.rank = 0
+        self._own_group = False
+        check_multi_rank_run(config, self.world)
+        if self.world > 1:
+            self._join_group()
+            if self.rank != 0:
+                config.quiet()                       # rank 0 logs for every rank
         super().__init__(config)
+
+    def _join_group(self):
+        import torch
+        import torch.distributed as dist
+        if not dist.is_initialized():
+            torch.cuda.set_device(self.local_rank)
+            dist.init_process_group("nccl", device_id=torch.device("cuda", self.local_rank))
+            self._own_group = True
+        if dist.get_world_size() != self.world:
+            raise ValueError("WORLD_SIZE=%d but the process group has %d ranks" % (self.world, dist.get_world_size()))
+        self.rank = dist.get_rank()
+
+    def log(self, msg):
+        if self.rank == 0:
+            super().log(msg)
+
+    def _all_ok(self, work, ranks=None):
+        """work() on this rank if it is one of `ranks` (default: every rank), then every rank learns whether any rank
+        failed, so all of them raise together instead of waiting in the next collective for a rank that has gone."""
+        import torch.distributed as dist
+        err = None
+        if ranks is None or self.rank in ranks:
+            try:
+                work()
+            except Exception as exc:
+                err = exc
+        status = [None] * self.world
+        dist.all_gather_object(status, None if err is None else "%s: %s" % (type(err).__name__, err))
+        if err is not None:
+            raise err
+        failed = [(r, s) for r, s in enumerate(status) if s]
+        if failed:
+            raise RuntimeError("rank %d failed: %s" % failed[0])
+
+    def _init_num_of_examples(self):
+        if self.world == 1:
+            return super()._init_num_of_examples()
+        # rank 0 counts the examples and writes the `.num_examples` side-cars; the other ranks then read them
+        self._all_ok(super()._init_num_of_examples, ranks=(0,))
+        if self.rank != 0:
+            super()._init_num_of_examples()
 
     # ---- engine life cycle -------------------------------------------------------------------
     def _engine_dims(self) -> EngineDims:
@@ -138,15 +200,19 @@ class Code2VecModel(Code2VecModelBase):
                           max_batch=max(c.TRAIN_BATCH_SIZE, c.TEST_BATCH_SIZE, 1),
                           top_k=c.TOP_K_WORDS_CONSIDERED_DURING_PREDICTION)
 
-    def _make_engine(self):
+    def _make_engine(self, init: bool = False):
+        """The engine and, for training or any multi-GPU run, its Trainer.  init: draw the initial parameters (on several
+        GPUs before the Trainer moves the embedding tables into row shards)."""
         import torch
-        if int(os.environ.get("WORLD_SIZE", "1")) > 1:
-            # The multi-GPU schedules live in code2vec_b200.trainer (and bench.py drives them); wiring them into
-            # train() also needs per-rank data sharding and sharded checkpoints, which this backend does not do yet.
-            raise NotImplementedError("Code2VecModel.train()/evaluate() run one process on one GPU; "
-                                      "use code2vec_b200.trainer.Trainer for multi-GPU steps")
-        device = int(os.environ.get("LOCAL_RANK", "0")) if torch.cuda.device_count() > 1 else 0
-        self.engine = PathAttentionEngine(self._engine_dims(), device=device, training=self.config.is_training)
+        if self.world > 1:
+            # this rank's engine: a block of target rows, sized for the global batch (trainer.make_fully_sharded_engine)
+            self.engine = make_fully_sharded_engine(self._engine_dims(), self.config.TRAIN_BATCH_SIZE // self.world,
+                                                    self.local_rank, training=self.config.is_training)
+            if init:
+                self.engine.init_params(whole_target_table=True)
+        else:
+            device = int(os.environ.get("LOCAL_RANK", "0")) if torch.cuda.device_count() > 1 else 0
+            self.engine = PathAttentionEngine(self._engine_dims(), device=device, training=self.config.is_training)
         # arithmetic of the big matrix products: tensor cores (tf32 operands, fp32 accumulate) for training
         # steps, the reference's own fp32 FMA class for evaluate()/predict() so that top-k is decided on
         # fp32 logits.  C2V_MATH=fp32|tf32 forces one mode for both.
@@ -165,16 +231,26 @@ class Code2VecModel(Code2VecModelBase):
             self._deterministic, self._seed, self._deterministic, self._seed))
         # C2V_HINT_NEXT=1: pass each next batch to the engine (c2v_hint_next_batch); off by default
         self._hint_next = os.environ.get("C2V_HINT_NEXT", "0") == "1"
-        if self.config.is_training:
+        if self.world > 1:
+            # every multi-GPU run, evaluate-only ones too: the row shards and Trainer.predict live in the Trainer.
+            # C2V_DETERMINISTIC=1 sends the embedding gradients through the ordered exchange (DESIGN.md §5.1)
+            det = self._deterministic and self.config.is_training
+            self.trainer = Trainer(self.engine, keep_prob=self.config.DROPOUT_KEEP_RATE, seed=self._seed, adam=self._ADAM,
+                                   schedule="fully_sharded", deterministic=det, ordered_exchange=det)
+            self.log("b200 backend: %d ranks, fully sharded schedule, %d of each global batch of %d rows per rank" % (
+                self.world, self.engine.local_batch, self.config.TRAIN_BATCH_SIZE))
+        elif self.config.is_training:
             self.trainer = Trainer(self.engine, keep_prob=self.config.DROPOUT_KEEP_RATE, seed=self._seed, adam=self._ADAM,
                                    deterministic=self._deterministic)
+        if init and self.world == 1:
+            self.engine.init_params()
 
     def _create_inner_model(self):
-        self._make_engine()
-        self.engine.init_params()
-        n_params = sum(int(np.prod(s)) for s in self.engine.dims.shapes().values())
+        self._make_engine(init=True)
+        shapes = self._engine_dims().shapes()
+        n_params = sum(int(np.prod(s)) for s in shapes.values())
         self.log("Number of trainable params: {}".format(n_params))
-        for name, shape in self.engine.dims.shapes().items():
+        for name, shape in shapes.items():
             self.log("variable name: {} -- shape: {} -- #params: {}".format(name, shape, int(np.prod(shape))))
 
     def _load_inner_model(self):
@@ -186,40 +262,97 @@ class Code2VecModel(Code2VecModelBase):
 
     def close_session(self):
         if self.engine is not None:
+            if self.world > 1:
+                import torch
+                torch.cuda.synchronize(self.engine.dev)
+                _barrier()                               # no peer reads this rank's shards any more
             self.engine.close()
             self.engine = None
+        if self._own_group:
+            import torch.distributed as dist
+            dist.destroy_process_group()
+            self._own_group = False
+
+    def save(self, model_save_path=None):
+        if self.world == 1:
+            return super().save(model_save_path)
+        # rank 0 writes dictionaries.bin and makes the folder; every rank writes its rows of the checkpoint
+        target = model_save_path if model_save_path is not None else self.config.MODEL_SAVE_PATH
+        if self.rank == 0:
+            folder = target.rpartition("/")[0]
+            if folder:
+                os.makedirs(folder, exist_ok=True)
+            self.vocabs.save(self.config.get_vocabularies_path_from_model_path(target))
+        self._save_inner_model(target)
 
     # ---- checkpoint: header (json) + raw little-endian float32 tensors -------------------------
     def _save_inner_model(self, path: str, release: bool = False):
+        if self.world > 1:
+            return self._save_sharded(path)
         e = self.engine
         e.sync_tables()                                  # lazy Adam: replay deferred row updates before reading the tensors
-        tensors = [("theta/" + k, e.params[k]) for k in PARAM_NAMES]
+        tensors = [e.params[k] for k in PARAM_NAMES]
         with_optimizer = (not release) and e.adam_m is not None
         if with_optimizer:
-            tensors += [("adam_m/" + k, e.adam_m[k]) for k in PARAM_NAMES]
-            tensors += [("adam_v/" + k, e.adam_v[k]) for k in PARAM_NAMES]
-        meta = {"format": 1, "dims": vars(e.dims), "adam_t": int(e.adam_t) if with_optimizer else 0,
-                "epochs_trained": int(getattr(self, "nr_epochs_trained", 0)),
-                "tf_names": {"tok": "model/WORDS_VOCAB", "path": "model/PATHS_VOCAB", "tgt": "model/TARGET_WORDS_VOCAB",
-                             "W": "model/TRANSFORM", "a": "model/ATTENTION"},
-                "tensors": []}
-        offset = 0
-        for name, t in tensors:
-            n = int(t.numel()) * 4
-            meta["tensors"].append({"name": name, "shape": list(t.shape), "offset": offset, "nbytes": n})
-            offset += n
-        header = json.dumps(meta).encode()
+            tensors += [e.adam_m[k] for k in PARAM_NAMES] + [e.adam_v[k] for k in PARAM_NAMES]
+        prefix, _, _ = checkpoint_header(vars(e.dims), e.adam_t, getattr(self, "nr_epochs_trained", 0), with_optimizer)
         tmp = path + _CKPT_SUFFIX + ".tmp"
-        with open(tmp, "wb") as f:
-            f.write(_CKPT_MAGIC)
-            f.write(struct.pack("<Q", len(header)))
-            f.write(header)
-            for _, t in tensors:
-                f.write(t.detach().cpu().numpy().astype("<f4", copy=False).tobytes())
+        write_checkpoint(tmp, prefix, [t.detach().cpu().numpy() for t in tensors])
         os.replace(tmp, path + _CKPT_SUFFIX)
+
+    def _sharded_tensors(self, with_optimizer: bool) -> dict:
+        """{checkpoint tensor name: this rank's device tensor} (multi_rank's layout).  The replicated tok / path tensors
+        are stale once the Trainer has moved them into row shards; only the shards are used."""
+        e = self.engine
+        out = {"theta/tok": e.shard_params["tok"], "theta/path": e.shard_params["path"]}
+        out.update({"theta/" + k: e.params[k] for k in ("tgt", "W", "a")})
+        if with_optimizer:
+            for g, shard, rest in (("adam_m", e.shard_m, e.adam_m), ("adam_v", e.shard_v, e.adam_v)):
+                out.update({g + "/tok": shard["tok"], g + "/path": shard["path"]})
+                out.update({g + "/" + k: rest[k] for k in ("tgt", "W", "a")})
+        return out
+
+    def _save_sharded(self, path: str):
+        """All ranks write one file: rank 0 writes the header and sizes the file, every rank writes its own rows
+        (embedding-shard rows, its target block; W and a from rank 0), rank 0 renames the file once all are done."""
+        e = self.engine
+        with_optimizer = e.adam_m is not None
+        prefix, entries, total = checkpoint_header(vars(self._engine_dims()), e.adam_t,
+                                                   getattr(self, "nr_epochs_trained", 0), with_optimizer)
+        tmp = path + _CKPT_SUFFIX + ".tmp"
+        rows = (e.target_row0, e.target_row0 + e.dims.target_vocab)
+
+        def write_rows():
+            local = {name: t.detach().cpu().numpy() for name, t in self._sharded_tensors(with_optimizer).items()
+                     if self.rank == 0 or name.split("/")[1] not in ("W", "a")}
+            write_checkpoint_part(tmp, len(prefix), entries, self.rank, self.world, rows, local)
+        # each step ends in a collective that also reports a failure on any rank, so no rank waits for one that has gone
+        self._all_ok(lambda: create_checkpoint_file(tmp, prefix, total), ranks=(0,))
+        self._all_ok(write_rows)
+        self._all_ok(lambda: os.replace(tmp, path + _CKPT_SUFFIX), ranks=(0,))     # the file exists on return, on any rank
+
+    def _read_sharded(self, file_path: str):
+        """This rank's rows of a checkpoint saved on any number of GPUs, into the shards, the target block and W / a
+        (with the Adam slots when training, so a resumed run continues exactly).  Runs after the Trainer is built:
+        enable_table_sharding would overwrite the shards and zero their Adam slots."""
+        import torch
+        e = self.engine
+
+        def read_rows():
+            out = self._sharded_tensors(with_optimizer=e.training)
+            check_checkpoint_dims(read_checkpoint_header(file_path)[0], vars(self._engine_dims()))
+            meta = read_checkpoint_part(file_path, self.rank, self.world,
+                                        (e.target_row0, e.target_row0 + e.dims.target_vocab), out)
+            e.adam_t = int(meta.get("adam_t", 0))
+            if e.training:
+                e.set_option("adam_step_count", e.adam_t)
+            torch.cuda.synchronize(e.dev)
+        self._all_ok(read_rows)                          # every shard is loaded before any peer reads it
 
     def _read_checkpoint(self, file_path: str):
         import torch
+        if self.world > 1:
+            return self._read_sharded(file_path)
         if not os.path.isfile(file_path):
             raise ValueError("There is no model at path `{}`.".format(file_path))
         e = self.engine
@@ -265,8 +398,11 @@ class Code2VecModel(Code2VecModelBase):
         # page-locked slot, its upload overlaps the previous step, and the loop never waits for the GPU except to read
         # the losses at each progress line.  C2V_BATCH_RING=0 (or a reader without the native tensoriser) keeps the
         # synchronous c2v_train_batch_host path.
+        # several GPUs: every rank reads the same global batches (same file, same shuffle seed) and steps on its slice
+        multi = self.world > 1
+        dropped_rows = 0
         ring = None
-        if os.environ.get("C2V_BATCH_RING", "1") != "0" and not self._hint_next and train_reader._native_ready():
+        if not multi and os.environ.get("C2V_BATCH_RING", "1") != "0" and not self._hint_next and train_reader._native_ready():
             import torch
             from .batch_ring import PinnedBatchRing
             ring = PinnedBatchRing(torch, self.engine.dev, cfg.TRAIN_BATCH_SIZE, cfg.MAX_CONTEXTS)
@@ -276,8 +412,14 @@ class Code2VecModel(Code2VecModelBase):
         self.h2d_bytes = 0
         for batch, following in _with_next(_prefetch(train_reader.get_dataset(), depth=4 if ring else 8)):
             t = former.from_model_input_form(batch)
+            if multi:
+                # a short last batch runs as a step of world * floor(rows / world) rows (the loss is their mean)
+                lo, hi, dropped = batch_split(int(t.target_index.shape[0]), self.world, self.rank)
+                dropped_rows += dropped
+                if hi == lo:                       # fewer rows than ranks: the batch is skipped
+                    continue
             nxt = None
-            if self._hint_next and following is not None:
+            if self._hint_next and not multi and following is not None:
                 n = former.from_model_input_form(following)
                 nxt = (n.path_source_token_indices, n.path_indices, n.path_target_token_indices)
             batch_num += 1
@@ -294,6 +436,10 @@ class Code2VecModel(Code2VecModelBase):
                     torch.cuda.current_stream(self.engine.dev).synchronize()
                     batch_loss = float(loss_hist[:n_hist].sum())
                     n_hist = 0
+            elif multi:                            # the fully sharded loss is already the mean over the global batch
+                batch_loss = self.trainer.step_host(*(a[lo:hi] for a in (
+                    t.path_source_token_indices, t.path_indices, t.path_target_token_indices, t.context_valid_mask,
+                    t.target_index)))
             else:
                 batch_loss = self.trainer.step_host(t.path_source_token_indices, t.path_indices, t.path_target_token_indices,
                                                     t.context_valid_mask, t.target_index, next_batch=nxt)
@@ -319,6 +465,9 @@ class Code2VecModel(Code2VecModelBase):
                 sum_loss += float(loss_hist[:n_hist].sum())
             ring.close()
             train_reader.batch_ring = None
+        if multi:
+            self.log("%d training rows left out: a short batch trains on a multiple of the %d ranks" % (
+                dropped_rows, self.world))
         self.log("Done training")
         if cfg.MODEL_SAVE_PATH:
             self.save(cfg.MODEL_SAVE_PATH)
@@ -344,15 +493,22 @@ class Code2VecModel(Code2VecModelBase):
         topk_metric = TopKAccuracyEvaluationMetric(cfg.TOP_K_WORDS_CONSIDERED_DURING_PREDICTION,
                                                    partial(common.get_first_match_word_from_top_predictions, special))
         total_predictions, total_batches = 0, 0
-        code_vectors_file = open(cfg.TEST_DATA_PATH + ".vectors", "w") if cfg.EXPORT_CODE_VECTORS else None
-        with open("log.txt", "w") as log_output_file:
+        # several GPUs: every rank predicts its slice of each batch, rank 0 gathers the rows and writes every file
+        writer = self.rank == 0
+        code_vectors_file = open(cfg.TEST_DATA_PATH + ".vectors", "w") if cfg.EXPORT_CODE_VECTORS and writer else None
+        with (open("log.txt", "w") if writer else contextlib.nullcontext()) as log_output_file:
             start_time = time.time()
             self.log("Starting evaluation")
             for batch in _prefetch(self.eval_reader.get_dataset()):
                 t = _EvaluateInputFormer().from_model_input_form(batch)
-                idx, _vals, code_vectors, _attn = self.engine.predict_batch_host(
-                    t.path_source_token_indices, t.path_indices, t.path_target_token_indices, t.context_valid_mask,
-                    normalize=False, want_code=cfg.EXPORT_CODE_VECTORS, want_attention=False)
+                if self.world > 1:
+                    idx, code_vectors = self._predict_sharded(t, cfg.EXPORT_CODE_VECTORS)
+                    if not writer:
+                        continue
+                else:
+                    idx, _vals, code_vectors, _attn = self.engine.predict_batch_host(
+                        t.path_source_token_indices, t.path_indices, t.path_target_token_indices, t.context_valid_mask,
+                        normalize=False, want_code=cfg.EXPORT_CODE_VECTORS, want_attention=False)
                 top_words = self.vocabs.target_vocab.lookup_word(idx)          # (batch, top_k) strings   (:302)
                 original_names = list(t.target_string)
                 self._log_predictions_during_evaluation(zip(original_names, top_words), log_output_file)
@@ -365,14 +521,49 @@ class Code2VecModel(Code2VecModelBase):
                 if total_batches % cfg.NUM_BATCHES_TO_LOG_PROGRESS == 0:
                     self._trace_evaluation(total_predictions, time.time() - start_time)
             self.log("Done evaluating, epoch reached")
-            log_output_file.write(str(topk_metric.topk_correct_predictions) + "\n")
+            if writer:
+                log_output_file.write(str(topk_metric.topk_correct_predictions) + "\n")
         if code_vectors_file is not None:
             code_vectors_file.close()
         elapsed = int(time.time() - eval_start_time)
         self.log("Evaluation time: %sH:%sM:%sS" % ((elapsed // 60 // 60), (elapsed // 60) % 60, elapsed % 60))
-        return ModelEvaluationResults(topk_acc=topk_metric.topk_correct_predictions,
-                                      subtoken_precision=subtokens_metric.precision,
-                                      subtoken_recall=subtokens_metric.recall, subtoken_f1=subtokens_metric.f1)
+        results = None
+        if writer:
+            results = ModelEvaluationResults(topk_acc=topk_metric.topk_correct_predictions,
+                                             subtoken_precision=subtokens_metric.precision,
+                                             subtoken_recall=subtokens_metric.recall, subtoken_f1=subtokens_metric.f1)
+        if self.world > 1:                         # every rank returns rank 0's results
+            import torch.distributed as dist
+            gathered = [None] * self.world
+            dist.all_gather_object(gathered, results)
+            results = gathered[0]
+        return results
+
+    def _predict_sharded(self, t: ReaderInputTensors, want_code: bool):
+        """(top-k ids [n, k], code vectors [n, D] or None) of the n rows of one reader batch, on rank 0; the other ranks
+        get the same arrays.  The rows go in global batches of at most world * local_batch rows: each rank takes an
+        equal slice (the last global batch padded with copies of its last row), Trainer.predict ranks it against the
+        whole target table, and the slices are all-gathered back in file order without the padding."""
+        import torch
+        import torch.distributed as dist
+        e, W, r = self.engine, self.world, self.rank
+        arrays = ((t.path_source_token_indices, torch.int32), (t.path_indices, torch.int32),
+                  (t.path_target_token_indices, torch.int32), (t.context_valid_mask, torch.float32))
+        n_all = int(t.path_source_token_indices.shape[0])
+        idx_parts, code_parts = [], []
+        for s in range(0, n_all, W * e.local_batch):
+            n = min(W * e.local_batch, n_all - s)
+            b = -(-n // W)
+            rows = np.minimum(np.arange(s + r * b, s + (r + 1) * b), s + n - 1)
+            idx, _val, code = self.trainer.predict(*(e.to_device(a[rows], dt) for a, dt in arrays), normalize=0)
+            idx_all = torch.empty((W * b, idx.shape[1]), dtype=idx.dtype, device=e.dev)
+            dist.all_gather_into_tensor(idx_all, idx)
+            idx_parts.append(idx_all[:n].cpu().numpy())
+            if want_code:
+                code_all = torch.empty((W * b, code.shape[1]), dtype=code.dtype, device=e.dev)
+                dist.all_gather_into_tensor(code_all, code)
+                code_parts.append(code_all[:n].cpu().numpy())
+        return np.concatenate(idx_parts), (np.concatenate(code_parts) if want_code else None)
 
     # ---- predict (tensorflow_model.py:311-368) ----------------------------------------------------------
     def predict(self, predict_data_lines: Iterable[str]) -> List[ModelPredictionResults]:
@@ -398,8 +589,35 @@ class Code2VecModel(Code2VecModelBase):
 
     def _get_vocab_embedding_as_np_array(self, vocab_type: VocabType) -> np.ndarray:
         assert vocab_type in VocabType
+        if self.world > 1:
+            return self._gather_table(self._param_of_vocab[vocab_type])
         self.engine.sync_tables()
         return self.engine.params[self._param_of_vocab[vocab_type]].detach().cpu().numpy()
+
+    def _gather_table(self, name: str) -> np.ndarray:
+        """The whole table `name` on every rank (a collective): the embedding shards all-gathered and interleaved back
+        (global row = local row * world + rank), or the target blocks all-gathered and concatenated."""
+        import torch
+        import torch.distributed as dist
+        e, W = self.engine, self.world
+        if name in ("tok", "path"):
+            shard = e.shard_params[name]
+            whole = torch.empty((W,) + tuple(shard.shape), dtype=shard.dtype, device=e.dev)
+            dist.all_gather_into_tensor(whole, shard)
+            n_rows = self._engine_dims().shapes()[name][0]
+            return whole.transpose(0, 1).reshape(-1, shard.shape[1])[:n_rows].cpu().numpy()
+        Y, per = e.global_target_vocab, -(-e.global_target_vocab // W)     # blocks of `per` rows, the last one shorter
+        block = torch.zeros((per, e.dims.code_dim), dtype=torch.float32, device=e.dev)
+        block[:e.dims.target_vocab].copy_(e.params["tgt"])
+        whole = torch.empty((W * per, e.dims.code_dim), dtype=torch.float32, device=e.dev)
+        dist.all_gather_into_tensor(whole, block)
+        return whole[:Y].cpu().numpy()
+
+    def save_word2vec_format(self, dest_save_path: str, vocab_type: VocabType):
+        if self.world > 1 and self.rank != 0:
+            self._get_vocab_embedding_as_np_array(vocab_type)        # the gather is a collective; rank 0 writes the file
+            return
+        super().save_word2vec_format(dest_save_path, vocab_type)
 
     # ---- logging helpers (tensorflow_model.py:411-437) ------------------------------------------------------
     def _log_predictions_during_evaluation(self, results, output_file):

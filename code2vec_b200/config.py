@@ -118,6 +118,7 @@ class Config:
         self.NUM_TRAIN_EXAMPLES = 0
         self.NUM_TEST_EXAMPLES = 0
         self.__logger: Optional[logging.Logger] = None
+        self.__quiet = False
         if set_defaults:
             self.set_defaults()
         if load_from_args:
@@ -226,4 +227,9 @@ class Config:
         return self.__logger
 
     def log(self, msg):
-        self.get_logger().info(msg)
+        if not self.__quiet:
+            self.get_logger().info(msg)
+
+    def quiet(self):
+        """Drop every later log() line: the ranks other than 0 of a multi-GPU run, where rank 0 logs for all."""
+        self.__quiet = True

@@ -357,16 +357,20 @@ class PathAttentionEngine:
         return out
 
     # ---- parameters -----------------------------------------------------------------------
-    def init_params(self, seed: int = 4321, scheme: str = "tensorflow"):
+    def init_params(self, seed: int = 4321, scheme: str = "tensorflow", whole_target_table: bool = False):
         """The reference's initialisers.  scheme "tensorflow" (tensorflow_model.py:205-220,249-250): tables
         U(+-sqrt(3/cols)) (variance_scaling fan_out uniform), TRANSFORM / ATTENTION glorot-uniform.
         scheme "keras" (keras_model.py:46-70, keras_attention_layer.py:29-34): embeddings and the attention
         vector U(+-0.05), both Dense kernels glorot-uniform (the output kernel is [D, |Y|] there).
-        Drawn on the device with torch's generator (initialisation is not the hot path)."""
+        Drawn on the device with torch's generator (initialisation is not the hot path).
+        whole_target_table: an engine of make_fully_sharded_engine draws the whole target table of global_target_vocab
+        rows and keeps its own block, so every rank holds the values a one-GPU engine with the same seed starts from."""
         torch = self.torch
         g = torch.Generator(device=self.dev)
         g.manual_seed(seed)
         d, D, Y = self.dims.embed_dim, self.dims.code_dim, self.dims.target_vocab
+        if whole_target_table:
+            Y = self.global_target_vocab
         if scheme == "tensorflow":
             lim = {"tok": (3.0 / d) ** 0.5, "path": (3.0 / d) ** 0.5, "tgt": (3.0 / D) ** 0.5,
                    "W": (6.0 / (3 * d + D)) ** 0.5, "a": (6.0 / (D + 1)) ** 0.5}
@@ -375,6 +379,10 @@ class PathAttentionEngine:
         else:
             raise ValueError("unknown initialisation scheme: %r" % (scheme,))
         for k in PARAM_NAMES:
+            if k == "tgt" and whole_target_table:
+                whole = torch.empty((Y, D), dtype=torch.float32, device=self.dev).uniform_(-lim[k], lim[k], generator=g)
+                self.params[k].copy_(whole[self.target_row0:self.target_row0 + self.dims.target_vocab])
+                continue
             self.params[k].uniform_(-lim[k], lim[k], generator=g)
 
     def load_params(self, arrays: Dict[str, np.ndarray]):

@@ -314,9 +314,9 @@ class Trainer:
             code, _ = e.forward(src, path, tgt, mask, want_attention=False)
             idx, val = e.topk(code, normalize)
             return idx, val, code
-        dist, fs, pr = _dist(), self._fs, self._pred
-        if int(src.shape[0]) != e.local_batch:
-            raise ValueError("fully_sharded needs the same local batch (%d) on every rank" % e.local_batch)
+        dist = _dist()
+        Bl = int(src.shape[0])
+        fs, pr = self._fs_views(Bl), self._pred_views(Bl)
         full = normalize == 2
         e.forward(src, path, tgt, mask, want_attention=False, code_out=fs["v_local"])
         dist.all_gather_into_tensor(fs["v_all"], fs["v_local"], group=self.group)
@@ -328,17 +328,47 @@ class Trainer:
         if full:
             dist.all_gather_into_tensor(fs["maxes"].view(-1), fs["rmax"], group=self.group)
             dist.all_gather_into_tensor(fs["sums"].view(-1), fs["rsum"], group=self.group)
-        Bl = e.local_batch
         e.topk_merge(pr["idx_all"], pr["val_all"], fs["maxes"] if full else None, fs["sums"] if full else None,
                      self.rank * Bl, Bl, normalize, pr["idx_out"], pr["val_out"])
         return pr["idx_out"], pr["val_out"], fs["v_local"]
 
+    def _local_batch(self, B: int):
+        if not 0 < B <= self.e.local_batch:
+            raise ValueError("fully_sharded takes 1 to %d rows per rank (the engine's local batch), the same number on "
+                             "every rank; got %d" % (self.e.local_batch, B))
+
+    def _fs_views(self, B: int):
+        """The step's buffers for a local batch of B <= local_batch rows (the same B on every rank): the [Bl] / [Bt]
+        buffers as leading views, the [W, Bt] ones as contiguous [W, B * W] views of their first elements."""
+        self._local_batch(B)
+        fs = self._fs
+        if B == self.e.local_batch:
+            return fs
+        W, Bt = self.world, B * self.world
+        v = dict(fs)
+        for name in ("v_local", "dv_local"):
+            v[name] = fs[name][:B]
+        for name in ("v_all", "tgt_all", "rmax", "rsum", "tlogit", "lse", "dv_part"):
+            v[name] = fs[name][:Bt]
+        for name in ("maxes", "sums"):
+            v[name] = fs[name].view(-1)[:W * Bt].view(W, Bt)
+        return v
+
+    def _pred_views(self, B: int):
+        """predict()'s buffers for a local batch of B rows, as _fs_views."""
+        pr = self._pred
+        if B == self.e.local_batch:
+            return pr
+        W, Bt, k = self.world, B * self.world, pr["idx"].shape[1]
+        v = dict(idx=pr["idx"][:Bt], val=pr["val"][:Bt], idx_out=pr["idx_out"][:B], val_out=pr["val_out"][:B])
+        for name in ("idx_all", "val_all"):
+            v[name] = pr[name].view(-1)[:W * Bt * k].view(W, Bt, k)
+        return v
+
     def _fully_sharded_step(self, src, path, tgt, mask, target):
-        e, dist, fs = self.e, _dist(), self._fs
+        e, dist = self.e, _dist()
         t = e.adam_t + 1
-        B, W = int(src.shape[0]), self.world
-        if B != e.local_batch:
-            raise ValueError("fully_sharded needs the same local batch (%d) on every rank" % e.local_batch)
+        fs = self._fs_views(int(src.shape[0]))
         seed = self.seed + self.rank
         e.context_forward(src, path, tgt, mask, fs["v_local"], keep=self.keep, seed=seed, step=t)
         dist.all_gather_into_tensor(fs["v_all"], fs["v_local"], group=self.group)
