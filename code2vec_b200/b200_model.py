@@ -32,6 +32,7 @@ from .path_context_reader import EstimatorAction, ModelInputTensorsFormer, PathC
 from .multi_rank import (CKPT_MAGIC, CKPT_SUFFIX, batch_split, check_checkpoint_dims, check_multi_rank_run,
                          checkpoint_header, create_checkpoint_file, read_checkpoint_header, read_checkpoint_part, run_world,
                          write_checkpoint, write_checkpoint_part)
+from .device_reader import device_reader_flag
 from .trainer import Trainer, make_fully_sharded_engine
 from .vocabularies import VocabType
 
@@ -140,6 +141,11 @@ class Code2VecModel(Code2VecModelBase):
         self.rank = 0
         self._own_group = False
         check_multi_rank_run(config, self.world)
+        # C2V_DEVICE_READER=1: train() reads its batches on the GPU (device_reader.py, DESIGN.md §6d)
+        self._device_reader = device_reader_flag(os.environ)
+        if self._device_reader and config.DL_FRAMEWORK == "b200-keras":
+            raise ValueError("C2V_DEVICE_READER=1 is not available with --framework b200-keras: its training loop reads "
+                             "batches on the host; unset C2V_DEVICE_READER or train with --framework b200")
         if self.world > 1:
             self._join_group()
             if self.rank != 0:
@@ -231,6 +237,8 @@ class Code2VecModel(Code2VecModelBase):
             self._deterministic, self._seed, self._deterministic, self._seed))
         # C2V_HINT_NEXT=1: pass each next batch to the engine (c2v_hint_next_batch); off by default
         self._hint_next = os.environ.get("C2V_HINT_NEXT", "0") == "1"
+        self.log("b200 backend training reader: %s (C2V_DEVICE_READER=%d)" % (
+            "on the GPU" if self._device_reader else "on the host", self._device_reader))
         if self.world > 1:
             # every multi-GPU run, evaluate-only ones too: the row shards and Trainer.predict live in the Trainer.
             # C2V_DETERMINISTIC=1 sends the embedding gradients through the ordered exchange (DESIGN.md §5.1)
@@ -401,48 +409,88 @@ class Code2VecModel(Code2VecModelBase):
         # several GPUs: every rank reads the same global batches (same file, same shuffle seed) and steps on its slice
         multi = self.world > 1
         dropped_rows = 0
-        ring = None
-        if not multi and os.environ.get("C2V_BATCH_RING", "1") != "0" and not self._hint_next and train_reader._native_ready():
+        ring = dev_reader = None
+        if self._device_reader:
+            # C2V_DEVICE_READER=1: batches are parsed and drawn on the GPU into device slots (device_reader.py); the steps
+            # read them there (step_device) and the losses collect in the pinned history, as on the ring path
+            from .device_reader import DeviceBatchReader
+            dev_reader = DeviceBatchReader(train_reader, self.engine.dev, world=self.world, rank=self.rank)
+        elif not multi and os.environ.get("C2V_BATCH_RING", "1") != "0" and not self._hint_next and train_reader._native_ready():
             import torch
             from .batch_ring import PinnedBatchRing
             ring = PinnedBatchRing(torch, self.engine.dev, cfg.TRAIN_BATCH_SIZE, cfg.MAX_CONTEXTS)
             train_reader.batch_ring = ring
+        if ring is not None or dev_reader is not None:
+            import torch
             loss_hist = torch.zeros(max(int(cfg.NUM_BATCHES_TO_LOG_PROGRESS), 1), dtype=torch.float32).pin_memory()
             n_hist = 0
+        # the losses of a device-reader run are summed as the host path it replaces sums them: the ring path adds a float32
+        # sum of the history, the synchronous path (C2V_HINT_NEXT=1, several GPUs) adds each step's loss in turn
+        ring_sum = dev_reader is not None and not multi and not self._hint_next
         self.h2d_bytes = 0
-        for batch, following in _with_next(_prefetch(train_reader.get_dataset(), depth=4 if ring else 8)):
-            t = former.from_model_input_form(batch)
-            if multi:
-                # a short last batch runs as a step of world * floor(rows / world) rows (the loss is their mean)
-                lo, hi, dropped = batch_split(int(t.target_index.shape[0]), self.world, self.rank)
-                dropped_rows += dropped
-                if hi == lo:                       # fewer rows than ranks: the batch is skipped
-                    continue
-            nxt = None
-            if self._hint_next and not multi and following is not None:
-                n = former.from_model_input_form(following)
-                nxt = (n.path_source_token_indices, n.path_indices, n.path_target_token_indices)
-            batch_num += 1
-            self.engine.set_option("math_mode", self._math_train)
-            if ring is not None:
-                rows = int(t.target_index.shape[0])
-                self.trainer.step_ring(ring, rows, loss_hist[n_hist:n_hist + 1])      # upload + step queued; nothing waited for
+        batches = dev_reader if dev_reader is not None else _prefetch(train_reader.get_dataset(), depth=4 if ring else 8)
+        for batch, following in _with_next(batches):
+            if dev_reader is not None:
+                batch.wait()                       # the current stream waits for the draw into this slot
+                if multi:
+                    dropped_rows += batch.dropped
+                    if batch.hi == batch.lo:       # fewer rows than ranks: the batch is skipped
+                        batch.release()
+                        continue
+                nxt = None
+                if self._hint_next and not multi and following is not None:
+                    following.wait()
+                    nxt = following.tensors[:3]
+                batch_num += 1
+                self.engine.set_option("math_mode", self._math_train)
+                loss = self.trainer.step_device(*batch.tensors, next_batch=nxt)
+                batch.release()                    # the slot is reused once this step has run
+                loss_hist[n_hist:n_hist + 1].copy_(loss, non_blocking=True)
                 n_hist += 1
-                self.h2d_bytes += rows * (4 * cfg.MAX_CONTEXTS + 1) * 4
                 flush = (batch_num % cfg.NUM_BATCHES_TO_LOG_PROGRESS == 0) or (batch_num % num_batches_to_save_and_eval == 0) \
                     or n_hist == loss_hist.numel()
                 batch_loss = 0.0
-                if flush:                          # the losses of the steps since the last progress line reach the host here
+                if flush:
                     torch.cuda.current_stream(self.engine.dev).synchronize()
-                    batch_loss = float(loss_hist[:n_hist].sum())
+                    if ring_sum:
+                        batch_loss = float(loss_hist[:n_hist].sum())
+                    else:
+                        for v in loss_hist[:n_hist].tolist():
+                            sum_loss += v
                     n_hist = 0
-            elif multi:                            # the fully sharded loss is already the mean over the global batch
-                batch_loss = self.trainer.step_host(*(a[lo:hi] for a in (
-                    t.path_source_token_indices, t.path_indices, t.path_target_token_indices, t.context_valid_mask,
-                    t.target_index)))
             else:
-                batch_loss = self.trainer.step_host(t.path_source_token_indices, t.path_indices, t.path_target_token_indices,
-                                                    t.context_valid_mask, t.target_index, next_batch=nxt)
+                t = former.from_model_input_form(batch)
+                if multi:
+                    # a short last batch runs as a step of world * floor(rows / world) rows (the loss is their mean)
+                    lo, hi, dropped = batch_split(int(t.target_index.shape[0]), self.world, self.rank)
+                    dropped_rows += dropped
+                    if hi == lo:                       # fewer rows than ranks: the batch is skipped
+                        continue
+                nxt = None
+                if self._hint_next and not multi and following is not None:
+                    n = former.from_model_input_form(following)
+                    nxt = (n.path_source_token_indices, n.path_indices, n.path_target_token_indices)
+                batch_num += 1
+                self.engine.set_option("math_mode", self._math_train)
+                if ring is not None:
+                    rows = int(t.target_index.shape[0])
+                    self.trainer.step_ring(ring, rows, loss_hist[n_hist:n_hist + 1])      # upload + step queued; nothing waited for
+                    n_hist += 1
+                    self.h2d_bytes += rows * (4 * cfg.MAX_CONTEXTS + 1) * 4
+                    flush = (batch_num % cfg.NUM_BATCHES_TO_LOG_PROGRESS == 0) or (batch_num % num_batches_to_save_and_eval == 0) \
+                        or n_hist == loss_hist.numel()
+                    batch_loss = 0.0
+                    if flush:                          # the losses of the steps since the last progress line reach the host here
+                        torch.cuda.current_stream(self.engine.dev).synchronize()
+                        batch_loss = float(loss_hist[:n_hist].sum())
+                        n_hist = 0
+                elif multi:                            # the fully sharded loss is already the mean over the global batch
+                    batch_loss = self.trainer.step_host(*(a[lo:hi] for a in (
+                        t.path_source_token_indices, t.path_indices, t.path_target_token_indices, t.context_valid_mask,
+                        t.target_index)))
+                else:
+                    batch_loss = self.trainer.step_host(t.path_source_token_indices, t.path_indices, t.path_target_token_indices,
+                                                        t.context_valid_mask, t.target_index, next_batch=nxt)
             sum_loss += batch_loss
             if batch_num % cfg.NUM_BATCHES_TO_LOG_PROGRESS == 0:
                 self._trace_training(sum_loss, batch_num, multi_batch_start_time)
@@ -465,6 +513,17 @@ class Code2VecModel(Code2VecModelBase):
                 sum_loss += float(loss_hist[:n_hist].sum())
             ring.close()
             train_reader.batch_ring = None
+        if dev_reader is not None:
+            torch.cuda.current_stream(self.engine.dev).synchronize()
+            if ring_sum:
+                sum_loss += float(loss_hist[:n_hist].sum()) if n_hist else 0.0
+            else:
+                for v in loss_hist[:n_hist].tolist():
+                    sum_loss += v
+            self.h2d_bytes = dev_reader.h2d_bytes
+            self.log("Device reader: %.1f MB of text and draw indices uploaded, %.1f MB of device memory held" % (
+                dev_reader.h2d_bytes / 1e6, dev_reader.device_bytes() / 1e6))
+            dev_reader.close()
         if multi:
             self.log("%d training rows left out: a short batch trains on a multiple of the %d ranks" % (
                 dropped_rows, self.world))

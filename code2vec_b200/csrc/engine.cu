@@ -1533,6 +1533,11 @@ int adam_impl(c2v_engine* e, cudaStream_t st, float lr, float b1, float b2, floa
 
 }  // namespace
 
+// failures of calls without an engine handle in other translation units (reader.cu): c2v_last_error(NULL) returns them
+namespace c2v {
+void set_global_error(const std::string& msg) { g_create_error = msg; }
+}
+
 // ================================== C ABI =======================================================
 extern "C" {
 

@@ -1,0 +1,625 @@
+// Device reader of `.c2v` training text (include/c2v_b200.h "Device reader", DESIGN.md §6d): a chunk of complete lines
+// already in device memory -> rows of the training shuffle pool, and draws from that pool into device batch buffers.
+// It computes what the host tensoriser computes (native/batcher.cpp parse_line, c2v_pool_take) and what the host
+// reader's shuffle pool does with it (path_context_reader._RowPool.commit / take), so its batches are the host reader's
+// batches, bit for bit:
+//   line index : per-tile counts of record starts and newlines, one-block scans, then each record's byte offset and the
+//                number of its line (blank lines are skipped but keep their line numbers, as the host's errors count them)
+//   parse      : one warp per record; fields are split on ' ' and parts on ',' with ballots, each part is hashed
+//                (FNV-1a 64) by one lane and probed in the host's own open-addressing tables, bytes compared
+//   commit     : rows land behind the pool's live end; dropped rows below the kept count are filled by the kept rows
+//                beyond it, j-th hole from j-th mover (not a stable compaction: the host pool's order)
+//   draw       : the picked rows (the host's random draw) are gathered into a batch buffer, then the holes they leave
+//                below the new end are filled with the surviving tail rows, both in ascending order
+#include <cuda_runtime.h>
+#include <stdint.h>
+#include <string.h>
+
+#include <cub/block/block_reduce.cuh>
+#include <cub/block/block_scan.cuh>
+#include <string>
+
+#include "../../include/c2v_b200.h"
+
+namespace c2v {
+void set_global_error(const std::string& msg);     // engine.cu: the message c2v_last_error(NULL) returns
+}
+
+namespace {
+
+struct DevSlot {                  // native/batcher.cpp Vocab::Slot, byte for byte
+  unsigned long long h;           // FNV-1a 64 of the word (0: empty slot)
+  long long off;                  // offset of the word's bytes
+  int32_t len, idx;
+};
+static_assert(sizeof(DevSlot) == 24, "slot layout of batcher.cpp");
+
+struct DevVocab {
+  const DevSlot* slots;
+  const unsigned char* bytes;
+  unsigned long long mask;
+  int32_t oov, pad;
+};
+
+constexpr int kTile = 4096;                        // bytes per block of the line index
+constexpr int kTileThreads = 256;
+constexpr int kPerThread = kTile / kTileThreads;
+constexpr int kRowTile = 1024;                     // rows per block of the commit scan
+constexpr int kParseWarps = 4;
+constexpr unsigned kFull = 0xffffffffu;
+
+__device__ __forceinline__ unsigned long long fnv1a(const unsigned char* p, long long n) {
+  unsigned long long h = 1469598103934665603ull;
+  for (long long i = 0; i < n; ++i) { h ^= p[i]; h *= 1099511628211ull; }
+  return h ? h : 1;
+}
+
+// batcher.cpp Vocab::lookup: linear probing from h & mask, the first slot with the same hash, length and bytes wins
+__device__ int32_t lookup(const DevVocab& v, const unsigned char* p, long long n) {
+  const unsigned long long h = fnv1a(p, n);
+  for (unsigned long long i = h & v.mask;; i = (i + 1) & v.mask) {
+    const DevSlot* s = v.slots + i;
+    const unsigned long long sh = s->h;
+    if (sh == 0) return v.oov;
+    if (sh == h && (long long)s->len == n) {
+      const unsigned char* w = v.bytes + s->off;
+      long long k = 0;
+      while (k < n && w[k] == p[k]) ++k;
+      if (k == n) return s->idx;
+    }
+  }
+}
+
+// ---- line index ----------------------------------------------------------------------------------------------------
+// a record starts at byte p when p == 0 or text[p-1] == '\n', unless text[p] is '\n' itself (a blank line)
+__device__ __forceinline__ void count_bytes(const unsigned char* text, long long n, long long lo, int& recs, int& nls) {
+  recs = nls = 0;
+  for (int k = 0; k < kPerThread; ++k) {
+    const long long p = lo + k;
+    if (p >= n) break;
+    const unsigned char c = text[p];
+    recs += (p == 0 || text[p - 1] == '\n') && c != '\n';
+    nls += c == '\n';
+  }
+}
+
+__global__ void __launch_bounds__(kTileThreads)
+line_count_kernel(const unsigned char* __restrict__ text, long long n, int* __restrict__ rec_cnt, int* __restrict__ nl_cnt) {
+  using Reduce = cub::BlockReduce<long long, kTileThreads>;
+  __shared__ typename Reduce::TempStorage tmp;
+  int r, l;
+  count_bytes(text, n, (long long)blockIdx.x * kTile + threadIdx.x * kPerThread, r, l);
+  const long long s = Reduce(tmp).Sum(((long long)r << 32) | l);      // both counts are <= kTile: no carry between halves
+  if (threadIdx.x == 0) {
+    rec_cnt[blockIdx.x] = (int)(s >> 32);
+    nl_cnt[blockIdx.x] = (int)(s & 0xffffffff);
+  }
+}
+
+// exclusive scan of in[0, n) into out[0, n), out[n] = the total (one block)
+__global__ void __launch_bounds__(1024) exclusive_scan_kernel(const int* __restrict__ in, int* __restrict__ out, int n) {
+  using Scan = cub::BlockScan<int, 1024>;
+  __shared__ typename Scan::TempStorage tmp;
+  const int per = (n + 1023) / 1024;
+  const int lo = min(n, (int)threadIdx.x * per), hi = min(n, lo + per);
+  int s = 0;
+  for (int i = lo; i < hi; ++i) s += in[i];
+  int run, total;
+  Scan(tmp).ExclusiveSum(s, run, total);
+  for (int i = lo; i < hi; ++i) {
+    out[i] = run;
+    run += in[i];
+  }
+  if (threadIdx.x == 0) out[n] = total;
+}
+
+// rec_off[i] = first byte of record i, rec_line[i] = its line number (newlines before it), for the first `cap` records
+__global__ void __launch_bounds__(kTileThreads)
+line_index_kernel(const unsigned char* __restrict__ text, long long n, const int* __restrict__ rec_base,
+                  const int* __restrict__ nl_base, long long cap, long long* __restrict__ rec_off,
+                  long long* __restrict__ rec_line) {
+  using Scan = cub::BlockScan<long long, kTileThreads>;
+  __shared__ typename Scan::TempStorage tmp;
+  const long long lo = (long long)blockIdx.x * kTile + threadIdx.x * kPerThread;
+  int r, l;
+  count_bytes(text, n, lo, r, l);
+  long long before;
+  Scan(tmp).ExclusiveSum(((long long)r << 32) | l, before);
+  long long rec = rec_base[blockIdx.x] + (before >> 32);
+  long long line = nl_base[blockIdx.x] + (before & 0xffffffff);
+  for (int k = 0; k < kPerThread; ++k) {
+    const long long p = lo + k;
+    if (p >= n) break;
+    const unsigned char c = text[p];
+    if ((p == 0 || text[p - 1] == '\n') && c != '\n') {
+      if (rec < cap) { rec_off[rec] = p; rec_line[rec] = line; }
+      ++rec;
+    }
+    line += c == '\n';
+  }
+}
+
+// ---- parse ---------------------------------------------------------------------------------------------------------
+struct ParseArgs {
+  const unsigned char* text;
+  long long nbytes;
+  int C;
+  DevVocab tok, pth, tgt;
+  const long long* rec_off;
+  const int* n_rec;               // records in the chunk (line_count scan total)
+  long long cap;                  // rows reserved behind the pool's end
+  int32_t *src, *path, *dst, *target;     // pool rows from the live end
+  float* mask;
+  uint8_t* keep;                  // per record: passes the training filter
+  unsigned long long* bad;        // lowest malformed record << 2 | kind
+};
+
+// a part that ends at a separator: part kk of context field f, bytes [start, start + len) of the line
+__device__ __forceinline__ void note_part(longlong2* parts, int C, long long f, int kk, long long start, long long len,
+                                          bool by_space) {
+  if (f < 1 || f > C || kk > 2) return;
+  if (by_space && kk == 0 && len == 0) return;        // an empty context: all three parts stay absent (PAD)
+  parts[(f - 1) * 3 + kk] = make_longlong2(start, len);
+}
+
+__global__ void __launch_bounds__(32 * kParseWarps) parse_kernel(const __grid_constant__ ParseArgs a) {
+  extern __shared__ longlong2 shm[];
+  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+  const int C = a.C;
+  longlong2* parts = shm + (size_t)warp * 3 * C;       // per part: (start, len), len -1 = absent
+  const long long R = min((long long)*a.n_rec, a.cap);
+  const unsigned lt = (1u << lane) - 1;
+  for (long long li = (long long)blockIdx.x * kParseWarps + warp; li < R; li += (long long)gridDim.x * kParseWarps) {
+    const long long b0 = a.rec_off[li];
+    long long e = li + 1 < R ? a.rec_off[li + 1] : a.nbytes;     // a record runs to the next one (blank lines included)
+    const unsigned char* p = a.text + b0;
+    while (e > b0 && (a.text[e - 1] == '\n' || a.text[e - 1] == '\r')) --e;
+    const long long len = e - b0;
+    for (int i = lane; i < 3 * C; i += 32) parts[i] = make_longlong2(0, -1);
+    __syncwarp();
+    long long f = 0;              // spaces before the window: the field the window starts in
+    int k = 0;                    // context commas since the current field began
+    long long last = -1;          // the last separator before the window
+    long long tgt_len = -1;       // length of field 0 (the target) once its space is seen
+    bool bad3 = false;            // a context among the first C has a third comma
+    for (long long w = 0; w < len; w += 32) {
+      const long long pos = w + lane;
+      const unsigned char c = pos < len ? p[pos] : 0;
+      const unsigned sp = __ballot_sync(kFull, c == ' ');
+      const long long f_here = f + __popc(sp & lt);
+      const unsigned cm = __ballot_sync(kFull, c == ',' && f_here >= 1);     // commas inside field 0 are target bytes
+      const unsigned sep = sp | cm;
+      if ((sep >> lane) & 1) {
+        const unsigned before = sep & lt;
+        const long long start = before ? w + (31 - __clz(before)) + 1 : last + 1;
+        const unsigned sp_before = sp & lt;
+        int kk;
+        if (sp_before) {
+          const int ls = 31 - __clz(sp_before);
+          kk = __popc(cm & lt & ~((2u << ls) - 1u));
+        } else {
+          kk = k + __popc(cm & lt);
+        }
+        if (c == ',' && kk >= 2 && f_here <= C) bad3 = true;
+        note_part(parts, C, f_here, kk, start, pos - start, c == ' ');
+      }
+      if (f == 0 && sp) tgt_len = w + __ffs(sp) - 1;
+      if (sep) last = w + (31 - __clz(sep));
+      if (sp) {
+        const int ls = 31 - __clz(sp);
+        k = __popc(cm & ~((2u << ls) - 1u));
+      } else {
+        k += __popc(cm);
+      }
+      f += __popc(sp);
+    }
+    if (lane == 0 && f >= 1) note_part(parts, C, f, k, last + 1, len - last - 1, true);    // the line's last part
+    const bool any3 = __any_sync(kFull, bad3);
+    const int kind = any3 ? 2 : (f + 1 != C + 1 ? 1 : 0);
+    if (kind) {
+      if (lane == 0) atomicMin(a.bad, ((unsigned long long)li << 2) | (unsigned long long)kind);
+      __syncwarp();
+      continue;
+    }
+    if (tgt_len < 0) tgt_len = len;
+    __syncwarp();
+    for (int i = lane; i < 3 * C; i += 32) {
+      const longlong2 q = parts[i];
+      const DevVocab& v = (i % 3 == 1) ? a.pth : a.tok;
+      const int32_t r = q.y < 0 ? v.pad : lookup(v, p + q.x, q.y);
+      parts[i].x = r;
+    }
+    int32_t ty = 0;
+    if (lane == 0) ty = tgt_len == 0 ? a.tgt.oov : lookup(a.tgt, p, tgt_len);
+    __syncwarp();
+    const long long row = li * C;
+    int max_s = INT32_MIN, max_p = INT32_MIN, max_t = INT32_MIN;
+    for (int c = lane; c < C; c += 32) {
+      const int32_t s = (int32_t)parts[3 * c].x, q = (int32_t)parts[3 * c + 1].x, t = (int32_t)parts[3 * c + 2].x;
+      a.src[row + c] = s;
+      a.path[row + c] = q;
+      a.dst[row + c] = t;
+      a.mask[row + c] = (s != a.tok.pad || t != a.tok.pad || q != a.pth.pad) ? 1.0f : 0.0f;
+      max_s = max(max_s, s);
+      max_p = max(max_p, q);
+      max_t = max(max_t, t);
+    }
+    max_s = __reduce_max_sync(kFull, max_s);
+    max_p = __reduce_max_sync(kFull, max_p);
+    max_t = __reduce_max_sync(kFull, max_t);
+    if (lane == 0) {
+      const bool any_valid = max_s != a.tok.pad || max_t != a.tok.pad || max_p != a.pth.pad;
+      a.target[li] = ty;
+      a.keep[li] = (any_valid && ty > a.tgt.oov) ? 1 : 0;
+    }
+    __syncwarp();
+  }
+}
+
+// ---- pool commit -----------------------------------------------------------------------------------------------------
+__global__ void __launch_bounds__(256) keep_count_kernel(const uint8_t* __restrict__ keep, const int* __restrict__ n_rec,
+                                                         long long cap, int* __restrict__ cnt) {
+  using Reduce = cub::BlockReduce<int, 256>;
+  __shared__ typename Reduce::TempStorage tmp;
+  const long long R = min((long long)*n_rec, cap);
+  const long long lo = (long long)blockIdx.x * kRowTile + threadIdx.x * 4;
+  int s = 0;
+  for (int k = 0; k < 4; ++k) s += (lo + k < R) ? keep[lo + k] : 0;
+  s = Reduce(tmp).Sum(s);
+  if (threadIdx.x == 0) cnt[blockIdx.x] = s;
+}
+
+// holes[j] = the j-th dropped row below the kept count, movers[j] = the j-th kept row at or beyond it (_RowPool.commit);
+// *n_moves = their number.  K(i) = kept rows before row i; kept = K(R).
+__global__ void __launch_bounds__(256)
+commit_index_kernel(const uint8_t* __restrict__ keep, const int* __restrict__ n_rec, long long cap,
+                    const int* __restrict__ base, int tiles, int* __restrict__ holes, int* __restrict__ movers,
+                    int* __restrict__ n_moves) {
+  using Scan = cub::BlockScan<int, 256>;
+  using Reduce = cub::BlockReduce<int, 256>;
+  __shared__ typename Scan::TempStorage tmp;
+  __shared__ typename Reduce::TempStorage rtmp;
+  __shared__ int Kk_shared;
+  const long long R = min((long long)*n_rec, cap);
+  const int kept = base[tiles];
+  // K(kept): the kept rows below the kept count
+  const int tk = kept / kRowTile;
+  int part = 0;
+  for (long long i = (long long)tk * kRowTile + threadIdx.x; i < kept; i += 256) part += keep[i];
+  part = Reduce(rtmp).Sum(part);                 // valid in thread 0 only
+  if (threadIdx.x == 0) Kk_shared = (tk < tiles ? base[tk] : kept) + part;
+  __syncthreads();
+  const int Kk = Kk_shared;
+  const long long lo = (long long)blockIdx.x * kRowTile + threadIdx.x * 4;
+  int s = 0;
+  for (int k = 0; k < 4; ++k) s += (lo + k < R) ? keep[lo + k] : 0;
+  int K;
+  Scan(tmp).ExclusiveSum(s, K);
+  K += base[blockIdx.x];
+  for (int k = 0; k < 4; ++k) {
+    const long long i = lo + k;
+    if (i >= R) break;
+    const int kp = keep[i];
+    if (i < kept && !kp) holes[i - K] = (int)i;
+    if (i >= kept && kp) movers[K - Kk] = (int)i;
+    K += kp;
+  }
+  if (blockIdx.x == 0 && threadIdx.x == 0) *n_moves = kept - Kk;
+}
+
+struct PoolRows {
+  int32_t *src, *path, *dst, *target;
+  float* mask;
+};
+
+// pool row to[j] <- pool row from[j] for j < *count (one warp per row; the two index sets are disjoint)
+__global__ void __launch_bounds__(256)
+move_rows_kernel(PoolRows pool, int C, long long row0, const int* __restrict__ to, const int* __restrict__ from,
+                 const int* __restrict__ count) {
+  const int n = *count;
+  const int lane = threadIdx.x & 31;
+  for (long long j = ((long long)blockIdx.x * 256 + threadIdx.x) >> 5; j < n; j += ((long long)gridDim.x * 256) >> 5) {
+    const long long d = (row0 + to[j]) * C, s = (row0 + from[j]) * C;
+    for (int c = lane; c < C; c += 32) {
+      pool.src[d + c] = pool.src[s + c];
+      pool.path[d + c] = pool.path[s + c];
+      pool.dst[d + c] = pool.dst[s + c];
+      pool.mask[d + c] = pool.mask[s + c];
+    }
+    if (lane == 0) pool.target[row0 + to[j]] = pool.target[row0 + from[j]];
+  }
+}
+
+// ---- draw ------------------------------------------------------------------------------------------------------------
+// c2v_pool_take's index sets, one block: holes = the picks below new_n in ascending order, movers = the rows of the tail
+// [new_n, n) that were not picked, ascending.  tail: b bytes of scratch.
+__global__ void __launch_bounds__(1024)
+draw_index_kernel(const long long* __restrict__ pick, int b, long long n, uint8_t* __restrict__ tail,
+                  int* __restrict__ holes, int* __restrict__ movers, int* __restrict__ n_moves) {
+  using Scan = cub::BlockScan<int, 1024>;
+  __shared__ typename Scan::TempStorage tmp;
+  const long long new_n = n - b;
+  for (int i = threadIdx.x; i < b; i += 1024) tail[i] = 0;
+  __syncthreads();
+  for (int i = threadIdx.x; i < b; i += 1024)
+    if (pick[i] >= new_n) tail[pick[i] - new_n] = 1;
+  __syncthreads();
+  for (int i = threadIdx.x; i < b; i += 1024) {      // a pick's rank among the picks below new_n: how many are smaller
+    const long long v = pick[i];
+    if (v >= new_n) continue;
+    int rank = 0;
+    for (int q = 0; q < b; ++q) rank += pick[q] < v;
+    holes[rank] = (int)v;
+  }
+  const int per = (b + 1023) / 1024;
+  const int lo = min(b, (int)threadIdx.x * per), hi = min(b, lo + per);
+  int s = 0;
+  for (int i = lo; i < hi; ++i) s += !tail[i];
+  int run, total;
+  Scan(tmp).ExclusiveSum(s, run, total);
+  for (int i = lo; i < hi; ++i)
+    if (!tail[i]) movers[run++] = (int)(new_n + i);
+  if (threadIdx.x == 0) *n_moves = total;
+}
+
+// out row i - lo <- pool row pick[i] for i in [lo, hi) (one warp per row)
+__global__ void __launch_bounds__(256)
+gather_kernel(PoolRows pool, int C, const long long* __restrict__ pick, int lo, int hi, PoolRows out) {
+  const int lane = threadIdx.x & 31;
+  for (long long i = lo + (((long long)blockIdx.x * 256 + threadIdx.x) >> 5); i < hi; i += ((long long)gridDim.x * 256) >> 5) {
+    const long long r = pick[i], d = (i - lo) * C, s = r * C;
+    for (int c = lane; c < C; c += 32) {
+      out.src[d + c] = pool.src[s + c];
+      out.path[d + c] = pool.path[s + c];
+      out.dst[d + c] = pool.dst[s + c];
+      out.mask[d + c] = pool.mask[s + c];
+    }
+    if (lane == 0) out.target[i - lo] = pool.target[r];
+  }
+}
+
+}  // namespace
+
+struct c2v_reader {
+  int device = 0, C = 0, num_sms = 1;
+  DevVocab tok{}, pth{}, tgt{};
+  // shuffle pool: rows [0, live) are the pool, [live, cap) room for the next chunk
+  PoolRows pool{};
+  long long pool_cap = 0, live = 0;
+  // per-chunk scratch (sized for the largest chunk so far)
+  long long text_cap = 0, row_cap = 0, pick_cap = 0;
+  int *rec_cnt = nullptr, *nl_cnt = nullptr, *rec_base = nullptr, *nl_base = nullptr;     // [tiles + 1]
+  long long *rec_off = nullptr, *rec_line = nullptr;                                        // [rows]
+  uint8_t* keep = nullptr;                                                                  // [rows]
+  int *keep_cnt = nullptr, *keep_base = nullptr;                                            // [row tiles + 1]
+  int *holes = nullptr, *movers = nullptr;                                                  // [max(rows, picks)]
+  long long* pick = nullptr;                                                                // [picks]
+  uint8_t* tail = nullptr;                                                                  // [picks]
+  unsigned long long* bad = nullptr;
+  int* n_moves = nullptr;
+  struct Status { int records, kept; unsigned long long bad; long long line; } *host = nullptr;   // pinned read-back
+  size_t bytes = 0;               // device memory held
+};
+
+namespace {
+
+int rfail(int code, const std::string& msg) {
+  c2v::set_global_error(msg);
+  return code;
+}
+
+#define RD_CUDA(call)                                                                                   \
+  do {                                                                                                  \
+    cudaError_t _e = (call);                                                                            \
+    if (_e != cudaSuccess) return rfail(C2V_ERR_CUDA, std::string(#call) + ": " + cudaGetErrorString(_e)); \
+  } while (0)
+
+template <class T>
+int realloc_dev(c2v_reader* r, T*& p, long long old_n, long long n) {
+  if (p) { RD_CUDA(cudaFree(p)); r->bytes -= (size_t)old_n * sizeof(T); }
+  p = nullptr;
+  RD_CUDA(cudaMalloc(&p, (size_t)(n > 0 ? n : 1) * sizeof(T)));
+  r->bytes += (size_t)n * sizeof(T);
+  return C2V_OK;
+}
+
+// scratch for a chunk of `nbytes` bytes and up to `rows` records; draws of up to `picks` rows
+int reserve_scratch(c2v_reader* r, long long nbytes, long long rows, long long picks, cudaStream_t st) {
+  const long long tiles = (nbytes + kTile - 1) / kTile + 1, row_tiles = (rows + kRowTile - 1) / kRowTile + 1;
+  const long long old_tiles = (r->text_cap + kTile - 1) / kTile + 1, old_row_tiles = (r->row_cap + kRowTile - 1) / kRowTile + 1;
+  if (nbytes > r->text_cap || rows > r->row_cap || picks > r->pick_cap) RD_CUDA(cudaStreamSynchronize(st));
+  int rc;
+  if (nbytes > r->text_cap) {
+    for (int** p : {&r->rec_cnt, &r->nl_cnt, &r->rec_base, &r->nl_base})
+      if ((rc = realloc_dev(r, *p, r->text_cap ? old_tiles : 0, tiles))) return rc;
+    r->text_cap = nbytes;
+  }
+  const long long old_idx = r->row_cap > r->pick_cap ? r->row_cap : r->pick_cap;     // holes / movers serve both
+  const long long idx = rows > picks ? rows : picks;
+  if (idx > old_idx) {
+    if ((rc = realloc_dev(r, r->holes, old_idx, idx)) || (rc = realloc_dev(r, r->movers, old_idx, idx))) return rc;
+  }
+  if (rows > r->row_cap) {
+    if ((rc = realloc_dev(r, r->rec_off, r->row_cap ? r->row_cap + 1 : 0, rows + 1)) ||
+        (rc = realloc_dev(r, r->rec_line, r->row_cap ? r->row_cap + 1 : 0, rows + 1)) ||
+        (rc = realloc_dev(r, r->keep, r->row_cap, rows)) ||
+        (rc = realloc_dev(r, r->keep_cnt, r->row_cap ? old_row_tiles : 0, row_tiles)) ||
+        (rc = realloc_dev(r, r->keep_base, r->row_cap ? old_row_tiles : 0, row_tiles)))
+      return rc;
+    r->row_cap = rows;
+  }
+  if (picks > r->pick_cap) {
+    if ((rc = realloc_dev(r, r->pick, r->pick_cap, picks)) || (rc = realloc_dev(r, r->tail, r->pick_cap, picks))) return rc;
+    r->pick_cap = picks;
+  }
+  return C2V_OK;
+}
+
+// room for `more` rows behind the live end; the live rows move to the grown arrays
+int reserve_pool(c2v_reader* r, long long more, cudaStream_t st) {
+  const long long need = r->live + more;
+  if (need <= r->pool_cap) return C2V_OK;
+  long long cap = r->pool_cap ? 2 * r->pool_cap : 1024;
+  if (cap < need) cap = need;
+  const size_t C = (size_t)r->C, n = (size_t)r->live;
+  PoolRows g{};
+  RD_CUDA(cudaMalloc(&g.src, (size_t)cap * C * 4));
+  RD_CUDA(cudaMalloc(&g.path, (size_t)cap * C * 4));
+  RD_CUDA(cudaMalloc(&g.dst, (size_t)cap * C * 4));
+  RD_CUDA(cudaMalloc(&g.mask, (size_t)cap * C * 4));
+  RD_CUDA(cudaMalloc(&g.target, (size_t)cap * 4));
+  if (r->pool_cap) {
+    RD_CUDA(cudaMemcpyAsync(g.src, r->pool.src, n * C * 4, cudaMemcpyDeviceToDevice, st));
+    RD_CUDA(cudaMemcpyAsync(g.path, r->pool.path, n * C * 4, cudaMemcpyDeviceToDevice, st));
+    RD_CUDA(cudaMemcpyAsync(g.dst, r->pool.dst, n * C * 4, cudaMemcpyDeviceToDevice, st));
+    RD_CUDA(cudaMemcpyAsync(g.mask, r->pool.mask, n * C * 4, cudaMemcpyDeviceToDevice, st));
+    RD_CUDA(cudaMemcpyAsync(g.target, r->pool.target, n * 4, cudaMemcpyDeviceToDevice, st));
+    RD_CUDA(cudaStreamSynchronize(st));
+    for (void* p : {(void*)r->pool.src, (void*)r->pool.path, (void*)r->pool.dst, (void*)r->pool.mask, (void*)r->pool.target})
+      RD_CUDA(cudaFree(p));
+    r->bytes -= (size_t)r->pool_cap * (4 * C + 1) * 4;
+  }
+  r->pool = g;
+  r->pool_cap = cap;
+  r->bytes += (size_t)cap * (4 * C + 1) * 4;
+  return C2V_OK;
+}
+
+DevVocab dev_vocab(const c2v_reader_vocab& v) {
+  return DevVocab{(const DevSlot*)v.slots, (const unsigned char*)v.bytes, (unsigned long long)v.mask, v.oov, v.pad};
+}
+
+size_t parse_smem(int C) { return (size_t)kParseWarps * 3 * C * sizeof(longlong2); }
+
+}  // namespace
+
+extern "C" {
+
+int c2v_reader_create(int32_t max_contexts, const c2v_reader_vocab* tok, const c2v_reader_vocab* path,
+                      const c2v_reader_vocab* target, int device, c2v_reader** out) {
+  if (!out || !tok || !path || !target) return rfail(C2V_ERR_INVALID, "c2v_reader_create: NULL argument");
+  *out = nullptr;
+  if (max_contexts < 1) return rfail(C2V_ERR_INVALID, "c2v_reader_create: max_contexts must be >= 1");
+  for (const c2v_reader_vocab* v : {tok, path, target})
+    if (!v->slots || !v->bytes || ((v->mask + 1) & v->mask) != 0)
+      return rfail(C2V_ERR_INVALID, "c2v_reader_create: a vocabulary needs device slots, bytes and a 2^k - 1 mask");
+  RD_CUDA(cudaSetDevice(device));
+  cudaDeviceProp prop;
+  RD_CUDA(cudaGetDeviceProperties(&prop, device));
+  if (parse_smem(max_contexts) > prop.sharedMemPerBlockOptin)
+    return rfail(C2V_ERR_UNSUPPORTED, "c2v_reader_create: max_contexts too large for the parse kernel's shared memory");
+  RD_CUDA(cudaFuncSetAttribute(parse_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)parse_smem(max_contexts)));
+  c2v_reader* r = new c2v_reader();
+  r->device = device;
+  r->C = max_contexts;
+  r->num_sms = prop.multiProcessorCount;
+  r->tok = dev_vocab(*tok);
+  r->pth = dev_vocab(*path);
+  r->tgt = dev_vocab(*target);
+  cudaError_t e = cudaMalloc(&r->bad, sizeof(unsigned long long));
+  if (e == cudaSuccess) e = cudaMalloc(&r->n_moves, sizeof(int));
+  if (e == cudaSuccess) e = cudaHostAlloc((void**)&r->host, sizeof(c2v_reader::Status), cudaHostAllocDefault);
+  if (e != cudaSuccess) {
+    c2v_reader_destroy(r);
+    return rfail(C2V_ERR_CUDA, std::string("c2v_reader_create: ") + cudaGetErrorString(e));
+  }
+  r->bytes = sizeof(unsigned long long) + sizeof(int);
+  *out = r;
+  return C2V_OK;
+}
+
+void c2v_reader_destroy(c2v_reader* r) {
+  if (!r) return;
+  cudaSetDevice(r->device);
+  cudaDeviceSynchronize();
+  for (void* p : {(void*)r->pool.src, (void*)r->pool.path, (void*)r->pool.dst, (void*)r->pool.mask, (void*)r->pool.target,
+                  (void*)r->rec_cnt, (void*)r->nl_cnt, (void*)r->rec_base, (void*)r->nl_base, (void*)r->rec_off,
+                  (void*)r->rec_line, (void*)r->keep, (void*)r->keep_cnt, (void*)r->keep_base, (void*)r->holes,
+                  (void*)r->movers, (void*)r->pick, (void*)r->tail, (void*)r->bad, (void*)r->n_moves})
+    if (p) cudaFree(p);
+  if (r->host) cudaFreeHost(r->host);
+  delete r;
+}
+
+int c2v_reader_parse_chunk(c2v_reader* r, const char* text, int64_t nbytes, int64_t* kept, int64_t* bad_line,
+                           int32_t* bad_kind, void* stream) {
+  if (!r || !text || !kept || !bad_line || !bad_kind || nbytes < 0)
+    return rfail(C2V_ERR_INVALID, "c2v_reader_parse_chunk: NULL argument or negative size");
+  *kept = 0; *bad_line = -1; *bad_kind = 0;
+  if (nbytes == 0) return C2V_OK;
+  RD_CUDA(cudaSetDevice(r->device));
+  cudaStream_t st = (cudaStream_t)stream;
+  const long long cap = nbytes / (r->C + 1) + 1;      // a well-formed line is at least MAX_CONTEXTS spaces + a newline long
+  int rc;
+  if ((rc = reserve_scratch(r, nbytes, cap, 0, st)) || (rc = reserve_pool(r, cap, st))) return rc;
+  const int tiles = (int)((nbytes + kTile - 1) / kTile), row_tiles = (int)((cap + kRowTile - 1) / kRowTile);
+  const unsigned char* t = (const unsigned char*)text;
+  RD_CUDA(cudaMemsetAsync(r->bad, 0xff, sizeof(unsigned long long), st));
+  if (tiles) line_count_kernel<<<tiles, kTileThreads, 0, st>>>(t, nbytes, r->rec_cnt, r->nl_cnt);
+  exclusive_scan_kernel<<<1, 1024, 0, st>>>(r->rec_cnt, r->rec_base, tiles);
+  exclusive_scan_kernel<<<1, 1024, 0, st>>>(r->nl_cnt, r->nl_base, tiles);
+  if (tiles) line_index_kernel<<<tiles, kTileThreads, 0, st>>>(t, nbytes, r->rec_base, r->nl_base, cap, r->rec_off, r->rec_line);
+  const long long l0 = r->live * r->C;
+  ParseArgs a{t, nbytes, r->C, r->tok, r->pth, r->tgt, r->rec_off, r->rec_base + tiles, cap,
+              r->pool.src + l0, r->pool.path + l0, r->pool.dst + l0, r->pool.target + r->live, r->pool.mask + l0,
+              r->keep, r->bad};
+  long long grid = (cap + kParseWarps - 1) / kParseWarps;
+  if (grid > (long long)r->num_sms * 16) grid = (long long)r->num_sms * 16;
+  parse_kernel<<<(unsigned)grid, 32 * kParseWarps, parse_smem(r->C), st>>>(a);
+  keep_count_kernel<<<row_tiles, 256, 0, st>>>(r->keep, r->rec_base + tiles, cap, r->keep_cnt);
+  exclusive_scan_kernel<<<1, 1024, 0, st>>>(r->keep_cnt, r->keep_base, row_tiles);
+  commit_index_kernel<<<row_tiles, 256, 0, st>>>(r->keep, r->rec_base + tiles, cap, r->keep_base, row_tiles, r->holes,
+                                                 r->movers, r->n_moves);
+  move_rows_kernel<<<r->num_sms * 8, 256, 0, st>>>(r->pool, r->C, r->live, r->holes, r->movers, r->n_moves);
+  RD_CUDA(cudaGetLastError());
+  RD_CUDA(cudaMemcpyAsync(&r->host->records, r->rec_base + tiles, sizeof(int), cudaMemcpyDeviceToHost, st));
+  RD_CUDA(cudaMemcpyAsync(&r->host->kept, r->keep_base + row_tiles, sizeof(int), cudaMemcpyDeviceToHost, st));
+  RD_CUDA(cudaMemcpyAsync(&r->host->bad, r->bad, sizeof(unsigned long long), cudaMemcpyDeviceToHost, st));
+  RD_CUDA(cudaStreamSynchronize(st));
+  if (r->host->records > cap) {
+    *bad_kind = 3;
+    return rfail(C2V_ERR_INVALID, "c2v_reader_parse_chunk: more records than a chunk of this size holds well-formed lines");
+  }
+  if (r->host->bad != ~0ull) {
+    const long long li = (long long)(r->host->bad >> 2);
+    RD_CUDA(cudaMemcpyAsync(&r->host->line, r->rec_line + li, sizeof(long long), cudaMemcpyDeviceToHost, st));
+    RD_CUDA(cudaStreamSynchronize(st));
+    *bad_line = r->host->line;
+    *bad_kind = (int32_t)(r->host->bad & 3);
+    return rfail(C2V_ERR_INVALID, std::string("c2v_reader_parse_chunk: malformed line ") + std::to_string(*bad_line) +
+                                      (*bad_kind == 2 ? " (a context has more than 3 parts)" : " (field count)"));
+  }
+  *kept = r->host->kept;
+  r->live += r->host->kept;
+  return C2V_OK;
+}
+
+int c2v_reader_draw(c2v_reader* r, const int64_t* pick, int32_t b, int32_t lo, int32_t hi, int32_t* src, int32_t* path,
+                    int32_t* tgt, float* mask, int32_t* target, void* stream) {
+  if (!r || !pick) return rfail(C2V_ERR_INVALID, "c2v_reader_draw: NULL argument");
+  if (b < 1 || b > r->live) return rfail(C2V_ERR_INVALID, "c2v_reader_draw: b must be in [1, live rows]");
+  if (lo < 0 || lo > hi || hi > b) return rfail(C2V_ERR_INVALID, "c2v_reader_draw: need 0 <= lo <= hi <= b");
+  if (hi > lo && (!src || !path || !tgt || !mask || !target)) return rfail(C2V_ERR_INVALID, "c2v_reader_draw: NULL output");
+  RD_CUDA(cudaSetDevice(r->device));
+  cudaStream_t st = (cudaStream_t)stream;
+  int rc;
+  if ((rc = reserve_scratch(r, 0, 0, b, st))) return rc;
+  RD_CUDA(cudaMemcpyAsync(r->pick, pick, (size_t)b * sizeof(long long), cudaMemcpyHostToDevice, st));
+  draw_index_kernel<<<1, 1024, 0, st>>>(r->pick, b, r->live, r->tail, r->holes, r->movers, r->n_moves);
+  if (hi > lo) {
+    long long grid = ((long long)(hi - lo) * 32 + 255) / 256;
+    if (grid > (long long)r->num_sms * 8) grid = (long long)r->num_sms * 8;
+    gather_kernel<<<(unsigned)grid, 256, 0, st>>>(r->pool, r->C, r->pick, lo, hi, PoolRows{src, path, tgt, target, mask});
+  }
+  // every picked row has been gathered (same stream) before a hole is overwritten
+  move_rows_kernel<<<r->num_sms * 4, 256, 0, st>>>(r->pool, r->C, 0, r->holes, r->movers, r->n_moves);
+  RD_CUDA(cudaGetLastError());
+  r->live -= b;
+  return C2V_OK;
+}
+
+int64_t c2v_reader_live_rows(const c2v_reader* r) { return r ? r->live : -1; }
+
+size_t c2v_reader_device_bytes(const c2v_reader* r) { return r ? r->bytes : 0; }
+
+}  // extern "C"

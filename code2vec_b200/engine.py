@@ -36,6 +36,10 @@ class c2v_table_shards(C.Structure):
     _fields_ = [("world", C.c_int32), ("rank", C.c_int32), ("tok", C.c_void_p * 8), ("path", C.c_void_p * 8)]
 
 
+class c2v_reader_vocab(C.Structure):
+    _fields_ = [("slots", C.c_void_p), ("bytes", C.c_void_p), ("mask", C.c_uint64), ("oov", C.c_int32), ("pad", C.c_int32)]
+
+
 class _DeviceArray:
     """A raw device allocation presented through __cuda_array_interface__ so torch can view it."""
 
@@ -105,6 +109,14 @@ _SIGNATURES = {
     "c2v_phase_count": (C.c_int, []),
     "c2v_phase_name": (C.c_char_p, [C.c_int]),
     "c2v_phase_stats": (C.c_int, [_P, C.c_int, C.POINTER(C.c_double), C.POINTER(C.c_int64), C.c_int]),
+    # device reader (device_reader.py)
+    "c2v_reader_create": (C.c_int, [_I32, C.POINTER(c2v_reader_vocab), C.POINTER(c2v_reader_vocab),
+                                    C.POINTER(c2v_reader_vocab), C.c_int, C.POINTER(_P)]),
+    "c2v_reader_destroy": (None, [_P]),
+    "c2v_reader_parse_chunk": (C.c_int, [_P, _P, C.c_int64, C.POINTER(C.c_int64), C.POINTER(C.c_int64), C.POINTER(_I32), _P]),
+    "c2v_reader_draw": (C.c_int, [_P, _P, _I32, _I32, _I32, _P, _P, _P, _P, _P, _P]),
+    "c2v_reader_live_rows": (C.c_int64, [_P]),
+    "c2v_reader_device_bytes": (C.c_size_t, [_P]),
 }
 
 _lib = None

@@ -6,6 +6,7 @@
 //
 // C ABI (bound with ctypes in path_context_reader.py):
 //   c2v_vocab_create / c2v_vocab_destroy
+//   c2v_vocab_export (the tables, for the device reader)
 //   c2v_parse_chunk
 #include <stdint.h>
 #include <string.h>
@@ -207,6 +208,21 @@ void* c2v_vocab_create(const char* words, const int64_t* offsets, const int32_t*
 void c2v_vocab_destroy(void* v) { delete (Vocab*)v; }
 
 int32_t c2v_vocab_lookup(const void* v, const char* word, int64_t len) { return ((const Vocab*)v)->lookup(word, (size_t)len); }
+
+// The table as it is, for the device reader (c2v_b200.h c2v_reader_vocab): *slots -> mask + 1 slots of 24 bytes
+// {uint64 h, int64 off, int32 len, int32 idx} (h == 0: empty), *bytes -> the words' bytes (*n_bytes of them), and the
+// OOV / PAD indices.  The pointers stay valid until c2v_vocab_destroy.
+void c2v_vocab_export(const void* vp, const void** slots, uint64_t* mask, const char** bytes, int64_t* n_bytes,
+                      int32_t* oov, int32_t* pad) {
+  static_assert(sizeof(Vocab::Slot) == 24, "the device reader reads 24-byte slots");
+  const Vocab* v = (const Vocab*)vp;
+  *slots = v->slots.data();
+  *mask = v->mask;
+  *bytes = v->bytes.data();
+  *n_bytes = (int64_t)v->bytes.size();
+  *oov = v->oov;
+  *pad = v->pad;
+}
 
 // Parses the complete lines in text[0, len) (the last line may lack a trailing newline).
 // Outputs hold one row per line, in line order: src/path/dst [n, C] int32, mask [n, C] float32,

@@ -448,6 +448,56 @@ int c2v_phase_count(void);
 const char* c2v_phase_name(int phase);
 int c2v_phase_stats(c2v_engine* e, int phase, double* total_ms, int64_t* count, int reset);
 
+/* ---- Device reader (DESIGN.md §6d) ------------------------------------------------------------------------------
+ * Turns `.c2v` training text in device memory into the rows of a training shuffle pool held on the device, and draws
+ * batches from that pool into caller buffers: the host reader's train path (path_context_reader.py
+ * _iterate_batches_native: native/batcher.cpp c2v_parse_chunk in train mode, _RowPool.commit, _RowPool.take) with every
+ * row, every pool move and every batch identical to the host's for the same draws.  A reader handle is independent of
+ * any engine handle.  Failures return a negative c2v_status with the message in c2v_last_error(NULL) (of the calling
+ * thread).  Calls on one handle run on one caller stream (or the caller orders them); one host thread at a time. */
+typedef struct c2v_reader c2v_reader;
+
+/* One vocabulary as native/batcher.cpp holds it (c2v_vocab_export), copied to the device by the caller and kept alive
+ * until c2v_reader_destroy: slots [mask + 1] of 24 bytes {uint64 h (FNV-1a 64 of the word, 0 = empty), int64 off,
+ * int32 len, int32 idx}, probed linearly from h & mask; bytes: the words, concatenated. */
+typedef struct c2v_reader_vocab {
+  const void* slots;
+  const char* bytes;
+  uint64_t mask;
+  int32_t oov;     /* index of an unknown word (and of an empty target) */
+  int32_t pad;     /* index of an absent context part                     */
+} c2v_reader_vocab;
+
+/* A reader for rows of max_contexts contexts on `device`, with an empty pool.  The handle allocates its own device
+ * buffers (pool, per-chunk scratch), growing them as chunks and draws need; c2v_reader_device_bytes reports them. */
+int c2v_reader_create(int32_t max_contexts, const c2v_reader_vocab* token, const c2v_reader_vocab* path,
+                      const c2v_reader_vocab* target, int device, c2v_reader** out);
+void c2v_reader_destroy(c2v_reader* r);      /* synchronises the device, then frees the handle's buffers */
+
+/* Parses the complete lines of text[0, nbytes) (device memory; the last line may lack its newline) as c2v_parse_chunk
+ * does in train mode -- trailing '\r' stripped, blank lines skipped, exactly max_contexts + 1 space-separated fields, at
+ * most 3 comma-separated parts per context, the row filter "any index != PAD and target > OOV" -- and appends the kept
+ * rows behind the pool's live end in the host pool's order (_RowPool.commit: the j-th dropped row below the kept count
+ * takes the j-th kept row beyond it).  Synchronises `stream` and sets *kept to the rows added.  A malformed chunk leaves
+ * the pool unusable and returns C2V_ERR_INVALID with *bad_line = the lowest malformed line's number (0-based, blank
+ * lines counted) and *bad_kind = 1 (field count) or 2 (a context with more than 3 parts), or *bad_kind = 3 when the
+ * chunk has more lines than nbytes / (max_contexts + 1) + 1, which no well-formed chunk has. */
+int c2v_reader_parse_chunk(c2v_reader* r, const char* text, int64_t nbytes, int64_t* kept, int64_t* bad_line,
+                           int32_t* bad_kind, void* stream);
+
+/* One draw of b rows from the pool's n live rows (_RowPool.take / c2v_pool_take): pick[0, b) are b distinct row
+ * indices in [0, n) (host memory; page-locked keeps the copy asynchronous; unchanged until the draw has run).  Rows
+ * pick[lo, hi) are written to src / path / tgt / mask [hi - lo, max_contexts] and target [hi - lo] (device memory; may
+ * be NULL when lo == hi), then the holes the picks leave below n - b are filled with the tail rows that were not
+ * picked, both in ascending order.  A rank of a multi-GPU run passes its slice [lo, hi) of the global batch and draws
+ * the whole pick, so every rank's pool stays the same.  Asynchronous on `stream`. */
+int c2v_reader_draw(c2v_reader* r, const int64_t* pick, int32_t b, int32_t lo, int32_t hi, int32_t* src, int32_t* path,
+                    int32_t* tgt, float* mask, int32_t* target, void* stream);
+
+/* Rows in the pool once the queued calls have run (-1 for a NULL handle); device memory the handle holds. */
+int64_t c2v_reader_live_rows(const c2v_reader* r);
+size_t c2v_reader_device_bytes(const c2v_reader* r);
+
 #ifdef __cplusplus
 }
 #endif
