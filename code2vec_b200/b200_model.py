@@ -32,7 +32,8 @@ from .path_context_reader import EstimatorAction, ModelInputTensorsFormer, PathC
 from .multi_rank import (CKPT_MAGIC, CKPT_SUFFIX, batch_split, check_checkpoint_dims, check_multi_rank_run,
                          checkpoint_header, create_checkpoint_file, read_checkpoint_header, read_checkpoint_part, run_world,
                          write_checkpoint, write_checkpoint_part)
-from .device_reader import device_reader_flag
+from . import device_reader as _device_reader_mod
+from .device_reader import device_reader_flag, sharded_reader_flag
 from .trainer import Trainer, make_fully_sharded_engine
 from .vocabularies import VocabType
 
@@ -143,6 +144,11 @@ class Code2VecModel(Code2VecModelBase):
         check_multi_rank_run(config, self.world)
         # C2V_DEVICE_READER=1: train() reads its batches on the GPU (device_reader.py, DESIGN.md §6d)
         self._device_reader = device_reader_flag(os.environ)
+        # C2V_SHARDED_READER=1: on several GPUs each rank reads and parses 1/W of every chunk (DESIGN.md §6d)
+        self._sharded_reader = sharded_reader_flag(os.environ)
+        self._reader_transport = None
+        if self._sharded_reader and not self._device_reader:
+            raise ValueError("C2V_SHARDED_READER=1 shards the device reader: it needs C2V_DEVICE_READER=1")
         if self._device_reader and config.DL_FRAMEWORK == "b200-keras":
             raise ValueError("C2V_DEVICE_READER=1 is not available with --framework b200-keras: its training loop reads "
                              "batches on the host; unset C2V_DEVICE_READER or train with --framework b200")
@@ -276,6 +282,9 @@ class Code2VecModel(Code2VecModelBase):
                 _barrier()                               # no peer reads this rank's shards any more
             self.engine.close()
             self.engine = None
+        if self._reader_transport is not None:
+            self._reader_transport.destroy()
+            self._reader_transport = None
         if self._own_group:
             import torch.distributed as dist
             dist.destroy_process_group()
@@ -414,7 +423,17 @@ class Code2VecModel(Code2VecModelBase):
             # C2V_DEVICE_READER=1: batches are parsed and drawn on the GPU into device slots (device_reader.py); the steps
             # read them there (step_device) and the losses collect in the pinned history, as on the ring path
             from .device_reader import DeviceBatchReader
-            dev_reader = DeviceBatchReader(train_reader, self.engine.dev, world=self.world, rank=self.rank)
+            if self._sharded_reader and multi:
+                # C2V_SHARDED_READER=1: each rank reads 1/W of every chunk; the ranks meet once per chunk on a gloo group
+                # of the reader's own (device_reader.make_share_transport), closed in close_session()
+                if self._reader_transport is None:
+                    self._reader_transport = _device_reader_mod.make_share_transport(self.engine.dev.index or 0)
+                self.log("Training reader sharded across %d ranks: each reads and parses 1/%d of every chunk" % (
+                    self.world, self.world))
+            elif self._sharded_reader:
+                self.log("C2V_SHARDED_READER=1 has no effect on one GPU: the device reader reads the whole file")
+            dev_reader = DeviceBatchReader(train_reader, self.engine.dev, world=self.world, rank=self.rank,
+                                           transport=self._reader_transport if multi else None)
         elif not multi and os.environ.get("C2V_BATCH_RING", "1") != "0" and not self._hint_next and train_reader._native_ready():
             import torch
             from .batch_ring import PinnedBatchRing
@@ -521,8 +540,9 @@ class Code2VecModel(Code2VecModelBase):
                 for v in loss_hist[:n_hist].tolist():
                     sum_loss += v
             self.h2d_bytes = dev_reader.h2d_bytes
-            self.log("Device reader: %.1f MB of text and draw indices uploaded, %.1f MB of device memory held" % (
-                dev_reader.h2d_bytes / 1e6, dev_reader.device_bytes() / 1e6))
+            peers = "" if dev_reader.transport is None else ", %.1f MB of rows read from peers" % (dev_reader.peer_bytes / 1e6)
+            self.log("Device reader: %.1f MB of text and draw indices uploaded, %.1f MB of device memory held%s" % (
+                dev_reader.h2d_bytes / 1e6, dev_reader.device_bytes() / 1e6, peers))
             dev_reader.close()
         if multi:
             self.log("%d training rows left out: a short batch trains on a multiple of the %d ranks" % (

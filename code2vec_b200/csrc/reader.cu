@@ -11,6 +11,9 @@
 //                beyond it, j-th hole from j-th mover (not a stable compaction: the host pool's order)
 //   draw       : the picked rows (the host's random draw) are gathered into a batch buffer, then the holes they leave
 //                below the new end are filled with the surviving tail rows, both in ascending order
+// A chunk read sharded across ranks (DESIGN.md §6d) runs the line index and the parse over one rank's share of the chunk
+// into a peer-visible stage; every rank then copies all stages behind its pool's live end in rank order (assemble) and
+// commits the whole chunk's records as above, so its pool is the one a whole-chunk parse builds.
 #include <cuda_runtime.h>
 #include <stdint.h>
 #include <string.h>
@@ -378,6 +381,75 @@ gather_kernel(PoolRows pool, int C, const long long* __restrict__ pick, int lo, 
   }
 }
 
+// ---- sharded chunks --------------------------------------------------------------------------------------------------
+// A stage of `rows` rows: the share's status (c2v_reader_share_status, its `rows` field included) in the first 256 bytes,
+// then src, path, dst, mask [rows, C], target [rows] and keep [rows], each at a 256-byte boundary.
+constexpr long long kStageHeader = 256;
+constexpr int kMaxShares = 64;
+
+struct StageLayout { long long src, path, dst, mask, target, keep, bytes; };
+
+__host__ __device__ __forceinline__ long long align256(long long x) { return (x + 255) & ~255ll; }
+
+__host__ __device__ __forceinline__ StageLayout stage_layout(int C, long long rows) {
+  const long long m = align256(rows * C * 4);
+  StageLayout L;
+  L.src = kStageHeader;
+  L.path = L.src + m;
+  L.dst = L.path + m;
+  L.mask = L.dst + m;
+  L.target = L.mask + m;
+  L.keep = L.target + align256(rows * 4);
+  L.bytes = L.keep + align256(rows);
+  return L;
+}
+
+struct ShareSrc {
+  const unsigned char* stage;     // this rank's stage or a peer's, opened through CUDA IPC
+  long long row0, records;        // first row of the share in the chunk, its records
+};
+
+struct AssembleArgs {
+  ShareSrc share[kMaxShares];
+  int n, C;
+  PoolRows pool;
+  long long live;                 // the pool's live end: the chunk's row 0
+  uint8_t* keep;                  // per record of the chunk
+  int* n_rec;                     // <- the chunk's records
+  long long total;
+};
+
+// pool rows [live + row0, live + row0 + records) and keep[row0, row0 + records) <- stage blockIdx.y's rows and keep flags
+__global__ void __launch_bounds__(256) assemble_shares_kernel(const __grid_constant__ AssembleArgs a) {
+  __shared__ long long rows;
+  const ShareSrc sh = a.share[blockIdx.y];
+  if (blockIdx.x == 0 && blockIdx.y == 0 && threadIdx.x == 0) *a.n_rec = (int)a.total;
+  if (sh.records == 0) return;
+  if (threadIdx.x == 0) rows = ((const c2v_reader_share_status*)sh.stage)->rows;
+  __syncthreads();
+  const StageLayout L = stage_layout(a.C, rows);
+  const int32_t* src = (const int32_t*)(sh.stage + L.src);
+  const int32_t* path = (const int32_t*)(sh.stage + L.path);
+  const int32_t* dst = (const int32_t*)(sh.stage + L.dst);
+  const float* mask = (const float*)(sh.stage + L.mask);
+  const int32_t* target = (const int32_t*)(sh.stage + L.target);
+  const uint8_t* keep = sh.stage + L.keep;
+  const long long n = sh.records * a.C, d0 = (a.live + sh.row0) * a.C;
+  const long long stride = (long long)gridDim.x * 256;
+  for (long long i = (long long)blockIdx.x * 256 + threadIdx.x; i < n; i += stride) {
+    const int32_t s = src[i], q = path[i], t = dst[i];
+    const float m = mask[i];
+    a.pool.src[d0 + i] = s;
+    a.pool.path[d0 + i] = q;
+    a.pool.dst[d0 + i] = t;
+    a.pool.mask[d0 + i] = m;
+  }
+  for (long long i = (long long)blockIdx.x * 256 + threadIdx.x; i < sh.records; i += stride) {
+    a.pool.target[a.live + sh.row0 + i] = target[i];
+    a.keep[sh.row0 + i] = keep[i];
+  }
+}
+
 }  // namespace
 
 struct c2v_reader {
@@ -397,7 +469,8 @@ struct c2v_reader {
   uint8_t* tail = nullptr;                                                                  // [picks]
   unsigned long long* bad = nullptr;
   int* n_moves = nullptr;
-  struct Status { int records, kept; unsigned long long bad; long long line; } *host = nullptr;   // pinned read-back
+  int* n_rec = nullptr;                                                                     // records of assembled shares
+  struct Status { int records, kept, newlines; unsigned long long bad; long long line; } *host = nullptr;   // pinned read-back
   size_t bytes = 0;               // device memory held
 };
 
@@ -491,6 +564,41 @@ DevVocab dev_vocab(const c2v_reader_vocab& v) {
 
 size_t parse_smem(int C) { return (size_t)kParseWarps * 3 * C * sizeof(longlong2); }
 
+// line index and parse of text[0, nbytes) (nbytes > 0, `tiles` tiles of it, scratch reserved for `cap` records): the
+// first `cap` records land in rows[0, cap) and keep[0, cap), the lowest malformed one in r->bad
+int index_and_parse(c2v_reader* r, const unsigned char* t, long long nbytes, int tiles, long long cap, PoolRows rows,
+                    uint8_t* keep, cudaStream_t st) {
+  RD_CUDA(cudaMemsetAsync(r->bad, 0xff, sizeof(unsigned long long), st));
+  line_count_kernel<<<tiles, kTileThreads, 0, st>>>(t, nbytes, r->rec_cnt, r->nl_cnt);
+  exclusive_scan_kernel<<<1, 1024, 0, st>>>(r->rec_cnt, r->rec_base, tiles);
+  exclusive_scan_kernel<<<1, 1024, 0, st>>>(r->nl_cnt, r->nl_base, tiles);
+  line_index_kernel<<<tiles, kTileThreads, 0, st>>>(t, nbytes, r->rec_base, r->nl_base, cap, r->rec_off, r->rec_line);
+  ParseArgs a{t, nbytes, r->C, r->tok, r->pth, r->tgt, r->rec_off, r->rec_base + tiles, cap,
+              rows.src, rows.path, rows.dst, rows.target, rows.mask, keep, r->bad};
+  long long grid = (cap + kParseWarps - 1) / kParseWarps;
+  if (grid > (long long)r->num_sms * 16) grid = (long long)r->num_sms * 16;
+  parse_kernel<<<(unsigned)grid, 32 * kParseWarps, parse_smem(r->C), st>>>(a);
+  RD_CUDA(cudaGetLastError());
+  return C2V_OK;
+}
+
+// keep_count + scan + commit_index + move_rows over the `cap`-bounded records (*n_rec) just behind the live end, then
+// reads the kept count back (synchronises st) and advances the live end.  The records' keep flags are in r->keep.
+int commit_records(c2v_reader* r, const int* n_rec, long long cap, int64_t* kept, cudaStream_t st) {
+  const int row_tiles = (int)((cap + kRowTile - 1) / kRowTile);
+  keep_count_kernel<<<row_tiles, 256, 0, st>>>(r->keep, n_rec, cap, r->keep_cnt);
+  exclusive_scan_kernel<<<1, 1024, 0, st>>>(r->keep_cnt, r->keep_base, row_tiles);
+  commit_index_kernel<<<row_tiles, 256, 0, st>>>(r->keep, n_rec, cap, r->keep_base, row_tiles, r->holes, r->movers,
+                                                 r->n_moves);
+  move_rows_kernel<<<r->num_sms * 8, 256, 0, st>>>(r->pool, r->C, r->live, r->holes, r->movers, r->n_moves);
+  RD_CUDA(cudaGetLastError());
+  RD_CUDA(cudaMemcpyAsync(&r->host->kept, r->keep_base + row_tiles, sizeof(int), cudaMemcpyDeviceToHost, st));
+  RD_CUDA(cudaStreamSynchronize(st));
+  *kept = r->host->kept;
+  r->live += r->host->kept;
+  return C2V_OK;
+}
+
 }  // namespace
 
 extern "C" {
@@ -518,12 +626,13 @@ int c2v_reader_create(int32_t max_contexts, const c2v_reader_vocab* tok, const c
   r->tgt = dev_vocab(*target);
   cudaError_t e = cudaMalloc(&r->bad, sizeof(unsigned long long));
   if (e == cudaSuccess) e = cudaMalloc(&r->n_moves, sizeof(int));
+  if (e == cudaSuccess) e = cudaMalloc(&r->n_rec, sizeof(int));
   if (e == cudaSuccess) e = cudaHostAlloc((void**)&r->host, sizeof(c2v_reader::Status), cudaHostAllocDefault);
   if (e != cudaSuccess) {
     c2v_reader_destroy(r);
     return rfail(C2V_ERR_CUDA, std::string("c2v_reader_create: ") + cudaGetErrorString(e));
   }
-  r->bytes = sizeof(unsigned long long) + sizeof(int);
+  r->bytes = sizeof(unsigned long long) + 2 * sizeof(int);
   *out = r;
   return C2V_OK;
 }
@@ -535,7 +644,7 @@ void c2v_reader_destroy(c2v_reader* r) {
   for (void* p : {(void*)r->pool.src, (void*)r->pool.path, (void*)r->pool.dst, (void*)r->pool.mask, (void*)r->pool.target,
                   (void*)r->rec_cnt, (void*)r->nl_cnt, (void*)r->rec_base, (void*)r->nl_base, (void*)r->rec_off,
                   (void*)r->rec_line, (void*)r->keep, (void*)r->keep_cnt, (void*)r->keep_base, (void*)r->holes,
-                  (void*)r->movers, (void*)r->pick, (void*)r->tail, (void*)r->bad, (void*)r->n_moves})
+                  (void*)r->movers, (void*)r->pick, (void*)r->tail, (void*)r->bad, (void*)r->n_moves, (void*)r->n_rec})
     if (p) cudaFree(p);
   if (r->host) cudaFreeHost(r->host);
   delete r;
@@ -554,18 +663,9 @@ int c2v_reader_parse_chunk(c2v_reader* r, const char* text, int64_t nbytes, int6
   if ((rc = reserve_scratch(r, nbytes, cap, 0, st)) || (rc = reserve_pool(r, cap, st))) return rc;
   const int tiles = (int)((nbytes + kTile - 1) / kTile), row_tiles = (int)((cap + kRowTile - 1) / kRowTile);
   const unsigned char* t = (const unsigned char*)text;
-  RD_CUDA(cudaMemsetAsync(r->bad, 0xff, sizeof(unsigned long long), st));
-  if (tiles) line_count_kernel<<<tiles, kTileThreads, 0, st>>>(t, nbytes, r->rec_cnt, r->nl_cnt);
-  exclusive_scan_kernel<<<1, 1024, 0, st>>>(r->rec_cnt, r->rec_base, tiles);
-  exclusive_scan_kernel<<<1, 1024, 0, st>>>(r->nl_cnt, r->nl_base, tiles);
-  if (tiles) line_index_kernel<<<tiles, kTileThreads, 0, st>>>(t, nbytes, r->rec_base, r->nl_base, cap, r->rec_off, r->rec_line);
   const long long l0 = r->live * r->C;
-  ParseArgs a{t, nbytes, r->C, r->tok, r->pth, r->tgt, r->rec_off, r->rec_base + tiles, cap,
-              r->pool.src + l0, r->pool.path + l0, r->pool.dst + l0, r->pool.target + r->live, r->pool.mask + l0,
-              r->keep, r->bad};
-  long long grid = (cap + kParseWarps - 1) / kParseWarps;
-  if (grid > (long long)r->num_sms * 16) grid = (long long)r->num_sms * 16;
-  parse_kernel<<<(unsigned)grid, 32 * kParseWarps, parse_smem(r->C), st>>>(a);
+  const PoolRows tail{r->pool.src + l0, r->pool.path + l0, r->pool.dst + l0, r->pool.target + r->live, r->pool.mask + l0};
+  if ((rc = index_and_parse(r, t, nbytes, tiles, cap, tail, r->keep, st))) return rc;
   keep_count_kernel<<<row_tiles, 256, 0, st>>>(r->keep, r->rec_base + tiles, cap, r->keep_cnt);
   exclusive_scan_kernel<<<1, 1024, 0, st>>>(r->keep_cnt, r->keep_base, row_tiles);
   commit_index_kernel<<<row_tiles, 256, 0, st>>>(r->keep, r->rec_base + tiles, cap, r->keep_base, row_tiles, r->holes,
@@ -616,6 +716,109 @@ int c2v_reader_draw(c2v_reader* r, const int64_t* pick, int32_t b, int32_t lo, i
   RD_CUDA(cudaGetLastError());
   r->live -= b;
   return C2V_OK;
+}
+
+size_t c2v_reader_stage_bytes(int32_t max_contexts, int64_t rows) {
+  if (max_contexts < 1 || rows < 1) return 0;
+  return (size_t)stage_layout(max_contexts, rows).bytes;
+}
+
+int c2v_reader_parse_share(c2v_reader* r, const char* text, int64_t nbytes, int64_t chunk_bytes, void* stage,
+                           int64_t stage_rows, c2v_reader_share_status* status, void* stream) {
+  if (!r || !stage || !status || (nbytes > 0 && !text))
+    return rfail(C2V_ERR_INVALID, "c2v_reader_parse_share: NULL argument");
+  if (nbytes < 0 || chunk_bytes < nbytes || stage_rows < 1)
+    return rfail(C2V_ERR_INVALID, "c2v_reader_parse_share: need 0 <= nbytes <= chunk_bytes and stage_rows >= 1");
+  RD_CUDA(cudaSetDevice(r->device));
+  cudaStream_t st = (cudaStream_t)stream;
+  c2v_reader_share_status s{};
+  s.rows = stage_rows;
+  s.bad_line = -1;
+  if (nbytes > 0) {
+    const unsigned char* t = (const unsigned char*)text;
+    unsigned char* g = (unsigned char*)stage;
+    const StageLayout L = stage_layout(r->C, stage_rows);
+    const PoolRows rows{(int32_t*)(g + L.src), (int32_t*)(g + L.path), (int32_t*)(g + L.dst), (int32_t*)(g + L.target),
+                        (float*)(g + L.mask)};
+    const int tiles = (int)((nbytes + kTile - 1) / kTile), row_tiles = (int)((stage_rows + kRowTile - 1) / kRowTile);
+    int rc;
+    if ((rc = reserve_scratch(r, nbytes, stage_rows, 0, st))) return rc;
+    if ((rc = index_and_parse(r, t, nbytes, tiles, stage_rows, rows, g + L.keep, st))) return rc;
+    keep_count_kernel<<<row_tiles, 256, 0, st>>>(g + L.keep, r->rec_base + tiles, stage_rows, r->keep_cnt);
+    exclusive_scan_kernel<<<1, 1024, 0, st>>>(r->keep_cnt, r->keep_base, row_tiles);
+    RD_CUDA(cudaGetLastError());
+    RD_CUDA(cudaMemcpyAsync(&r->host->records, r->rec_base + tiles, sizeof(int), cudaMemcpyDeviceToHost, st));
+    RD_CUDA(cudaMemcpyAsync(&r->host->newlines, r->nl_base + tiles, sizeof(int), cudaMemcpyDeviceToHost, st));
+    RD_CUDA(cudaMemcpyAsync(&r->host->kept, r->keep_base + row_tiles, sizeof(int), cudaMemcpyDeviceToHost, st));
+    RD_CUDA(cudaMemcpyAsync(&r->host->bad, r->bad, sizeof(unsigned long long), cudaMemcpyDeviceToHost, st));
+    RD_CUDA(cudaStreamSynchronize(st));
+    s.records = r->host->records;
+    s.newlines = r->host->newlines;
+    if (s.records > stage_rows) {
+      // more records than the share holds well-formed lines: one of them is malformed.  The first pass's last record ran
+      // to the end of the text, so its verdict is void; the lowest malformed line is found in a second pass over every
+      // record, in the pool's room behind its live end.  With more records than the whole chunk holds well-formed lines
+      // the chunk fails with kind 3 whatever the lines are, and no pass is needed.
+      s.overflow = 1;
+      r->host->bad = ~0ull;
+      const long long chunk_cap = chunk_bytes / (r->C + 1) + 1;
+      if (s.records <= chunk_cap) {
+        if ((rc = reserve_scratch(r, nbytes, s.records, 0, st)) || (rc = reserve_pool(r, s.records, st))) return rc;
+        const long long l0 = r->live * r->C;
+        const PoolRows tail{r->pool.src + l0, r->pool.path + l0, r->pool.dst + l0, r->pool.target + r->live,
+                            r->pool.mask + l0};
+        if ((rc = index_and_parse(r, t, nbytes, tiles, s.records, tail, r->keep, st))) return rc;
+        RD_CUDA(cudaMemcpyAsync(&r->host->bad, r->bad, sizeof(unsigned long long), cudaMemcpyDeviceToHost, st));
+        RD_CUDA(cudaStreamSynchronize(st));
+      }
+    }
+    if (r->host->bad != ~0ull) {
+      const long long li = (long long)(r->host->bad >> 2);
+      RD_CUDA(cudaMemcpyAsync(&r->host->line, r->rec_line + li, sizeof(long long), cudaMemcpyDeviceToHost, st));
+      RD_CUDA(cudaStreamSynchronize(st));
+      s.bad_line = r->host->line;
+      s.bad_kind = (int32_t)(r->host->bad & 3);
+    } else if (!s.overflow) {
+      s.kept = r->host->kept;
+    }
+  }
+  RD_CUDA(cudaMemcpyAsync(stage, &s, sizeof(s), cudaMemcpyHostToDevice, st));
+  RD_CUDA(cudaStreamSynchronize(st));
+  *status = s;
+  return C2V_OK;
+}
+
+int c2v_reader_commit_shares(c2v_reader* r, const void* const* stages, const int64_t* records, int32_t n_shares,
+                             int64_t* kept, void* stream) {
+  if (!r || !stages || !records || !kept) return rfail(C2V_ERR_INVALID, "c2v_reader_commit_shares: NULL argument");
+  if (n_shares < 1 || n_shares > kMaxShares)
+    return rfail(C2V_ERR_INVALID, "c2v_reader_commit_shares: n_shares must be in [1, " + std::to_string(kMaxShares) + "]");
+  *kept = 0;
+  AssembleArgs a{};
+  long long total = 0;
+  for (int i = 0; i < n_shares; ++i) {
+    if (records[i] < 0 || (records[i] > 0 && !stages[i]))
+      return rfail(C2V_ERR_INVALID, "c2v_reader_commit_shares: a share with records needs its stage");
+    a.share[i] = ShareSrc{(const unsigned char*)stages[i], total, (long long)records[i]};
+    total += records[i];
+  }
+  if (total == 0) return C2V_OK;
+  if (total > INT32_MAX) return rfail(C2V_ERR_INVALID, "c2v_reader_commit_shares: more than 2^31 - 1 records");
+  RD_CUDA(cudaSetDevice(r->device));
+  cudaStream_t st = (cudaStream_t)stream;
+  int rc;
+  if ((rc = reserve_scratch(r, 0, total, 0, st)) || (rc = reserve_pool(r, total, st))) return rc;
+  a.n = n_shares;
+  a.C = r->C;
+  a.pool = r->pool;
+  a.live = r->live;
+  a.keep = r->keep;
+  a.n_rec = r->n_rec;
+  a.total = total;
+  const int per = (r->num_sms * 4 + n_shares - 1) / n_shares;
+  assemble_shares_kernel<<<dim3((unsigned)per, (unsigned)n_shares), 256, 0, st>>>(a);
+  RD_CUDA(cudaGetLastError());
+  return commit_records(r, r->n_rec, total, kept, st);
 }
 
 int64_t c2v_reader_live_rows(const c2v_reader* r) { return r ? r->live : -1; }

@@ -8,19 +8,29 @@ yields in train mode for the same config and shuffle seed:
   * the host draws every batch's row indices with the reader's np.random.Generator exactly as _RowPool.take does, and the
     pool on the device is committed and drawn from in the host pool's order, so the same indices pick the same rows.
 The host's work per chunk is a file read, one copy into a page-locked buffer and its upload; per batch, the draw of the
-indices (8 bytes a row).  Code2VecModel.train() uses it when C2V_DEVICE_READER=1."""
+indices (8 bytes a row).  Code2VecModel.train() uses it when C2V_DEVICE_READER=1.
+
+Sharded (C2V_SHARDED_READER=1 on W > 1 ranks, a ShareTransport given): the ranks cut every chunk into W shares of whole
+lines (path_context_reader.share_range); each rank reads, uploads and parses only its own share into a stage of its
+device memory (c2v_reader_parse_share), the ranks gather their share statuses once per chunk, and every rank assembles
+all W stages, its peers' read through CUDA IPC, into its pool (c2v_reader_commit_shares).  Chunk bounds, pool, kept
+counts and draws stay exactly those of the unsharded reader, so the batches do too."""
 from __future__ import annotations
 
 import ctypes as C
+import datetime
 import queue
 import threading
 from typing import Optional
 
 import numpy as np
 
-from .engine import EngineError, c2v_reader_vocab, load_library
+from .engine import EngineError, c2v_reader_share_status, c2v_reader_vocab, load_library
 from .multi_rank import batch_split
-from .path_context_reader import _INT64_MIN, PathContextReader, _raise_parse_error
+from .path_context_reader import _INT64_MIN, PathContextReader, _raise_parse_error, pread_into, share_range
+
+# how long a rank waits in a chunk's exchange for its peers (they may be evaluating, or saving a checkpoint)
+EXCHANGE_TIMEOUT = datetime.timedelta(minutes=30)
 
 
 def device_reader_flag(environ) -> bool:
@@ -29,6 +39,92 @@ def device_reader_flag(environ) -> bool:
     if flag not in ("0", "1"):
         raise ValueError("C2V_DEVICE_READER must be 0 or 1, got %r" % flag)
     return flag == "1"
+
+
+def sharded_reader_flag(environ) -> bool:
+    """C2V_SHARDED_READER=1 (with C2V_DEVICE_READER=1): on several GPUs each rank reads and parses 1/W of every chunk and
+    takes the other rows from its peers; 0 (the default): every rank reads the whole file."""
+    flag = environ.get("C2V_SHARDED_READER", "0") or "0"
+    if flag not in ("0", "1"):
+        raise ValueError("C2V_SHARDED_READER must be 0 or 1, got %r" % flag)
+    return flag == "1"
+
+
+def chunk_error(statuses, chunk_bytes: int, max_contexts: int):
+    """The error of a chunk parsed as shares, from the shares' statuses in rank order (objects with records, newlines,
+    bad_line, bad_kind, overflow): None for a clean chunk, (None, 3) when the chunk has more records than
+    chunk_bytes / (max_contexts + 1) + 1, else (line, kind) of its lowest malformed line -- what a whole-chunk parse
+    reports."""
+    cap = chunk_bytes // (max_contexts + 1) + 1
+    if sum(s.records for s in statuses) > cap:
+        return None, 3
+    base = 0
+    for s in statuses:
+        if s.bad_kind:
+            return base + s.bad_line, s.bad_kind
+        if s.overflow:
+            raise RuntimeError("a share overflowed its stage but reported no malformed line")
+        base += s.newlines
+    return None
+
+
+def raise_chunk_error(err, max_contexts: int):
+    """chunk_error's verdict as the ValueError the host reader raises for the same chunk."""
+    line, kind = err
+    if kind == 3:
+        _raise_parse_error(_INT64_MIN, 0, max_contexts)
+    _raise_parse_error(-(line + 1), kind, max_contexts)
+
+
+class ShareTransport:
+    """How the ranks of a sharded device reader meet: `gather` is an all-gather of one small object per rank on a gloo
+    group of the reader's own (the reader thread never issues a collective on the training group, whose NCCL
+    collectives the training thread issues at the same time), and stages are CUDA-IPC allocations that peers open by
+    handle.  Tests replace it (make_share_transport) to run ranks as threads of one process."""
+
+    def __init__(self, lib, device: int, group, world: int, rank: int):
+        self.lib, self.device, self.group, self.world, self.rank = lib, int(device), group, int(world), int(rank)
+
+    def _check(self, rc):
+        if rc != 0:
+            raise EngineError(rc, self.lib.c2v_last_error(None).decode())
+
+    def alloc(self, nbytes: int):
+        """(device pointer, handle bytes) of a new peer-visible allocation on this rank's device."""
+        ptr, hbuf = C.c_void_p(), C.create_string_buffer(64)
+        self._check(self.lib.c2v_ipc_alloc(self.device, nbytes, C.byref(ptr), hbuf))
+        return ptr.value, hbuf.raw
+
+    def free(self, ptr: int):
+        self._check(self.lib.c2v_ipc_free(self.device, ptr))
+
+    def open(self, handle: bytes) -> int:
+        ptr = C.c_void_p()
+        self._check(self.lib.c2v_ipc_open(self.device, handle, C.byref(ptr)))
+        return ptr.value
+
+    def close(self, ptr: int):
+        self._check(self.lib.c2v_ipc_close(self.device, ptr))
+
+    def gather(self, obj) -> list:
+        import torch.distributed as dist
+        out = [None] * self.world
+        dist.all_gather_object(out, obj, group=self.group)
+        return out
+
+    def destroy(self):
+        import torch.distributed as dist
+        if self.group is not None:
+            dist.destroy_process_group(self.group)
+            self.group = None
+
+
+def make_share_transport(device: int) -> ShareTransport:
+    """The transport of a sharded reader on this rank of the default process group (every rank calls it, in the same
+    order as its other new_group calls)."""
+    import torch.distributed as dist
+    group = dist.new_group(backend="gloo", timeout=EXCHANGE_TIMEOUT)
+    return ShareTransport(load_library(), device, group, dist.get_world_size(), dist.get_rank())
 
 
 def export_vocab(lib, handle):
@@ -78,7 +174,9 @@ class DeviceBatchReader:
     iterating (training) thread never waits for the GPU.  Needs libc2v_batcher.so (RuntimeError otherwise, as
     use_native=True does)."""
 
-    def __init__(self, reader: PathContextReader, device, world: int = 1, rank: int = 0, slots: int = 4):
+    def __init__(self, reader: PathContextReader, device, world: int = 1, rank: int = 0, slots: int = 4,
+                 transport: Optional[ShareTransport] = None):
+        """transport: read the chunks sharded across the `world` ranks, meeting through it (ignored on one rank)."""
         import torch
         if not reader.estimator_action.is_train:
             raise ValueError("the device reader reads training files only")
@@ -106,6 +204,7 @@ class DeviceBatchReader:
                 self._vocab_tensors += [d_slots, d_bytes]
                 structs.append(c2v_reader_vocab(d_slots.data_ptr(), d_bytes.data_ptr(), mask, oov, pad))
             torch.cuda.synchronize(self.dev)
+            self._structs = structs
             h = C.c_void_p()
             rc = self.lib.c2v_reader_create(self.C, C.byref(structs[0]), C.byref(structs[1]), C.byref(structs[2]),
                                             self.dev.index or 0, C.byref(h))
@@ -130,6 +229,16 @@ class DeviceBatchReader:
         self._text = [None, None]
         self._thread: Optional[threading.Thread] = None
         self._stop = threading.Event()
+        # sharded: this rank's two stages (chunk k uses stage k % 2), the peers' stages opened by handle, and replaced
+        # stages waiting until no peer has them open
+        self.transport = transport if self.world > 1 else None
+        self._stages = [None, None]
+        self._peers = {}                       # (rank, stage) -> opened pointer
+        self._retired = []                     # (pointer, exchanges after which it is freed)
+        self._exchanges = 0
+        self._peers_know = False               # the peers know this rank is done with the pass's exchanges
+        self.peer_bytes = 0                    # bytes of rows this rank's assemblies read from its peers' stages
+        self._row_bytes = (4 * self.C + 1) * 4 + 1
 
     # ---- reader thread ---------------------------------------------------------------------------------------------
     def _text_buffers(self, i: int, n: int):
@@ -166,6 +275,114 @@ class DeviceBatchReader:
             if bad_kind.value in (1, 2):
                 _raise_parse_error(-(bad_line.value + 1), bad_kind.value, self.C)
             raise EngineError(rc, self.lib.c2v_last_error(None).decode())
+        return int(kept.value)
+
+    # ---- sharded chunks ----------------------------------------------------------------------------------------------
+    def _stage(self, j: int, rows: int):
+        """This rank's stage j with room for `rows` rows, and its handle if it is new (None otherwise)."""
+        s = self._stages[j]
+        if s is not None and s["rows"] >= rows:
+            return s, None
+        if s is not None:
+            # the peers close the old stage when the new handle reaches them in the coming exchange, before they enter
+            # the one after it: once that one is over, nobody has it open
+            self._retired.append((s["ptr"], self._exchanges + 2))
+            rows = max(rows, s["rows"] * 5 // 4)
+        nbytes = int(self.lib.c2v_reader_stage_bytes(self.C, rows))
+        ptr, handle = self.transport.alloc(nbytes)
+        # c2v_ipc_alloc zero-fills the new stage with a cudaMemset on the legacy default stream, which returns before the
+        # fill has run and which the reader stream (non-blocking) is not ordered after.  The parse that writes the stage
+        # must not run before the fill, or the fill, queued behind the training steps on that stream, could land later
+        # and zero rows, keep flags and the status header that the owner and its peers then read at different times.
+        filled = self.torch.cuda.Event()
+        filled.record(self.torch.cuda.default_stream(self.dev))
+        self.stream.wait_event(filled)
+        self._stages[j] = s = {"ptr": ptr, "rows": rows, "bytes": nbytes}
+        return s, handle
+
+    def _exchange(self, msg) -> list:
+        got = self.transport.gather(msg)
+        self._exchanges += 1
+        for ptr, due in [x for x in self._retired if x[1] <= self._exchanges]:
+            self.transport.free(ptr)
+            self._retired.remove((ptr, due))
+        return got
+
+    def _raise_if_a_peer_failed(self, got):
+        """Raises when a message of an exchange (status, handle, error) carries a rank's error: every rank raises."""
+        failed = [(r, m[2]) for r, m in enumerate(got) if m is not None and m[2]]
+        if failed:
+            self._peers_know = True
+            raise RuntimeError("rank %d of the sharded device reader failed: %s" % failed[0])
+
+    def _leave(self, why: str):
+        """This rank stops reading before the pass is over (an error after an exchange, or its consumer stopped): its
+        peers learn it in the exchange they enter next, and raise, instead of waiting for it there.  Nothing to do when
+        the peers know already (the error came out of an exchange, or the last exchange of the pass is behind)."""
+        if self.transport is None or self._peers_know:
+            return
+        self._peers_know = True
+        try:
+            self._exchange((None, None, why))
+        except Exception:                              # the peers may have gone too; the rank's own error stands
+            pass
+
+    def _parse_sharded(self, fd: int, a: int, b: int, k: int) -> int:
+        """Chunk k = [a, b) of file fd: this rank's share read, uploaded and parsed into stage k % 2, the shares' statuses
+        exchanged, then every stage assembled into the pool in rank order and committed.  Returns the rows kept."""
+        torch, j = self.torch, k % 2
+        status = handle = err = None
+        try:
+            s0, s1 = share_range(fd, a, b, self.world, self.rank)
+            n = s1 - s0
+            # Stage j last held chunk k - 2.  Every peer finished assembling that chunk (commit_shares synchronises)
+            # before it entered the exchange of chunk k - 1, which this rank has left, so no peer reads stage j now: it
+            # may be overwritten, grown or replaced.
+            stage, handle = self._stage(j, n // (self.C + 1) + 1)
+            text = 0
+            if n:
+                buf = self._text_buffers(j, n)
+                buf["uploaded"].synchronize()                   # the previous upload out of this host buffer has left
+                pread_into(fd, buf["np"][:n], s0)
+                with torch.cuda.stream(self.copy_stream):
+                    buf["dev"][:n].copy_(buf["host"][:n], non_blocking=True)
+                    buf["uploaded"].record(self.copy_stream)
+                self.stream.wait_event(buf["uploaded"])
+                self.h2d_bytes += n
+                text = buf["dev"].data_ptr()
+            st = c2v_reader_share_status()
+            rc = self.lib.c2v_reader_parse_share(self.h, text, n, b - a, stage["ptr"], stage["rows"], C.byref(st),
+                                                 self.stream.cuda_stream)          # synchronises: the stage is complete
+            if rc != 0:
+                raise EngineError(rc, self.lib.c2v_last_error(None).decode())
+            status = tuple(getattr(st, f) for f, _ in st._fields_)
+        except Exception as exc:
+            err = exc
+        # every rank enters the exchange, a failed one too, so that none waits for a rank that has gone
+        got = self._exchange((status, handle, None if err is None else "%s: %s" % (type(err).__name__, err)))
+        if err is not None:
+            self._peers_know = True
+            raise err
+        self._raise_if_a_peer_failed(got)
+        statuses = [c2v_reader_share_status(*m[0]) for m in got]
+        bad = chunk_error(statuses, b - a, self.C)
+        if bad is not None:
+            self._peers_know = True                    # every rank decides the same error from the same statuses
+            raise_chunk_error(bad, self.C)
+        for r, m in enumerate(got):
+            if r != self.rank and m[1] is not None:
+                old = self._peers.pop((r, j), None)
+                if old is not None:
+                    self.transport.close(old)
+                self._peers[(r, j)] = self.transport.open(m[1])
+        W = self.world
+        ptrs = (C.c_void_p * W)(*[self._stages[j]["ptr"] if r == self.rank else self._peers[(r, j)] for r in range(W)])
+        recs = (C.c_int64 * W)(*[s.records for s in statuses])
+        kept = C.c_int64()
+        rc = self.lib.c2v_reader_commit_shares(self.h, ptrs, recs, W, C.byref(kept), self.stream.cuda_stream)
+        if rc != 0:
+            raise EngineError(rc, self.lib.c2v_last_error(None).decode())
+        self.peer_bytes += sum(s.records for r, s in enumerate(statuses) if r != self.rank) * self._row_bytes
         return int(kept.value)
 
     def _acquire(self, k: int):
@@ -208,17 +425,28 @@ class DeviceBatchReader:
         try:
             with self.torch.cuda.device(self.dev):
                 n, k = 0, 0
-                chunks = self.reader._native_chunks_ahead()
+                if self.transport is not None:
+                    chunks = self.reader._native_chunk_ranges()
+                    parse = lambda chunk, i: self._parse_sharded(*chunk, i)
+                else:
+                    chunks = self.reader._native_chunks_ahead()
+                    parse = lambda chunk, i: self._parse(chunk, i % 2)
                 try:
                     for i, chunk in enumerate(chunks):
-                        n += self._parse(chunk, i % 2)
+                        n += parse(chunk, i)
                         while n >= self.S + self.B:
                             batch = self._draw(n, self.B, k)
                             if batch is None or not put(batch):
+                                self._leave("rank %d stopped reading: its consumer has gone" % self.rank)
                                 return
                             n, k = n - self.B, k + 1
                 finally:
                     chunks.close()
+                if self.transport is not None:
+                    # every rank has assembled the last chunk: no stage is read any more
+                    got = self._exchange(None)
+                    self._peers_know = True
+                    self._raise_if_a_peer_failed(got)
                 while n > 0:
                     b = min(self.B, n)
                     batch = self._draw(n, b, k)
@@ -227,6 +455,7 @@ class DeviceBatchReader:
                     n, k = n - b, k + 1
             put(done)
         except BaseException as exc:
+            self._leave("rank %d failed: %s: %s" % (self.rank, type(exc).__name__, exc))
             put(exc)
 
     def __iter__(self):
@@ -249,19 +478,30 @@ class DeviceBatchReader:
 
     # ---- life cycle --------------------------------------------------------------------------------------------------
     def device_bytes(self) -> int:
-        """Device memory the reader holds: vocabularies, batch slots, chunk text and the handle's pool and scratch."""
+        """Device memory the reader holds: vocabularies, batch slots, chunk text, this rank's stages (sharded) and the
+        handle's pool and scratch."""
         n = sum(t.numel() * t.element_size() for t in self._vocab_tensors)
         n += sum(t.numel() * t.element_size() for s in self.slots for t in s["tensors"])
         n += sum(b["dev"].numel() for b in self._text if b is not None)
+        n += sum(s["bytes"] for s in self._stages if s is not None)
         return int(n + (self.lib.c2v_reader_device_bytes(self.h) if self.h else 0))
 
     def close(self):
+        """Stops the reader thread and frees what the reader holds.  A sharded reader's stages are freed here: after a
+        whole pass every peer is done with them; after a failed one the peers stopped at the same exchange."""
         self._stop.set()
         if self._thread is not None:
             self._thread.join()
         if getattr(self, "h", None):
             self.lib.c2v_reader_destroy(self.h)        # synchronises the device first
             self.h = None
+        if self.transport is not None:
+            for ptr in self._peers.values():
+                self.transport.close(ptr)
+            self._peers = {}
+            for ptr in [s["ptr"] for s in self._stages if s is not None] + [p for p, _ in self._retired]:
+                self.transport.free(ptr)
+            self._stages, self._retired = [None, None], []
 
     def __del__(self):
         try:

@@ -40,6 +40,11 @@ class c2v_reader_vocab(C.Structure):
     _fields_ = [("slots", C.c_void_p), ("bytes", C.c_void_p), ("mask", C.c_uint64), ("oov", C.c_int32), ("pad", C.c_int32)]
 
 
+class c2v_reader_share_status(C.Structure):
+    _fields_ = [("rows", C.c_int64), ("records", C.c_int64), ("kept", C.c_int64), ("newlines", C.c_int64),
+                ("bad_line", C.c_int64), ("bad_kind", C.c_int32), ("overflow", C.c_int32)]
+
+
 class _DeviceArray:
     """A raw device allocation presented through __cuda_array_interface__ so torch can view it."""
 
@@ -117,6 +122,10 @@ _SIGNATURES = {
     "c2v_reader_draw": (C.c_int, [_P, _P, _I32, _I32, _I32, _P, _P, _P, _P, _P, _P]),
     "c2v_reader_live_rows": (C.c_int64, [_P]),
     "c2v_reader_device_bytes": (C.c_size_t, [_P]),
+    "c2v_reader_stage_bytes": (C.c_size_t, [_I32, C.c_int64]),
+    "c2v_reader_parse_share": (C.c_int, [_P, _P, C.c_int64, C.c_int64, _P, C.c_int64, C.POINTER(c2v_reader_share_status),
+                                         _P]),
+    "c2v_reader_commit_shares": (C.c_int, [_P, C.POINTER(_P), C.POINTER(C.c_int64), _I32, C.POINTER(C.c_int64), _P]),
 }
 
 _lib = None

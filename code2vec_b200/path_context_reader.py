@@ -25,6 +25,7 @@ tests/test_reader_native.py checks they agree row for row.
 from __future__ import annotations
 
 import abc
+import os
 from enum import Enum
 from typing import Iterable, Iterator, List, NamedTuple, Optional
 
@@ -72,6 +73,79 @@ class _Chunk:
 
     def __init__(self, buf: bytes, n: int):
         self.buf, self.n = buf, n
+
+
+_SCAN_BYTES = 1 << 16          # the backward scan for a chunk's last newline reads this many bytes at a time
+_PEEK_BYTES = 1 << 12          # the forward scan for a share's first line start
+
+
+def _rfind(fd: int, lo: int, hi: int, pred) -> int:
+    """The highest position p in [lo, hi) of file fd whose block satisfies pred(block) -> index within the block, or -1;
+    blocks are read backwards from hi."""
+    while hi > lo:
+        a = max(lo, hi - _SCAN_BYTES)
+        blk = os.pread(fd, hi - a, a)
+        i = pred(blk)
+        if i >= 0:
+            return a + i
+        hi = a
+    return -1
+
+
+def chunk_ranges(fd: int, chunk_bytes: int):
+    """The byte ranges [a, b) of the chunks one pass of _native_chunks reads from file fd: a window of chunk_bytes from
+    the end of the previous chunk is cut after its last newline; a window without one (a line longer than it) is retried
+    twice as large, and the larger window stays; the window that reaches the end of the file is the last chunk whole,
+    unless it holds no newline and nothing but '\\r' bytes, which yields nothing.  Each cut is found by reading the
+    window backwards from its end, so a chunk's bytes are not read here."""
+    end = os.fstat(fd).st_size
+    start, size = 0, int(chunk_bytes)
+    clean = 0                                  # [start, clean) is known to hold no newline
+    while start < end:
+        if end - start < size:                 # the window reaches the end of the file
+            if _rfind(fd, start, end, lambda blk: len(blk.rstrip(b"\r")) - 1) >= 0:
+                yield start, end
+            return
+        cut = _rfind(fd, max(start, clean), start + size, lambda blk: blk.rfind(b"\n"))
+        if cut < 0:
+            clean = start + size
+            size *= 2
+            continue
+        yield start, cut + 1
+        start = clean = cut + 1
+
+
+def line_start_at_or_after(fd: int, t: int, a: int, b: int) -> int:
+    """The first line start p >= t of the chunk [a, b) of file fd (p == a, or byte p - 1 is a newline); b if none."""
+    if t <= a:
+        return a
+    p = t - 1
+    while p < b:
+        blk = os.pread(fd, min(_PEEK_BYTES, b - p), p)
+        i = blk.find(b"\n")
+        if i >= 0:
+            return p + i + 1
+        p += len(blk)
+    return b
+
+
+def share_range(fd: int, a: int, b: int, world: int, rank: int):
+    """Rank `rank`'s share [s0, s1) of the chunk [a, b) of file fd among `world` ranks: from the first line start at or
+    after a + rank (b - a) / world to the next rank's start (b for the last rank).  Shares are whole lines in rank order
+    and cover the chunk; a line that spans a split point leaves the shares it swallows empty."""
+    split = lambda r: line_start_at_or_after(fd, a + r * (b - a) // world, a, b)
+    return split(rank), (b if rank == world - 1 else split(rank + 1))
+
+
+def pread_into(fd: int, out, offset: int):
+    """Fills the writable buffer `out` with the file's bytes from `offset` (os.preadv: no intermediate copy)."""
+    mv = memoryview(out).cast("B")
+    done = 0
+    while done < len(mv):
+        n = os.preadv(fd, [mv[done:]], offset + done)
+        if n <= 0:
+            raise EOFError("the data file ended %d bytes short of a chunk it was cut into" % (len(mv) - done))
+        done += n
 
 
 def _raise_parse_error(n: int, kind: int, max_contexts: int):
@@ -161,6 +235,8 @@ class PathContextReader:
         self.model_input_tensors_former = model_input_tensors_former
         self.estimator_action = estimator_action
         self.repeat_endlessly = repeat_endlessly
+        # bytes per chunk of the native path (chunk_ranges): where chunks end decides when the shuffle pool is drawn from
+        self.chunk_bytes = 16 << 20
         tok, pth, tgt = vocabs.token_vocab, vocabs.path_vocab, vocabs.target_vocab
         self.CONTEXT_PADDING = ",".join([tok.special_words.PAD, pth.special_words.PAD, tok.special_words.PAD])
         self.csv_record_defaults = [[tgt.special_words.OOV]] + ([[self.CONTEXT_PADDING]] * config.MAX_CONTEXTS)
@@ -367,11 +443,11 @@ class PathContextReader:
             _raise_parse_error(n, err.value, Cn)
         pool.commit(n, keep[:n])
 
-    def _native_chunks(self):
-        """Complete-line byte chunks of the data file, one pass per epoch like _raw_lines."""
+    def _native_chunk_ranges(self):
+        """(fd, a, b) for every chunk [a, b) of the data file (chunk_ranges), one pass per epoch like _raw_lines; fd is
+        open until the next pass begins."""
         action = self.estimator_action
         path = self.config.data_path(is_evaluating=action.is_evaluate)
-        chunk_bytes = 16 << 20
         passes = 1
         if action.is_train and not self.repeat_endlessly and self.config.NUM_TRAIN_EPOCHS > 1:
             passes = self.config.NUM_TRAIN_EPOCHS
@@ -379,27 +455,20 @@ class PathContextReader:
         while self.repeat_endlessly or p < passes:
             p += 1
             with open(path, "rb") as f:
-                size = chunk_bytes
-                while True:
-                    start = f.tell()
-                    buf = f.read(size)
-                    if not buf:
-                        break
-                    at_eof = len(buf) < size
-                    cut = buf.rfind(b"\n")
-                    if cut < 0:
-                        if at_eof:
-                            if buf.strip(b"\r\n"):
-                                yield _Chunk(buf, len(buf))
-                            break
-                        f.seek(start)                # a line longer than the chunk: retry with a bigger one
-                        size *= 2
-                        continue
-                    if at_eof:
-                        yield _Chunk(buf, len(buf))  # includes a last line without a trailing newline
-                        break
-                    f.seek(start + cut + 1)          # re-read the partial last line with the next chunk
-                    yield _Chunk(buf, cut + 1)           # no slice copy: the parser is told where the complete lines end
+                fd = f.fileno()
+                for a, b in chunk_ranges(fd, self.chunk_bytes):
+                    yield fd, a, b
+
+    def _native_chunks(self):
+        """Complete-line byte chunks of the data file, one pass per epoch like _raw_lines."""
+        for fd, a, b in self._native_chunk_ranges():
+            buf = os.pread(fd, b - a, a)
+            while len(buf) < b - a:                  # a short read: the rest follows
+                more = os.pread(fd, b - a - len(buf), a + len(buf))
+                if not more:
+                    raise EOFError("the data file ended %d bytes short of a chunk it was cut into" % (b - a - len(buf)))
+                buf += more
+            yield _Chunk(buf, b - a)
 
     def _native_chunks_ahead(self, depth: int = 2):
         """_native_chunks read `depth` chunks ahead by a helper thread (file reads and the slicing of complete lines release

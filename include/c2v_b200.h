@@ -498,6 +498,45 @@ int c2v_reader_draw(c2v_reader* r, const int64_t* pick, int32_t b, int32_t lo, i
 int64_t c2v_reader_live_rows(const c2v_reader* r);
 size_t c2v_reader_device_bytes(const c2v_reader* r);
 
+/* A chunk read sharded across W ranks (device_reader.py, DESIGN.md §6d).  The chunk's text is cut at line starts into W
+ * shares in rank order; each rank parses its own share into a *stage*, a peer-visible device allocation (c2v_ipc_alloc)
+ * of c2v_reader_stage_bytes(max_contexts, rows) bytes, and every rank then commits all W stages, its own and its peers'
+ * (opened through CUDA IPC), into its pool.  The pool that results is the one c2v_reader_parse_chunk builds from the
+ * whole chunk, and the chunk's error is decided from the W statuses: with R = the sum of their records and
+ * cap = chunk_bytes / (max_contexts + 1) + 1, kind 3 if R > cap, otherwise the lowest malformed line over the shares
+ * (each share's bad_line plus the newlines of the shares before it) with its share's kind.
+ * A stage holds this status in its first 256 bytes, then the rows and keep flags of up to `rows` records. */
+typedef struct c2v_reader_share_status {
+  int64_t rows;        /* the stage's row capacity                                                              */
+  int64_t records;     /* records (non-blank lines) of the share                                                 */
+  int64_t kept;        /* records that pass the training filter (0 when the share is malformed or overflows)     */
+  int64_t newlines;    /* '\n' bytes of the share                                                                 */
+  int64_t bad_line;    /* the share's lowest malformed line, counted from the share's first byte, or -1          */
+  int32_t bad_kind;    /* 1 (field count), 2 (a context with more than 3 parts) or 0                             */
+  int32_t overflow;    /* records > rows: the share holds a malformed line, or more records than the chunk allows */
+} c2v_reader_share_status;
+
+/* Bytes of a stage of `rows` rows (0 for max_contexts < 1 or rows < 1). */
+size_t c2v_reader_stage_bytes(int32_t max_contexts, int64_t rows);
+
+/* Parses the share text[0, nbytes) (device memory, whole lines) of a chunk of chunk_bytes bytes into `stage` (device
+ * memory of c2v_reader_stage_bytes(max_contexts, stage_rows) bytes) with c2v_reader_parse_chunk's rules, writes the
+ * share's status into the stage and *status, and synchronises `stream`.  A share with more records than stage_rows
+ * rows (a share of n bytes needs at most n / (max_contexts + 1) + 1) is malformed; its lowest malformed line is then
+ * found in the handle's own pool room, unless it has more records than the whole chunk allows.  A malformed share
+ * returns C2V_OK: the chunk's error is decided from every share's status.  The pool is not touched otherwise. */
+int c2v_reader_parse_share(c2v_reader* r, const char* text, int64_t nbytes, int64_t chunk_bytes, void* stage,
+                           int64_t stage_rows, c2v_reader_share_status* status, void* stream);
+
+/* Appends the chunk of n_shares parsed shares (1 <= n_shares <= 64) to the pool: stages[i] (this device's memory or a
+ * peer's opened through CUDA IPC; may be NULL when records[i] == 0) holds share i's records[i] records, shares in rank
+ * order.  The rows and keep flags of every stage are copied behind the live end (kernel assemble_shares_kernel) and the
+ * chunk's records are committed as c2v_reader_parse_chunk commits them.  Call it only for a chunk whose shares all
+ * parsed clean and whose record total is within the chunk's cap.  Synchronises `stream` (so no stage is read once it
+ * returns) and sets *kept to the rows added. */
+int c2v_reader_commit_shares(c2v_reader* r, const void* const* stages, const int64_t* records, int32_t n_shares,
+                             int64_t* kept, void* stream);
+
 #ifdef __cplusplus
 }
 #endif
