@@ -33,7 +33,7 @@ from .multi_rank import (CKPT_MAGIC, CKPT_SUFFIX, batch_split, check_checkpoint_
                          checkpoint_header, create_checkpoint_file, read_checkpoint_header, read_checkpoint_part, run_world,
                          write_checkpoint, write_checkpoint_part)
 from . import device_reader as _device_reader_mod
-from .device_reader import device_reader_flag, sharded_reader_flag
+from .device_reader import device_eval_flag, device_reader_flag, sharded_reader_flag
 from .trainer import Trainer, make_fully_sharded_engine
 from .vocabularies import VocabType
 
@@ -152,6 +152,14 @@ class Code2VecModel(Code2VecModelBase):
         if self._device_reader and config.DL_FRAMEWORK == "b200-keras":
             raise ValueError("C2V_DEVICE_READER=1 is not available with --framework b200-keras: its training loop reads "
                              "batches on the host; unset C2V_DEVICE_READER or train with --framework b200")
+        # C2V_DEVICE_EVAL=1: evaluate() reads, predicts and scores on the GPU (device_reader.py, DESIGN.md §6e)
+        self._device_eval = device_eval_flag(os.environ)
+        if self._device_eval and config.DL_FRAMEWORK == "b200-keras":
+            raise ValueError("C2V_DEVICE_EVAL=1 is not available with --framework b200-keras: its evaluation has its own "
+                             "metrics and loss on the host; unset C2V_DEVICE_EVAL or evaluate with --framework b200")
+        self._device_vocabs = None               # device_reader.DeviceVocabs, shared by the training and evaluation readers
+        self._eval_tables = None                 # device_reader.eval_tables of the target vocabulary
+        self._dev_eval_reader = None
         if self.world > 1:
             self._join_group()
             if self.rank != 0:
@@ -245,6 +253,9 @@ class Code2VecModel(Code2VecModelBase):
         self._hint_next = os.environ.get("C2V_HINT_NEXT", "0") == "1"
         self.log("b200 backend training reader: %s (C2V_DEVICE_READER=%d)" % (
             "on the GPU" if self._device_reader else "on the host", self._device_reader))
+        self.log("b200 backend evaluation: %s (C2V_DEVICE_EVAL=%d)" % (
+            "read, predicted and scored on the GPU" if self._device_eval else "read and scored on the host",
+            self._device_eval))
         if self.world > 1:
             # every multi-GPU run, evaluate-only ones too: the row shards and Trainer.predict live in the Trainer.
             # C2V_DETERMINISTIC=1 sends the embedding gradients through the ordered exchange (DESIGN.md §5.1)
@@ -275,6 +286,10 @@ class Code2VecModel(Code2VecModelBase):
         self.log("Done loading model weights")
 
     def close_session(self):
+        if self._dev_eval_reader is not None:
+            self._dev_eval_reader.close()
+            self._dev_eval_reader = None
+        self._device_vocabs = None
         if self.engine is not None:
             if self.world > 1:
                 import torch
@@ -433,7 +448,8 @@ class Code2VecModel(Code2VecModelBase):
             elif self._sharded_reader:
                 self.log("C2V_SHARDED_READER=1 has no effect on one GPU: the device reader reads the whole file")
             dev_reader = DeviceBatchReader(train_reader, self.engine.dev, world=self.world, rank=self.rank,
-                                           transport=self._reader_transport if multi else None)
+                                           transport=self._reader_transport if multi else None,
+                                           vocabs=self._shared_device_vocabs(train_reader))
         elif not multi and os.environ.get("C2V_BATCH_RING", "1") != "0" and not self._hint_next and train_reader._native_ready():
             import torch
             from .batch_ring import PinnedBatchRing
@@ -571,6 +587,8 @@ class Code2VecModel(Code2VecModelBase):
         subtokens_metric = SubtokensEvaluationMetric(partial(common.filter_impossible_names, special))
         topk_metric = TopKAccuracyEvaluationMetric(cfg.TOP_K_WORDS_CONSIDERED_DURING_PREDICTION,
                                                    partial(common.get_first_match_word_from_top_predictions, special))
+        if self._device_eval:
+            return self._evaluate_device(eval_start_time, subtokens_metric, topk_metric)
         total_predictions, total_batches = 0, 0
         # several GPUs: every rank predicts its slice of each batch, rank 0 gathers the rows and writes every file
         writer = self.rank == 0
@@ -617,6 +635,150 @@ class Code2VecModel(Code2VecModelBase):
             dist.all_gather_object(gathered, results)
             results = gathered[0]
         return results
+
+    # ---- evaluate on the GPU (C2V_DEVICE_EVAL=1, DESIGN.md §6e) -------------------------------------------------------
+    def _shared_device_vocabs(self, reader: PathContextReader):
+        """The model's vocabularies on its device, uploaded once and shared by its training and evaluation readers."""
+        if self._device_vocabs is None:
+            from .device_reader import DeviceVocabs
+            reader.use_native = True
+            reader._native_ready()                 # RuntimeError when libc2v_batcher.so cannot be built
+            self._device_vocabs = DeviceVocabs(reader, self.engine.dev)
+        return self._device_vocabs
+
+    def _device_eval_reader(self):
+        """The evaluation reader on the GPU, made once per model (and again after a pass that failed)."""
+        if self._dev_eval_reader is None:
+            from .device_reader import DeviceBatchReader, eval_tables
+            reader = PathContextReader(vocabs=self.vocabs, model_input_tensors_former=_EvaluateInputFormer(),
+                                       config=self.config, estimator_action=EstimatorAction.Evaluate)
+            if self._eval_tables is None:
+                self._eval_tables = eval_tables(self.vocabs.target_vocab)
+            self._dev_eval_reader = DeviceBatchReader(reader, self.engine.dev, vocabs=self._shared_device_vocabs(reader),
+                                                      tables=self._eval_tables)
+        return self._dev_eval_reader
+
+    def _evaluate_device(self, eval_start_time, subtokens_metric, topk_metric) -> Optional[ModelEvaluationResults]:
+        """evaluate() with the test file read, predicted and scored on the GPU: the same results, log.txt and .vectors
+        as the host route.  Rows the metric kernel flags (a name with a byte >= 0x80, or a top-k without a legal word)
+        are scored by the host metrics themselves; the device's integer sums of the other rows are added to the same
+        metric objects, whose properties then compute every float."""
+        cfg = self.config
+        top_k = cfg.TOP_K_WORDS_CONSIDERED_DURING_PREDICTION
+        index_to_word = self.vocabs.target_vocab.index_to_word
+        hist = np.zeros(top_k, dtype=np.int64)
+        counts = np.zeros(4, dtype=np.int64)          # rows, tp, fp, fn of the rows scored on the device
+        total_predictions, total_batches = 0, 0
+        writer = self.rank == 0
+        reader = self._device_eval_reader()
+        code_vectors_file = open(cfg.TEST_DATA_PATH + ".vectors", "w") if cfg.EXPORT_CODE_VECTORS and writer else None
+        try:
+            with (open("log.txt", "w") if writer else contextlib.nullcontext()) as log_output_file:
+                start_time = time.time()
+                self.log("Starting evaluation")
+                for batch in reader:
+                    batch.wait()                   # the current stream waits for the take into this slot
+                    n = batch.hi - batch.lo
+                    if self.world > 1:
+                        ids, code = self._predict_sharded_device(batch.tensors[:4], n, cfg.EXPORT_CODE_VECTORS)
+                    else:
+                        code, _ = self.engine.forward(*batch.tensors[:4], want_attention=False)
+                        ids, _ = self.engine.topk(code, normalize=False)
+                    if writer:
+                        sc = reader.score(batch, ids)              # synchronises the current stream
+                        code_vectors = code.cpu().numpy() if code_vectors_file is not None else None
+                    batch.release()
+                    total_predictions += n
+                    total_batches += 1
+                    if writer:
+                        k = sc.acc.size - 4
+                        hist[:k] += sc.acc[:k]
+                        counts += sc.acc[k:]
+                        self._log_and_score_host_rows(sc, n, index_to_word, log_output_file, subtokens_metric,
+                                                      topk_metric)
+                        if code_vectors_file is not None:
+                            self._write_code_vectors(code_vectors_file, code_vectors)
+                    if total_batches % cfg.NUM_BATCHES_TO_LOG_PROGRESS == 0:
+                        self._trace_evaluation(total_predictions, time.time() - start_time)
+                self.log("Done evaluating, epoch reached")
+                if writer:
+                    topk_metric.nr_correct_predictions = topk_metric.nr_correct_predictions + np.cumsum(hist).astype(np.float64)
+                    topk_metric.nr_predictions += int(counts[0])
+                    subtokens_metric.nr_predictions += int(counts[0])
+                    subtokens_metric.nr_true_positives += int(counts[1])
+                    subtokens_metric.nr_false_positives += int(counts[2])
+                    subtokens_metric.nr_false_negatives += int(counts[3])
+                    log_output_file.write(str(topk_metric.topk_correct_predictions) + "\n")
+        except BaseException:
+            reader.close()                         # a pass that stopped early leaves rows queued: the next is a new reader
+            self._dev_eval_reader = None
+            raise
+        finally:
+            if code_vectors_file is not None:
+                code_vectors_file.close()
+        self.log("Device evaluation: %.1f MB of text uploaded, %.1f MB of device memory held" % (
+            reader.h2d_bytes / 1e6, reader.device_bytes() / 1e6))
+        elapsed = int(time.time() - eval_start_time)
+        self.log("Evaluation time: %sH:%sM:%sS" % ((elapsed // 60 // 60), (elapsed // 60) % 60, elapsed % 60))
+        results = None
+        if writer:
+            results = ModelEvaluationResults(topk_acc=topk_metric.topk_correct_predictions,
+                                             subtoken_precision=subtokens_metric.precision,
+                                             subtoken_recall=subtokens_metric.recall, subtoken_f1=subtokens_metric.f1)
+        if self.world > 1:                         # every rank returns rank 0's results
+            import torch.distributed as dist
+            gathered = [None] * self.world
+            dist.all_gather_object(gathered, results)
+            results = gathered[0]
+        return results
+
+    def _log_and_score_host_rows(self, sc, n: int, index_to_word, output_file, subtokens_metric, topk_metric):
+        """log.txt lines of one scored batch, in row order: the three line forms of _log_predictions_during_evaluation
+        from the kernel's rank and first legal word, and for flagged rows that method itself; the flagged rows then go
+        through the host metrics (SubtokensEvaluationMetric raises IndexError for a top-k without a legal word)."""
+        names, off = sc.names
+        lines, host_rows = [], []
+        for j in range(n):
+            name = names[off[j]:off[j + 1]].decode("utf-8")
+            if sc.flags[j]:
+                top_words = self.vocabs.target_vocab.lookup_word(sc.ids[j])
+                output_file.write("".join(lines))
+                lines = []
+                self._log_predictions_during_evaluation([(name, top_words)], output_file)
+                host_rows.append((name, top_words))
+                continue
+            r = int(sc.rank[j])
+            if r < 0:
+                lines.append("No results for predicting: " + name)
+            elif r == 0:
+                lines.append("Original: " + name + ", predicted 1st: " + index_to_word[int(sc.first[j])] + "\n")
+            else:
+                lines.append("\t\t predicted correctly at rank: " + str(r + 1) + "\n")
+        output_file.write("".join(lines))
+        if host_rows:
+            topk_metric.update_batch(host_rows)
+            subtokens_metric.update_batch(host_rows)
+
+    def _predict_sharded_device(self, tensors, n_all: int, want_code: bool):
+        """_predict_sharded on a batch already in device memory: (top-k ids [n, k], code vectors [n, D] or None) as
+        device tensors, the slices and padding as there, the ids all-gathered into device memory."""
+        import torch
+        import torch.distributed as dist
+        e, W, r = self.engine, self.world, self.rank
+        idx_parts, code_parts = [], []
+        for s in range(0, n_all, W * e.local_batch):
+            n = min(W * e.local_batch, n_all - s)
+            b = -(-n // W)
+            rows = torch.clamp(torch.arange(s + r * b, s + (r + 1) * b, device=e.dev), max=s + n - 1)
+            idx, _val, code = self.trainer.predict(*(t.index_select(0, rows) for t in tensors), normalize=0)
+            idx_all = torch.empty((W * b, idx.shape[1]), dtype=idx.dtype, device=e.dev)
+            dist.all_gather_into_tensor(idx_all, idx)
+            idx_parts.append(idx_all[:n])
+            if want_code:
+                code_all = torch.empty((W * b, code.shape[1]), dtype=code.dtype, device=e.dev)
+                dist.all_gather_into_tensor(code_all, code)
+                code_parts.append(code_all[:n])
+        return torch.cat(idx_parts).contiguous(), (torch.cat(code_parts) if want_code else None)
 
     def _predict_sharded(self, t: ReaderInputTensors, want_code: bool):
         """(top-k ids [n, k], code vectors [n, D] or None) of the n rows of one reader batch, on rank 0; the other ranks

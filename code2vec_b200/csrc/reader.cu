@@ -14,6 +14,8 @@
 // A chunk read sharded across ranks (DESIGN.md §6d) runs the line index and the parse over one rank's share of the chunk
 // into a peer-visible stage; every rank then copies all stages behind its pool's live end in rank order (assemble) and
 // commits the whole chunk's records as above, so its pool is the one a whole-chunk parse builds.
+// Test files (DESIGN.md §6e) take the same line index and parse with the evaluate filter; their kept records go to an
+// evaluation queue in file order with their names, and eval_score_kernel scores the engine's top-k ids of a batch.
 #include <cuda_runtime.h>
 #include <stdint.h>
 #include <string.h>
@@ -153,8 +155,10 @@ struct ParseArgs {
   long long cap;                  // rows reserved behind the pool's end
   int32_t *src, *path, *dst, *target;     // pool rows from the live end
   float* mask;
-  uint8_t* keep;                  // per record: passes the training filter
+  uint8_t* keep;                  // per record: passes the filter of `mode`
   unsigned long long* bad;        // lowest malformed record << 2 | kind
+  int mode;                       // 0: training filter (a valid context and target > OOV), 1: evaluate (a valid context)
+  int* name_len;                  // evaluate: per record, the bytes of field 0 (the name; 0 = empty); NULL in training
 };
 
 // a part that ends at a separator: part kk of context field f, bytes [start, start + len) of the line
@@ -253,7 +257,8 @@ __global__ void __launch_bounds__(32 * kParseWarps) parse_kernel(const __grid_co
     if (lane == 0) {
       const bool any_valid = max_s != a.tok.pad || max_t != a.tok.pad || max_p != a.pth.pad;
       a.target[li] = ty;
-      a.keep[li] = (any_valid && ty > a.tgt.oov) ? 1 : 0;
+      a.keep[li] = (any_valid && (a.mode == 1 || ty > a.tgt.oov)) ? 1 : 0;
+      if (a.name_len) a.name_len[li] = (int)tgt_len;
     }
     __syncwarp();
   }
@@ -450,6 +455,255 @@ __global__ void __launch_bounds__(256) assemble_shares_kernel(const __grid_const
   }
 }
 
+// ---- evaluation queue (c2v_reader_eval_*) --------------------------------------------------------------------------
+// The kept records of a chunk parsed in evaluate mode, appended to a queue in file order (a stable compaction, unlike the
+// pool commit), each with its name: field 0's bytes, or the target vocabulary's OOV word when field 0 is empty.
+
+// movers[K] = i for the K-th kept record i (ascending); qlen[K] = its name's length, qlen[kept, cap) = 0
+__global__ void __launch_bounds__(256)
+eval_index_kernel(const uint8_t* __restrict__ keep, const int* __restrict__ n_rec, long long cap,
+                  const int* __restrict__ base, int tiles, const int* __restrict__ name_len, int oov_len,
+                  int* __restrict__ movers, int* __restrict__ qlen) {
+  using Scan = cub::BlockScan<int, 256>;
+  __shared__ typename Scan::TempStorage tmp;
+  const long long R = min((long long)*n_rec, cap);
+  const int kept = base[tiles];
+  const long long lo = (long long)blockIdx.x * kRowTile + threadIdx.x * 4;
+  int s = 0;
+  for (int k = 0; k < 4; ++k) s += (lo + k < R) ? keep[lo + k] : 0;
+  int K;
+  Scan(tmp).ExclusiveSum(s, K);
+  K += base[blockIdx.x];
+  for (int k = 0; k < 4; ++k) {
+    const long long i = lo + k;
+    if (i < R && keep[i]) {
+      movers[K] = (int)i;
+      qlen[K] = name_len[i] > 0 ? name_len[i] : oov_len;
+      ++K;
+    }
+    if (i >= kept && i < cap) qlen[i] = 0;
+  }
+}
+
+struct EvalAppendArgs {
+  PoolRows from, to;              // parsed records (pool room), queue rows from its end
+  int C, kept;
+  const int* movers;              // [kept] record of each appended row
+  const int* qoff;                // [kept] name offset from names_end (scan of qlen)
+  const long long* rec_off;       // record -> first byte in text
+  const int* name_len;            // record -> bytes of field 0 (0: the OOV word)
+  const unsigned char* text;
+  const unsigned char* oov_word;  // the target OOV word (word table entry)
+  int oov_len;
+  long long names_end;            // arena bytes in use before the append
+  unsigned char* names;
+  long long* noff;                // name offsets from the queue's end row
+  long long name_total;
+};
+
+// queue row j <- record movers[j], its name -> names[names_end + qoff[j]] (one warp per row)
+__global__ void __launch_bounds__(256) eval_append_kernel(const __grid_constant__ EvalAppendArgs a) {
+  const int lane = threadIdx.x & 31;
+  for (long long j = ((long long)blockIdx.x * 256 + threadIdx.x) >> 5; j < a.kept; j += ((long long)gridDim.x * 256) >> 5) {
+    const int i = a.movers[j];
+    const long long s = (long long)i * a.C, d = j * a.C;
+    for (int c = lane; c < a.C; c += 32) {
+      a.to.src[d + c] = a.from.src[s + c];
+      a.to.path[d + c] = a.from.path[s + c];
+      a.to.dst[d + c] = a.from.dst[s + c];
+      a.to.mask[d + c] = a.from.mask[s + c];
+    }
+    const long long o = a.names_end + a.qoff[j];
+    const long long n = (j + 1 < a.kept ? a.names_end + a.qoff[j + 1] : a.names_end + a.name_total) - o;
+    const unsigned char* src = a.name_len[i] > 0 ? a.text + a.rec_off[i] : a.oov_word;
+    for (long long b = lane; b < n; b += 32) a.names[o + b] = src[b];
+    if (lane == 0) {
+      a.to.target[j] = a.from.target[i];
+      a.noff[j] = o;
+      if (j + 1 == a.kept) a.noff[j + 1] = o + n;
+    }
+  }
+}
+
+// queue rows [head, head + n) -> [0, n), their names to the arena's front, offsets rebased (the two ranges are disjoint)
+__global__ void __launch_bounds__(256)
+eval_compact_kernel(PoolRows q, int C, long long head, long long n, long long* __restrict__ noff,
+                    unsigned char* __restrict__ names) {
+  const int lane = threadIdx.x & 31;
+  const long long nh = noff[head];
+  for (long long j = ((long long)blockIdx.x * 256 + threadIdx.x) >> 5; j < n; j += ((long long)gridDim.x * 256) >> 5) {
+    const long long s = (head + j) * C, d = j * C;
+    for (int c = lane; c < C; c += 32) {
+      q.src[d + c] = q.src[s + c];
+      q.path[d + c] = q.path[s + c];
+      q.dst[d + c] = q.dst[s + c];
+      q.mask[d + c] = q.mask[s + c];
+    }
+    const long long o = noff[head + j], e = noff[head + j + 1];
+    for (long long b = lane; b < e - o; b += 32) names[o - nh + b] = names[o + b];
+    if (lane == 0) {
+      q.target[j] = q.target[head + j];
+      noff[j] = o - nh;
+      if (j + 1 == n) noff[j + 1] = e - nh;
+    }
+  }
+}
+
+// out row j <- queue row head + j, its name -> out_names[out_off[j]] (offsets from the batch's first name; one warp a row)
+__global__ void __launch_bounds__(256)
+eval_take_kernel(PoolRows q, int C, long long head, int b, const long long* __restrict__ noff,
+                 const unsigned char* __restrict__ names, PoolRows out, long long* __restrict__ out_off,
+                 unsigned char* __restrict__ out_names, long long names_cap) {
+  const int lane = threadIdx.x & 31;
+  const long long nh = noff[head];
+  for (long long j = ((long long)blockIdx.x * 256 + threadIdx.x) >> 5; j < b; j += ((long long)gridDim.x * 256) >> 5) {
+    const long long s = (head + j) * C, d = j * C;
+    for (int c = lane; c < C; c += 32) {
+      out.src[d + c] = q.src[s + c];
+      out.path[d + c] = q.path[s + c];
+      out.dst[d + c] = q.dst[s + c];
+      out.mask[d + c] = q.mask[s + c];
+    }
+    const long long o = noff[head + j], e = noff[head + j + 1];
+    for (long long x = lane; x < e - o && o - nh + x < names_cap; x += 32) out_names[o - nh + x] = names[o + x];
+    if (lane == 0) {
+      out.target[j] = q.target[head + j];
+      out_off[j] = o - nh;
+      if (j + 1 == b) out_off[j + 1] = e - nh;
+    }
+  }
+}
+
+// ---- evaluation metrics (c2v_reader_eval_score) ----------------------------------------------------------------------
+struct EvalTables {
+  const unsigned char* words;     // target words, concatenated; word_off [Y + 1]
+  const long long* word_off;
+  const unsigned char* norm;      // normalize_word of each word; norm_off [Y + 1]
+  const long long* norm_off;
+  const uint8_t* legal;           // legal_method_names_checker of each word
+  int Y;
+};
+
+__device__ __forceinline__ bool ascii_letter(unsigned char c) { return (unsigned char)((c | 0x20) - 'a') < 26; }
+
+// normalize_word(name) == nw[0, m) for an ASCII name: its letters lowercased, or the name itself when it has none
+__device__ bool norm_equal(const unsigned char* name, long long L, bool letters, const unsigned char* nw, long long m) {
+  if (!letters) {
+    if (L != m) return false;
+    for (long long p = 0; p < L; ++p)
+      if (name[p] != nw[p]) return false;
+    return true;
+  }
+  long long j = 0;
+  for (long long p = 0; p < L; ++p) {
+    const unsigned char c = name[p];
+    if (!ascii_letter(c)) continue;
+    if (j >= m || (unsigned char)(c | 0x20) != nw[j]) return false;
+    ++j;
+  }
+  return j == m;
+}
+
+// the j-th '|'-separated subtoken of s[0, L) (empty ones count): *start, returns its length
+__device__ long long subtoken(const unsigned char* s, long long L, long long j, long long* start) {
+  long long p = 0;
+  for (long long t = 0; t < j; ++p)
+    if (s[p] == '|') ++t;
+  long long e = p;
+  while (e < L && s[e] != '|') ++e;
+  *start = p;
+  return e - p;
+}
+
+// whether t[0, tl) is one of the subtokens of s[0, L)
+__device__ bool has_subtoken(const unsigned char* s, long long L, const unsigned char* t, long long tl) {
+  long long start = 0;
+  for (long long p = 0; p <= L; ++p) {
+    if (p < L && s[p] != '|') continue;
+    if (p - start == tl) {
+      long long q = 0;
+      while (q < tl && s[start + q] == t[q]) ++q;
+      if (q == tl) return true;
+    }
+    start = p + 1;
+  }
+  return false;
+}
+
+// One warp per row: the rank of the first match among the legal words of the row's top-k (get_first_match_word_from_
+// top_predictions), the first legal word, and the subtoken counts of that word against the name
+// (SubtokensEvaluationMetric.update_batch).  Rows with a byte >= 0x80 in the name, or without a legal word, are flagged
+// and left to the host.  acc: hist [k], rows, tp, fp, fn over the rows scored here.
+__global__ void __launch_bounds__(256)
+eval_score_kernel(EvalTables T, const int32_t* __restrict__ ids, int n, int k, const long long* __restrict__ name_off,
+                  const unsigned char* __restrict__ names, int32_t* __restrict__ rank_out, int32_t* __restrict__ first_out,
+                  int32_t* __restrict__ flags_out, unsigned long long* __restrict__ acc) {
+  const int lane = threadIdx.x & 31;
+  for (long long row = ((long long)blockIdx.x * 256 + threadIdx.x) >> 5; row < n; row += ((long long)gridDim.x * 256) >> 5) {
+    const unsigned char* nm = names + name_off[row];
+    const long long L = name_off[row + 1] - name_off[row];
+    bool high = false, letters = false;
+    int bars = 0;
+    for (long long p = lane; p < L; p += 32) {
+      const unsigned char c = nm[p];
+      high |= c >= 0x80;
+      letters |= ascii_letter(c);
+      bars += c == '|';
+    }
+    high = __any_sync(kFull, high);
+    letters = __any_sync(kFull, letters);
+    bars = __reduce_add_sync(kFull, bars);
+    int rank = -1, first = -1, legal_before = 0;
+    if (!high) {
+      for (int w = 0; w < k; w += 32) {
+        const int i = w + lane;
+        const int id = i < k ? ids[(long long)row * k + i] : -1;
+        const bool lg = id >= 0 && id < T.Y && T.legal[id];
+        const unsigned lm = __ballot_sync(kFull, lg);
+        if (first < 0 && lm) first = __shfl_sync(kFull, id, __ffs(lm) - 1);
+        const bool mt = lg && rank < 0 &&
+                        norm_equal(nm, L, letters, T.norm + T.norm_off[id], T.norm_off[id + 1] - T.norm_off[id]);
+        const unsigned mm = __ballot_sync(kFull, mt);
+        if (rank < 0 && mm) rank = legal_before + __popc(lm & ((1u << (__ffs(mm) - 1)) - 1u));
+        legal_before += __popc(lm);
+      }
+    }
+    const int flags = (high ? 1 : 0) | (!high && first < 0 ? 2 : 0);
+    if (lane == 0) {
+      rank_out[row] = flags ? -1 : rank;
+      first_out[row] = first;
+      flags_out[row] = flags;
+    }
+    if (flags) continue;
+    const unsigned char* g = T.words + T.word_off[first];
+    const long long GL = T.word_off[first + 1] - T.word_off[first];
+    int g_bars = 0;
+    for (long long p = lane; p < GL; p += 32) g_bars += g[p] == '|';
+    g_bars = __reduce_add_sync(kFull, g_bars);
+    unsigned long long tp = 0, fp = 0, fn = 0;
+    for (int j = lane; j <= g_bars; j += 32) {          // guess subtokens, with multiplicity
+      long long s;
+      const long long tl = subtoken(g, GL, j, &s);
+      if (has_subtoken(nm, L, g + s, tl)) ++tp; else ++fp;
+    }
+    for (int j = lane; j <= bars; j += 32) {            // truth subtokens, with multiplicity
+      long long s;
+      const long long tl = subtoken(nm, L, j, &s);
+      if (!has_subtoken(g, GL, nm + s, tl)) ++fn;
+    }
+    tp = __reduce_add_sync(kFull, (unsigned)tp);
+    fp = __reduce_add_sync(kFull, (unsigned)fp);
+    fn = __reduce_add_sync(kFull, (unsigned)fn);
+    if (lane == 0) {
+      if (rank >= 0) atomicAdd(acc + rank, 1ull);
+      atomicAdd(acc + k, 1ull);
+      atomicAdd(acc + k + 1, tp);
+      atomicAdd(acc + k + 2, fp);
+      atomicAdd(acc + k + 3, fn);
+    }
+  }
+}
+
 }  // namespace
 
 struct c2v_reader {
@@ -470,7 +724,25 @@ struct c2v_reader {
   unsigned long long* bad = nullptr;
   int* n_moves = nullptr;
   int* n_rec = nullptr;                                                                     // records of assembled shares
-  struct Status { int records, kept, newlines; unsigned long long bad; long long line; } *host = nullptr;   // pinned read-back
+  // evaluation queue (c2v_reader_eval_*): rows [eq_head, eq_len) are queued in file order, row j's name is
+  // eq_names[eq_noff[j], eq_noff[j + 1])
+  PoolRows eq{};
+  long long eq_cap = 0, eq_head = 0, eq_len = 0;
+  long long* eq_noff = nullptr;                                                             // [eq_cap + 1]
+  unsigned char* eq_names = nullptr;
+  long long eq_names_cap = 0, eq_names_end = 0;
+  long long eval_row_cap = 0;
+  int *name_len = nullptr, *qlen = nullptr, *qoff = nullptr;                                // [eval rows (+ 1)]
+  EvalTables tab{};                                                                         // c2v_reader_eval_tables
+  unsigned char* tab_mem = nullptr;
+  size_t tab_bytes = 0;
+  long long oov_off = 0;                                                                    // the OOV word in tab.words
+  int oov_len = 0;
+  struct Status {
+    int records, kept, newlines, name_bytes;
+    unsigned long long bad;
+    long long line, noff_head;
+  } *host = nullptr;                                                                        // pinned read-back
   size_t bytes = 0;               // device memory held
 };
 
@@ -558,6 +830,75 @@ int reserve_pool(c2v_reader* r, long long more, cudaStream_t st) {
   return C2V_OK;
 }
 
+// evaluate-mode scratch for chunks of up to `rows` records
+int reserve_eval(c2v_reader* r, long long rows, cudaStream_t st) {
+  if (rows <= r->eval_row_cap) return C2V_OK;
+  RD_CUDA(cudaStreamSynchronize(st));
+  const long long old = r->eval_row_cap;
+  int rc;
+  if ((rc = realloc_dev(r, r->name_len, old, rows)) || (rc = realloc_dev(r, r->qlen, old, rows)) ||
+      (rc = realloc_dev(r, r->qoff, old ? old + 1 : 0, rows + 1)))
+    return rc;
+  r->eval_row_cap = rows;
+  return C2V_OK;
+}
+
+// room in the evaluation queue for `rows` rows from row 0 and `name_bytes` name bytes; the queued content moves along
+int reserve_queue(c2v_reader* r, long long rows, long long name_bytes, cudaStream_t st) {
+  const size_t C = (size_t)r->C, n = (size_t)r->eq_len;
+  if (rows > r->eq_cap) {
+    long long cap = r->eq_cap ? 2 * r->eq_cap : 1024;
+    if (cap < rows) cap = rows;
+    PoolRows g{};
+    long long* noff = nullptr;
+    RD_CUDA(cudaMalloc(&g.src, (size_t)cap * C * 4));
+    RD_CUDA(cudaMalloc(&g.path, (size_t)cap * C * 4));
+    RD_CUDA(cudaMalloc(&g.dst, (size_t)cap * C * 4));
+    RD_CUDA(cudaMalloc(&g.mask, (size_t)cap * C * 4));
+    RD_CUDA(cudaMalloc(&g.target, (size_t)cap * 4));
+    RD_CUDA(cudaMalloc(&noff, (size_t)(cap + 1) * 8));
+    if (r->eq_cap) {
+      RD_CUDA(cudaMemcpyAsync(g.src, r->eq.src, n * C * 4, cudaMemcpyDeviceToDevice, st));
+      RD_CUDA(cudaMemcpyAsync(g.path, r->eq.path, n * C * 4, cudaMemcpyDeviceToDevice, st));
+      RD_CUDA(cudaMemcpyAsync(g.dst, r->eq.dst, n * C * 4, cudaMemcpyDeviceToDevice, st));
+      RD_CUDA(cudaMemcpyAsync(g.mask, r->eq.mask, n * C * 4, cudaMemcpyDeviceToDevice, st));
+      RD_CUDA(cudaMemcpyAsync(g.target, r->eq.target, n * 4, cudaMemcpyDeviceToDevice, st));
+      RD_CUDA(cudaMemcpyAsync(noff, r->eq_noff, (n + 1) * 8, cudaMemcpyDeviceToDevice, st));
+      RD_CUDA(cudaStreamSynchronize(st));
+      for (void* p : {(void*)r->eq.src, (void*)r->eq.path, (void*)r->eq.dst, (void*)r->eq.mask, (void*)r->eq.target,
+                      (void*)r->eq_noff})
+        RD_CUDA(cudaFree(p));
+      r->bytes -= (size_t)r->eq_cap * (4 * C + 1) * 4 + (size_t)(r->eq_cap + 1) * 8;
+    }
+    r->eq = g;
+    r->eq_noff = noff;
+    r->eq_cap = cap;
+    r->bytes += (size_t)cap * (4 * C + 1) * 4 + (size_t)(cap + 1) * 8;
+  }
+  if (name_bytes > r->eq_names_cap) {
+    long long cap = r->eq_names_cap ? 2 * r->eq_names_cap : 1 << 16;
+    if (cap < name_bytes) cap = name_bytes;
+    unsigned char* g = nullptr;
+    RD_CUDA(cudaMalloc(&g, (size_t)cap));
+    if (r->eq_names) {
+      RD_CUDA(cudaMemcpyAsync(g, r->eq_names, (size_t)r->eq_names_end, cudaMemcpyDeviceToDevice, st));
+      RD_CUDA(cudaStreamSynchronize(st));
+      RD_CUDA(cudaFree(r->eq_names));
+      r->bytes -= (size_t)r->eq_names_cap;
+    }
+    r->eq_names = g;
+    r->eq_names_cap = cap;
+    r->bytes += (size_t)cap;
+  }
+  return C2V_OK;
+}
+
+int row_grid(const c2v_reader* r, long long rows) {            // one warp per row, 8 rows a block
+  long long g = (rows + 7) / 8;
+  if (g > (long long)r->num_sms * 8) g = (long long)r->num_sms * 8;
+  return (int)(g > 0 ? g : 1);
+}
+
 DevVocab dev_vocab(const c2v_reader_vocab& v) {
   return DevVocab{(const DevSlot*)v.slots, (const unsigned char*)v.bytes, (unsigned long long)v.mask, v.oov, v.pad};
 }
@@ -567,14 +908,14 @@ size_t parse_smem(int C) { return (size_t)kParseWarps * 3 * C * sizeof(longlong2
 // line index and parse of text[0, nbytes) (nbytes > 0, `tiles` tiles of it, scratch reserved for `cap` records): the
 // first `cap` records land in rows[0, cap) and keep[0, cap), the lowest malformed one in r->bad
 int index_and_parse(c2v_reader* r, const unsigned char* t, long long nbytes, int tiles, long long cap, PoolRows rows,
-                    uint8_t* keep, cudaStream_t st) {
+                    uint8_t* keep, cudaStream_t st, int mode = 0, int* name_len = nullptr) {
   RD_CUDA(cudaMemsetAsync(r->bad, 0xff, sizeof(unsigned long long), st));
   line_count_kernel<<<tiles, kTileThreads, 0, st>>>(t, nbytes, r->rec_cnt, r->nl_cnt);
   exclusive_scan_kernel<<<1, 1024, 0, st>>>(r->rec_cnt, r->rec_base, tiles);
   exclusive_scan_kernel<<<1, 1024, 0, st>>>(r->nl_cnt, r->nl_base, tiles);
   line_index_kernel<<<tiles, kTileThreads, 0, st>>>(t, nbytes, r->rec_base, r->nl_base, cap, r->rec_off, r->rec_line);
   ParseArgs a{t, nbytes, r->C, r->tok, r->pth, r->tgt, r->rec_off, r->rec_base + tiles, cap,
-              rows.src, rows.path, rows.dst, rows.target, rows.mask, keep, r->bad};
+              rows.src, rows.path, rows.dst, rows.target, rows.mask, keep, r->bad, mode, name_len};
   long long grid = (cap + kParseWarps - 1) / kParseWarps;
   if (grid > (long long)r->num_sms * 16) grid = (long long)r->num_sms * 16;
   parse_kernel<<<(unsigned)grid, 32 * kParseWarps, parse_smem(r->C), st>>>(a);
@@ -644,7 +985,10 @@ void c2v_reader_destroy(c2v_reader* r) {
   for (void* p : {(void*)r->pool.src, (void*)r->pool.path, (void*)r->pool.dst, (void*)r->pool.mask, (void*)r->pool.target,
                   (void*)r->rec_cnt, (void*)r->nl_cnt, (void*)r->rec_base, (void*)r->nl_base, (void*)r->rec_off,
                   (void*)r->rec_line, (void*)r->keep, (void*)r->keep_cnt, (void*)r->keep_base, (void*)r->holes,
-                  (void*)r->movers, (void*)r->pick, (void*)r->tail, (void*)r->bad, (void*)r->n_moves, (void*)r->n_rec})
+                  (void*)r->movers, (void*)r->pick, (void*)r->tail, (void*)r->bad, (void*)r->n_moves, (void*)r->n_rec,
+                  (void*)r->eq.src, (void*)r->eq.path, (void*)r->eq.dst, (void*)r->eq.mask, (void*)r->eq.target,
+                  (void*)r->eq_noff, (void*)r->eq_names, (void*)r->name_len, (void*)r->qlen, (void*)r->qoff,
+                  (void*)r->tab_mem})
     if (p) cudaFree(p);
   if (r->host) cudaFreeHost(r->host);
   delete r;
@@ -819,6 +1163,158 @@ int c2v_reader_commit_shares(c2v_reader* r, const void* const* stages, const int
   assemble_shares_kernel<<<dim3((unsigned)per, (unsigned)n_shares), 256, 0, st>>>(a);
   RD_CUDA(cudaGetLastError());
   return commit_records(r, r->n_rec, total, kept, st);
+}
+
+
+int c2v_reader_eval_tables(c2v_reader* r, int32_t n_words, const char* words, const int64_t* word_off, const char* norm,
+                           const int64_t* norm_off, const uint8_t* legal, void* stream) {
+  if (!r || !word_off || !norm_off || !legal || (word_off[n_words > 0 ? n_words : 0] > 0 && !words))
+    return rfail(C2V_ERR_INVALID, "c2v_reader_eval_tables: NULL argument");
+  if (n_words <= r->tgt.oov || r->tgt.oov < 0)
+    return rfail(C2V_ERR_INVALID, "c2v_reader_eval_tables: the tables must cover every target word, the OOV word included");
+  if (word_off[0] != 0 || norm_off[0] != 0) return rfail(C2V_ERR_INVALID, "c2v_reader_eval_tables: offsets start at 0");
+  for (int i = 0; i < n_words; ++i)
+    if (word_off[i + 1] < word_off[i] || norm_off[i + 1] < norm_off[i])
+      return rfail(C2V_ERR_INVALID, "c2v_reader_eval_tables: offsets must not decrease");
+  RD_CUDA(cudaSetDevice(r->device));
+  cudaStream_t st = (cudaStream_t)stream;
+  const long long Y = n_words, wb = word_off[Y], nb = norm_off[Y];
+  const long long o_woff = 0, o_noff = align256(o_woff + (Y + 1) * 8), o_legal = align256(o_noff + (Y + 1) * 8),
+                  o_words = align256(o_legal + Y), o_norm = align256(o_words + wb), total = align256(o_norm + nb);
+  RD_CUDA(cudaStreamSynchronize(st));
+  if (r->tab_mem) {
+    RD_CUDA(cudaFree(r->tab_mem));
+    r->bytes -= r->tab_bytes;
+    r->tab_mem = nullptr;
+    r->tab = EvalTables{};
+  }
+  RD_CUDA(cudaMalloc(&r->tab_mem, (size_t)total));
+  r->tab_bytes = (size_t)total;
+  r->bytes += r->tab_bytes;
+  unsigned char* m = r->tab_mem;
+  RD_CUDA(cudaMemcpyAsync(m + o_woff, word_off, (size_t)(Y + 1) * 8, cudaMemcpyHostToDevice, st));
+  RD_CUDA(cudaMemcpyAsync(m + o_noff, norm_off, (size_t)(Y + 1) * 8, cudaMemcpyHostToDevice, st));
+  RD_CUDA(cudaMemcpyAsync(m + o_legal, legal, (size_t)Y, cudaMemcpyHostToDevice, st));
+  if (wb) RD_CUDA(cudaMemcpyAsync(m + o_words, words, (size_t)wb, cudaMemcpyHostToDevice, st));
+  if (nb) RD_CUDA(cudaMemcpyAsync(m + o_norm, norm, (size_t)nb, cudaMemcpyHostToDevice, st));
+  RD_CUDA(cudaStreamSynchronize(st));
+  r->tab = EvalTables{m + o_words, (const long long*)(m + o_woff), m + o_norm, (const long long*)(m + o_noff),
+                      m + o_legal, (int)Y};
+  r->oov_off = word_off[r->tgt.oov];
+  r->oov_len = (int)(word_off[r->tgt.oov + 1] - word_off[r->tgt.oov]);
+  return C2V_OK;
+}
+
+int c2v_reader_eval_append(c2v_reader* r, const char* text, int64_t nbytes, int64_t* appended, int64_t* name_bytes,
+                           int64_t* bad_line, int32_t* bad_kind, void* stream) {
+  if (!r || !text || !appended || !name_bytes || !bad_line || !bad_kind || nbytes < 0)
+    return rfail(C2V_ERR_INVALID, "c2v_reader_eval_append: NULL argument or negative size");
+  *appended = 0; *bad_line = -1; *bad_kind = 0;
+  *name_bytes = r->eq_names_end;
+  if (!r->tab_mem) return rfail(C2V_ERR_STATE, "c2v_reader_eval_append: upload the tables first (c2v_reader_eval_tables)");
+  if (nbytes == 0) return C2V_OK;
+  RD_CUDA(cudaSetDevice(r->device));
+  cudaStream_t st = (cudaStream_t)stream;
+  const long long cap = nbytes / (r->C + 1) + 1;      // a well-formed line is at least MAX_CONTEXTS spaces + a newline long
+  int rc;
+  if ((rc = reserve_scratch(r, nbytes, cap, 0, st)) || (rc = reserve_pool(r, cap, st)) || (rc = reserve_eval(r, cap, st)))
+    return rc;
+  const int tiles = (int)((nbytes + kTile - 1) / kTile), row_tiles = (int)((cap + kRowTile - 1) / kRowTile);
+  const unsigned char* t = (const unsigned char*)text;
+  const long long l0 = r->live * r->C;
+  const PoolRows room{r->pool.src + l0, r->pool.path + l0, r->pool.dst + l0, r->pool.target + r->live, r->pool.mask + l0};
+  if ((rc = index_and_parse(r, t, nbytes, tiles, cap, room, r->keep, st, 1, r->name_len))) return rc;
+  const int* n_rec = r->rec_base + tiles;
+  keep_count_kernel<<<row_tiles, 256, 0, st>>>(r->keep, n_rec, cap, r->keep_cnt);
+  exclusive_scan_kernel<<<1, 1024, 0, st>>>(r->keep_cnt, r->keep_base, row_tiles);
+  eval_index_kernel<<<row_tiles, 256, 0, st>>>(r->keep, n_rec, cap, r->keep_base, row_tiles, r->name_len, r->oov_len,
+                                               r->movers, r->qlen);
+  exclusive_scan_kernel<<<1, 1024, 0, st>>>(r->qlen, r->qoff, (int)cap);
+  RD_CUDA(cudaGetLastError());
+  RD_CUDA(cudaMemcpyAsync(&r->host->records, n_rec, sizeof(int), cudaMemcpyDeviceToHost, st));
+  RD_CUDA(cudaMemcpyAsync(&r->host->kept, r->keep_base + row_tiles, sizeof(int), cudaMemcpyDeviceToHost, st));
+  RD_CUDA(cudaMemcpyAsync(&r->host->name_bytes, r->qoff + cap, sizeof(int), cudaMemcpyDeviceToHost, st));
+  RD_CUDA(cudaMemcpyAsync(&r->host->bad, r->bad, sizeof(unsigned long long), cudaMemcpyDeviceToHost, st));
+  if (r->eq_len > r->eq_head)
+    RD_CUDA(cudaMemcpyAsync(&r->host->noff_head, r->eq_noff + r->eq_head, sizeof(long long), cudaMemcpyDeviceToHost, st));
+  RD_CUDA(cudaStreamSynchronize(st));
+  if (r->host->records > cap) {
+    *bad_kind = 3;
+    return rfail(C2V_ERR_INVALID, "c2v_reader_eval_append: more records than a chunk of this size holds well-formed lines");
+  }
+  if (r->host->bad != ~0ull) {
+    const long long li = (long long)(r->host->bad >> 2);
+    RD_CUDA(cudaMemcpyAsync(&r->host->line, r->rec_line + li, sizeof(long long), cudaMemcpyDeviceToHost, st));
+    RD_CUDA(cudaStreamSynchronize(st));
+    *bad_line = r->host->line;
+    *bad_kind = (int32_t)(r->host->bad & 3);
+    return rfail(C2V_ERR_INVALID, std::string("c2v_reader_eval_append: malformed line ") + std::to_string(*bad_line) +
+                                      (*bad_kind == 2 ? " (a context has more than 3 parts)" : " (field count)"));
+  }
+  // the rows taken so far leave the queue: the rest moves to its front when the two ranges do not overlap
+  const long long left = r->eq_len - r->eq_head;
+  if (left == 0) {
+    r->eq_head = r->eq_len = r->eq_names_end = 0;
+  } else if (r->eq_head > 0 && left < r->eq_head && r->eq_names_end - r->host->noff_head <= r->host->noff_head) {
+    eval_compact_kernel<<<row_grid(r, left), 256, 0, st>>>(r->eq, r->C, r->eq_head, left, r->eq_noff, r->eq_names);
+    RD_CUDA(cudaGetLastError());
+    r->eq_names_end -= r->host->noff_head;
+    r->eq_head = 0;
+    r->eq_len = left;
+  }
+  const int kept = r->host->kept;
+  const long long nb = r->host->name_bytes;
+  if (kept > 0) {
+    if ((rc = reserve_queue(r, r->eq_len + kept, r->eq_names_end + nb, st))) return rc;
+    const long long q0 = r->eq_len * r->C;
+    EvalAppendArgs a{room, PoolRows{r->eq.src + q0, r->eq.path + q0, r->eq.dst + q0, r->eq.target + r->eq_len,
+                                    r->eq.mask + q0},
+                     r->C, kept, r->movers, r->qoff, r->rec_off, r->name_len, t, r->tab.words + r->oov_off, r->oov_len,
+                     r->eq_names_end, r->eq_names, r->eq_noff + r->eq_len, nb};
+    eval_append_kernel<<<row_grid(r, kept), 256, 0, st>>>(a);
+    RD_CUDA(cudaGetLastError());
+    r->eq_len += kept;
+    r->eq_names_end += nb;
+  }
+  *appended = kept;
+  *name_bytes = r->eq_names_end;
+  return C2V_OK;
+}
+
+int c2v_reader_eval_take(c2v_reader* r, int32_t b, int32_t* src, int32_t* path, int32_t* tgt, float* mask,
+                         int32_t* target, int64_t* name_off, char* names, int64_t names_cap, void* stream) {
+  if (!r || !src || !path || !tgt || !mask || !target || !name_off || !names)
+    return rfail(C2V_ERR_INVALID, "c2v_reader_eval_take: NULL argument");
+  if (b < 1 || b > r->eq_len - r->eq_head)
+    return rfail(C2V_ERR_INVALID, "c2v_reader_eval_take: b must be in [1, queued rows]");
+  if (names_cap < r->eq_names_end)
+    return rfail(C2V_ERR_INVALID, "c2v_reader_eval_take: names_cap must be at least the name bytes the last append reported");
+  RD_CUDA(cudaSetDevice(r->device));
+  cudaStream_t st = (cudaStream_t)stream;
+  eval_take_kernel<<<row_grid(r, b), 256, 0, st>>>(r->eq, r->C, r->eq_head, b, r->eq_noff, r->eq_names,
+                                                   PoolRows{src, path, tgt, target, mask}, (long long*)name_off,
+                                                   (unsigned char*)names, names_cap);
+  RD_CUDA(cudaGetLastError());
+  r->eq_head += b;
+  return C2V_OK;
+}
+
+int64_t c2v_reader_eval_queued(const c2v_reader* r) { return r ? r->eq_len - r->eq_head : -1; }
+
+int c2v_reader_eval_score(const c2v_reader* r, const int32_t* ids, int32_t n, int32_t k, const int64_t* name_off,
+                          const char* names, int32_t* rank, int32_t* first, int32_t* flags, int64_t* acc, void* stream) {
+  if (!r || !ids || !name_off || !names || !rank || !first || !flags || !acc)
+    return rfail(C2V_ERR_INVALID, "c2v_reader_eval_score: NULL argument");
+  if (n < 1 || k < 1) return rfail(C2V_ERR_INVALID, "c2v_reader_eval_score: need n >= 1 and k >= 1");
+  if (!r->tab_mem) return rfail(C2V_ERR_STATE, "c2v_reader_eval_score: upload the tables first (c2v_reader_eval_tables)");
+  RD_CUDA(cudaSetDevice(r->device));
+  cudaStream_t st = (cudaStream_t)stream;
+  RD_CUDA(cudaMemsetAsync(acc, 0, (size_t)(k + 4) * sizeof(int64_t), st));
+  eval_score_kernel<<<row_grid(r, n), 256, 0, st>>>(r->tab, ids, n, k, (const long long*)name_off,
+                                                    (const unsigned char*)names, rank, first, flags,
+                                                    (unsigned long long*)acc);
+  RD_CUDA(cudaGetLastError());
+  return C2V_OK;
 }
 
 int64_t c2v_reader_live_rows(const c2v_reader* r) { return r ? r->live : -1; }

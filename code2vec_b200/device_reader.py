@@ -14,7 +14,13 @@ Sharded (C2V_SHARDED_READER=1 on W > 1 ranks, a ShareTransport given): the ranks
 lines (path_context_reader.share_range); each rank reads, uploads and parses only its own share into a stage of its
 device memory (c2v_reader_parse_share), the ranks gather their share statuses once per chunk, and every rank assembles
 all W stages, its peers' read through CUDA IPC, into its pool (c2v_reader_commit_shares).  Chunk bounds, pool, kept
-counts and draws stay exactly those of the unsharded reader, so the batches do too."""
+counts and draws stay exactly those of the unsharded reader, so the batches do too.
+
+Evaluate mode (a PathContextReader with EstimatorAction.Evaluate; C2V_DEVICE_EVAL=1, DESIGN.md §6e): the test file is
+parsed in device memory with the evaluate filter, the kept rows queue in file order with their names, and every batch is
+the queue's next TEST_BATCH_SIZE rows -- the batches of _iterate_batches_native in evaluate mode, row for row, across
+chunk boundaries.  score() runs the metric kernel on the engine's top-k ids of a batch and brings back only the per-row
+results, the names and the integer accumulators."""
 from __future__ import annotations
 
 import ctypes as C
@@ -38,6 +44,14 @@ def device_reader_flag(environ) -> bool:
     flag = environ.get("C2V_DEVICE_READER", "0") or "0"
     if flag not in ("0", "1"):
         raise ValueError("C2V_DEVICE_READER must be 0 or 1, got %r" % flag)
+    return flag == "1"
+
+
+def device_eval_flag(environ) -> bool:
+    """C2V_DEVICE_EVAL=1: Code2VecModel.evaluate() reads, predicts and scores on the GPU; 0 (the default): on the host."""
+    flag = environ.get("C2V_DEVICE_EVAL", "0") or "0"
+    if flag not in ("0", "1"):
+        raise ValueError("C2V_DEVICE_EVAL must be 0 or 1, got %r" % flag)
     return flag == "1"
 
 
@@ -145,11 +159,66 @@ def export_vocab(lib, handle):
     return slot_arr, byte_arr, int(mask.value), int(oov.value), int(pad.value)
 
 
+class DeviceVocabs:
+    """The native tensoriser's three vocabularies (c2v_vocab_export) copied to one device, with the c2v_reader_vocab
+    structs that point at them.  One model uploads them once and shares them between its training and evaluation readers
+    (about 165 MB at java14m size); `reader` is any PathContextReader of the model with the native tensoriser ready."""
+
+    def __init__(self, reader: PathContextReader, device):
+        import torch
+        lib_b, tok, pth, tgt = reader._native
+        self.dev = torch.device(device)
+        self.tensors, self.structs = [], []
+        with torch.cuda.device(self.dev):
+            for v in (tok, pth, tgt):
+                slot_arr, byte_arr, mask, oov, pad = export_vocab(lib_b, v.h)
+                d_slots = torch.from_numpy(slot_arr).to(self.dev)
+                d_bytes = torch.from_numpy(byte_arr if byte_arr.size else np.zeros(1, dtype=np.uint8)).to(self.dev)
+                self.tensors += [d_slots, d_bytes]
+                self.structs.append(c2v_reader_vocab(d_slots.data_ptr(), d_bytes.data_ptr(), mask, oov, pad))
+            torch.cuda.synchronize(self.dev)
+
+    def nbytes(self) -> int:
+        return int(sum(t.numel() * t.element_size() for t in self.tensors))
+
+
+def eval_tables(target_vocab):
+    """The per-target-word tables of the metric kernel (c2v_reader_eval_tables), computed with the host metrics' own
+    functions: (words, word_off, norm, norm_off, legal) -- every word's UTF-8 bytes, its common.normalize_word bytes and
+    common.legal_method_names_checker, as numpy arrays."""
+    from .common import common
+    special = target_vocab.special_words
+    words = [target_vocab.index_to_word[i] for i in range(target_vocab.size)]
+    enc = [w.encode("utf-8") for w in words]
+    norm = [common.normalize_word(w).encode("utf-8") for w in words]
+    legal = np.fromiter((bool(common.legal_method_names_checker(special, w)) for w in words), dtype=np.uint8,
+                        count=len(words))
+
+    def packed(items):
+        off = np.zeros(len(items) + 1, dtype=np.int64)
+        np.cumsum([len(b) for b in items], out=off[1:])
+        return np.frombuffer(b"".join(items) or b"\0", dtype=np.uint8), off
+    w, w_off = packed(enc)
+    n, n_off = packed(norm)
+    return w, w_off, n, n_off, legal
+
+
+class EvalScores:
+    """What the metric kernel returns to the host for one batch of n rows: rank, first, flags [n] int32 (as
+    c2v_reader_eval_score defines them), acc [k + 4] int64 (rank histogram, rows, tp, fp, fn of the rows scored on the
+    device), and the rows' names (bytes).  ids [n, k] int32 only when a row is flagged: the host scores those rows."""
+    __slots__ = ("rank", "first", "flags", "acc", "names", "ids")
+
+    def __init__(self, rank, first, flags, acc, names, ids):
+        self.rank, self.first, self.flags, self.acc, self.names, self.ids = rank, first, flags, acc, names, ids
+
+
 class DeviceBatch:
     """One batch in a device slot: `tensors` = (src, path, tgt [rows, C] int32, mask [rows, C] float32, target [rows]
     int32) holding rows [lo, hi) of a global batch of `rows` rows (all of it on one GPU); `dropped` rows of a short batch
     are left out on several ranks (multi_rank.batch_split).  wait() makes the current stream wait for the draw; release()
-    hands the slot back once the work queued so far on the current stream (the step that read it) is done."""
+    hands the slot back once the work queued so far on the current stream (the step that read it) is done.  An
+    evaluation batch also has its rows' names on the device (score() reads them)."""
     __slots__ = ("tensors", "rows", "lo", "hi", "dropped", "_slot", "_reader")
 
     def __init__(self, slot, rows, lo, hi, dropped, reader):
@@ -172,14 +241,21 @@ class DeviceBatchReader:
     config decide every batch).  world / rank: this rank's slice of each global batch.  A reader thread uploads and parses
     the chunks and queues the draws into `slots` device slots, each reused only after the step that last read it; the
     iterating (training) thread never waits for the GPU.  Needs libc2v_batcher.so (RuntimeError otherwise, as
-    use_native=True does)."""
+    use_native=True does).  With an evaluate-mode `reader` the slots are filled by sequential takes from the evaluation
+    queue (no draws, no RNG), and the reader may be iterated again once a pass has ended."""
 
     def __init__(self, reader: PathContextReader, device, world: int = 1, rank: int = 0, slots: int = 4,
-                 transport: Optional[ShareTransport] = None):
-        """transport: read the chunks sharded across the `world` ranks, meeting through it (ignored on one rank)."""
+                 transport: Optional[ShareTransport] = None, vocabs: Optional[DeviceVocabs] = None, tables=None):
+        """transport: read the chunks sharded across the `world` ranks, meeting through it (ignored on one rank).
+        vocabs: the model's DeviceVocabs (uploaded here when None).  tables: eval_tables(target vocabulary), needed by
+        an evaluation reader (an evaluate-mode `reader`); every rank of an evaluation reads the whole file."""
         import torch
-        if not reader.estimator_action.is_train:
-            raise ValueError("the device reader reads training files only")
+        action = reader.estimator_action
+        if not (action.is_train or action.is_evaluate):
+            raise ValueError("the device reader reads training and evaluation files only")
+        self.evaluate = action.is_evaluate
+        if self.evaluate and tables is None:
+            raise ValueError("an evaluation reader needs the target-word tables (device_reader.eval_tables)")
         if slots < 3:
             raise ValueError("the device reader needs at least 3 batch slots")
         reader.use_native = True
@@ -190,21 +266,14 @@ class DeviceBatchReader:
         self.world, self.rank = int(world), int(rank)
         cfg = reader.config
         self.C = int(cfg.MAX_CONTEXTS)
-        self.B = int(cfg.TRAIN_BATCH_SIZE)
+        self.B = int(cfg.batch_size(is_evaluating=self.evaluate))
         self.S = max(int(cfg.SHUFFLE_BUFFER_SIZE), 1)
         self.h2d_bytes = 0
-        lib_b, tok, pth, tgt = reader._native
-        self._vocab_tensors = []
-        structs = []
+        self.vocabs = vocabs if vocabs is not None else DeviceVocabs(reader, self.dev)
+        self._own_vocabs = vocabs is None
+        structs = self.vocabs.structs
+        self._structs = structs
         with torch.cuda.device(self.dev):
-            for v in (tok, pth, tgt):
-                slot_arr, byte_arr, mask, oov, pad = export_vocab(lib_b, v.h)
-                d_slots = torch.from_numpy(slot_arr).to(self.dev)
-                d_bytes = torch.from_numpy(byte_arr if byte_arr.size else np.zeros(1, dtype=np.uint8)).to(self.dev)
-                self._vocab_tensors += [d_slots, d_bytes]
-                structs.append(c2v_reader_vocab(d_slots.data_ptr(), d_bytes.data_ptr(), mask, oov, pad))
-            torch.cuda.synchronize(self.dev)
-            self._structs = structs
             h = C.c_void_p()
             rc = self.lib.c2v_reader_create(self.C, C.byref(structs[0]), C.byref(structs[1]), C.byref(structs[2]),
                                             self.dev.index or 0, C.byref(h))
@@ -213,7 +282,16 @@ class DeviceBatchReader:
             self.h = h
             self.stream = torch.cuda.Stream(device=self.dev)
             self.copy_stream = torch.cuda.Stream(device=self.dev)
-            local = self.B // self.world
+            self._name_bytes = 0                   # evaluate: the bound on a take's name bytes (c2v_reader_eval_append)
+            self.table_bytes = 0
+            if self.evaluate:
+                w, w_off, n, n_off, legal = tables
+                rc = self.lib.c2v_reader_eval_tables(self.h, int(legal.size), w.ctypes.data, w_off.ctypes.data,
+                                                     n.ctypes.data, n_off.ctypes.data, legal.ctypes.data,
+                                                     self.stream.cuda_stream)
+                if rc != 0:
+                    raise EngineError(rc, self.lib.c2v_last_error(None).decode())
+            local = self.B if self.evaluate else self.B // self.world
             self.slots = []
             for _ in range(slots):
                 s = {"tensors": (torch.empty((local, self.C), dtype=torch.int32, device=self.dev),
@@ -223,6 +301,9 @@ class DeviceBatchReader:
                                  torch.empty((local,), dtype=torch.int32, device=self.dev)),
                      "pick": torch.empty(self.B, dtype=torch.int64).pin_memory(),
                      "ready": torch.cuda.Event(), "done": torch.cuda.Event(), "free": threading.Event()}
+                if self.evaluate:
+                    s["name_off"] = torch.empty(self.B + 1, dtype=torch.int64, device=self.dev)
+                    s["names"] = torch.empty(1 << 16, dtype=torch.uint8, device=self.dev)
                 s["free"].set()
                 self.slots.append(s)
         # chunk text: two page-locked buffers and two device buffers, so the upload of chunk k+1 overlaps the draws of k
@@ -276,6 +357,101 @@ class DeviceBatchReader:
                 _raise_parse_error(-(bad_line.value + 1), bad_kind.value, self.C)
             raise EngineError(rc, self.lib.c2v_last_error(None).decode())
         return int(kept.value)
+
+    # ---- evaluate mode -------------------------------------------------------------------------------------------------
+    def _append(self, chunk, i: int) -> int:
+        """Chunk `chunk` uploaded from host buffer i and appended to the evaluation queue; returns the rows kept."""
+        torch = self.torch
+        n = int(chunk.n)
+        buf = self._text_buffers(i, n)
+        buf["uploaded"].synchronize()
+        buf["np"][:n] = np.frombuffer(chunk.buf, dtype=np.uint8, count=n)
+        with torch.cuda.stream(self.copy_stream):
+            buf["dev"][:n].copy_(buf["host"][:n], non_blocking=True)
+            buf["uploaded"].record(self.copy_stream)
+        self.stream.wait_event(buf["uploaded"])
+        self.h2d_bytes += n
+        kept, name_bytes, bad_line, bad_kind = C.c_int64(), C.c_int64(), C.c_int64(), C.c_int32()
+        rc = self.lib.c2v_reader_eval_append(self.h, buf["dev"].data_ptr(), n, C.byref(kept), C.byref(name_bytes),
+                                             C.byref(bad_line), C.byref(bad_kind), self.stream.cuda_stream)
+        if rc != 0:
+            if bad_kind.value == 3:
+                _raise_parse_error(_INT64_MIN, 0, self.C)
+            if bad_kind.value in (1, 2):
+                _raise_parse_error(-(bad_line.value + 1), bad_kind.value, self.C)
+            raise EngineError(rc, self.lib.c2v_last_error(None).decode())
+        self._name_bytes = int(name_bytes.value)
+        return int(kept.value)
+
+    def _take(self, b: int, k: int):
+        """Batch k: the queue's next b rows and their names; None when the consumer has gone."""
+        s = self._acquire(k)
+        if s is None:
+            return None
+        if s["names"].numel() < self._name_bytes:          # the slot's last reader is done (_acquire): it may grow
+            s["names"] = self.torch.empty(max(self._name_bytes, 2 * s["names"].numel()), dtype=self.torch.uint8,
+                                          device=self.dev)
+        t = s["tensors"]
+        rc = self.lib.c2v_reader_eval_take(self.h, b, *(x.data_ptr() for x in t), s["name_off"].data_ptr(),
+                                           s["names"].data_ptr(), s["names"].numel(), self.stream.cuda_stream)
+        if rc != 0:
+            raise EngineError(rc, self.lib.c2v_last_error(None).decode())
+        s["ready"].record(self.stream)
+        return DeviceBatch(s, b, 0, b, 0, self)
+
+    def _run_eval(self, put) -> bool:
+        """One pass over the test file: every batch is the queue's next B rows, the last one what remains.  False when
+        the consumer has gone."""
+        n, k = 0, 0
+        chunks = self.reader._native_chunks_ahead()
+        try:
+            for i, chunk in enumerate(chunks):
+                n += self._append(chunk, i % 2)
+                while n >= self.B:
+                    batch = self._take(self.B, k)
+                    if batch is None or not put(batch):
+                        return False
+                    n, k = n - self.B, k + 1
+        finally:
+            chunks.close()
+        if n > 0:
+            batch = self._take(n, k)
+            if batch is None or not put(batch):
+                return False
+        return True
+
+    def score(self, batch: "DeviceBatch", ids) -> EvalScores:
+        """The metric kernel (c2v_reader_eval_score) on the top-k ids [rows, k] (int32, device) of an evaluation batch,
+        queued on the current stream; then the per-row results, the accumulators and the names are copied to the host
+        (the current stream is synchronised).  The ids come back too when a row is flagged."""
+        torch = self.torch
+        s = batch._slot
+        n, k = batch.hi - batch.lo, int(ids.shape[1])
+        r = s.get("res")
+        if r is None or r["acc"].numel() != k + 4:
+            r = {"rff": torch.empty((3, self.B), dtype=torch.int32, device=self.dev),
+                 "acc": torch.empty(k + 4, dtype=torch.int64, device=self.dev),
+                 "h_rff": torch.empty((3, self.B), dtype=torch.int32).pin_memory(),
+                 "h_acc": torch.empty(k + 4, dtype=torch.int64).pin_memory(),
+                 "h_off": torch.empty(self.B + 1, dtype=torch.int64).pin_memory()}
+            s["res"] = r
+        st = torch.cuda.current_stream(self.dev)
+        rff = r["rff"]
+        rc = self.lib.c2v_reader_eval_score(self.h, ids.data_ptr(), n, k, s["name_off"].data_ptr(), s["names"].data_ptr(),
+                                            rff[0].data_ptr(), rff[1].data_ptr(), rff[2].data_ptr(), r["acc"].data_ptr(),
+                                            st.cuda_stream)
+        if rc != 0:
+            raise EngineError(rc, self.lib.c2v_last_error(None).decode())
+        r["h_rff"][:, :n].copy_(rff[:, :n], non_blocking=True)
+        r["h_acc"].copy_(r["acc"], non_blocking=True)
+        r["h_off"][:n + 1].copy_(s["name_off"][:n + 1], non_blocking=True)
+        st.synchronize()
+        rff_h = r["h_rff"][:, :n].numpy().copy()
+        off = r["h_off"][:n + 1].numpy().copy()
+        names = s["names"][:int(off[n])].cpu().numpy().tobytes()
+        flagged = bool(rff_h[2].any())
+        return EvalScores(rff_h[0], rff_h[1], rff_h[2], r["h_acc"].numpy().copy(), (names, off),
+                          ids[:n].cpu().numpy() if flagged else None)
 
     # ---- sharded chunks ----------------------------------------------------------------------------------------------
     def _stage(self, j: int, rows: int):
@@ -424,6 +600,10 @@ class DeviceBatchReader:
 
         try:
             with self.torch.cuda.device(self.dev):
+                if self.evaluate:
+                    if self._run_eval(put):
+                        put(done)
+                    return
                 n, k = 0, 0
                 if self.transport is not None:
                     chunks = self.reader._native_chunk_ranges()
@@ -459,6 +639,13 @@ class DeviceBatchReader:
             put(exc)
 
     def __iter__(self):
+        if self._thread is not None and self.evaluate and not self._thread.is_alive():
+            # an evaluation reader reads the test file again: its queue is empty once a pass has ended
+            self._thread.join()
+            if self.lib.c2v_reader_eval_queued(self.h) != 0:
+                raise RuntimeError("the last evaluation pass stopped early; make a new DeviceBatchReader")
+            self._thread = None
+            self._stop.clear()
         if self._thread is not None:
             raise RuntimeError("a DeviceBatchReader reads one pass; make a new one for the next")
         q: "queue.Queue" = queue.Queue(maxsize=len(self.slots))
@@ -478,10 +665,15 @@ class DeviceBatchReader:
 
     # ---- life cycle --------------------------------------------------------------------------------------------------
     def device_bytes(self) -> int:
-        """Device memory the reader holds: vocabularies, batch slots, chunk text, this rank's stages (sharded) and the
-        handle's pool and scratch."""
-        n = sum(t.numel() * t.element_size() for t in self._vocab_tensors)
+        """Device memory the reader holds: vocabularies (shared with the model's other reader when given), batch slots
+        (with an evaluation batch's names and results), chunk text, this rank's stages (sharded) and the handle's pool,
+        scratch, evaluation queue and tables."""
+        n = self.vocabs.nbytes()
         n += sum(t.numel() * t.element_size() for s in self.slots for t in s["tensors"])
+        n += sum(t.numel() * t.element_size() for s in self.slots for key in ("name_off", "names") if key in s
+                 for t in (s[key],))
+        n += sum(t.numel() * t.element_size() for s in self.slots if "res" in s for key in ("rff", "acc")
+                 for t in (s["res"][key],))
         n += sum(b["dev"].numel() for b in self._text if b is not None)
         n += sum(s["bytes"] for s in self._stages if s is not None)
         return int(n + (self.lib.c2v_reader_device_bytes(self.h) if self.h else 0))

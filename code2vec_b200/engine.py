@@ -126,6 +126,12 @@ _SIGNATURES = {
     "c2v_reader_parse_share": (C.c_int, [_P, _P, C.c_int64, C.c_int64, _P, C.c_int64, C.POINTER(c2v_reader_share_status),
                                          _P]),
     "c2v_reader_commit_shares": (C.c_int, [_P, C.POINTER(_P), C.POINTER(C.c_int64), _I32, C.POINTER(C.c_int64), _P]),
+    "c2v_reader_eval_tables": (C.c_int, [_P, _I32, _P, _P, _P, _P, _P, _P]),
+    "c2v_reader_eval_append": (C.c_int, [_P, _P, C.c_int64, C.POINTER(C.c_int64), C.POINTER(C.c_int64),
+                                         C.POINTER(C.c_int64), C.POINTER(_I32), _P]),
+    "c2v_reader_eval_take": (C.c_int, [_P, _I32, _P, _P, _P, _P, _P, _P, _P, C.c_int64, _P]),
+    "c2v_reader_eval_queued": (C.c_int64, [_P]),
+    "c2v_reader_eval_score": (C.c_int, [_P, _P, _I32, _I32, _P, _P, _P, _P, _P, _P, _P]),
 }
 
 _lib = None

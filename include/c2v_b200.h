@@ -494,7 +494,8 @@ int c2v_reader_parse_chunk(c2v_reader* r, const char* text, int64_t nbytes, int6
 int c2v_reader_draw(c2v_reader* r, const int64_t* pick, int32_t b, int32_t lo, int32_t hi, int32_t* src, int32_t* path,
                     int32_t* tgt, float* mask, int32_t* target, void* stream);
 
-/* Rows in the pool once the queued calls have run (-1 for a NULL handle); device memory the handle holds. */
+/* Rows in the pool once the queued calls have run (-1 for a NULL handle); device memory the handle holds (pool, scratch,
+ * and the evaluation queue and tables). */
 int64_t c2v_reader_live_rows(const c2v_reader* r);
 size_t c2v_reader_device_bytes(const c2v_reader* r);
 
@@ -536,6 +537,53 @@ int c2v_reader_parse_share(c2v_reader* r, const char* text, int64_t nbytes, int6
  * returns) and sets *kept to the rows added. */
 int c2v_reader_commit_shares(c2v_reader* r, const void* const* stages, const int64_t* records, int32_t n_shares,
                              int64_t* kept, void* stream);
+
+/* ---- Evaluation on the device (DESIGN.md §6e) ----------------------------------------------------------------------
+ * A reader handle also reads `.c2v` test files: c2v_reader_eval_append parses a chunk in evaluate mode and appends the
+ * kept rows to an evaluation queue in file order, c2v_reader_eval_take hands out the next rows with their names, and
+ * c2v_reader_eval_score scores the engine's top-k ids of a batch against the names.  This is the host reader's evaluate
+ * path (path_context_reader.py _iterate_batches_native with c2v_parse_chunk mode 1) and the host metrics
+ * (common.get_first_match_word_from_top_predictions, SubtokensEvaluationMetric.update_batch) row for row.  The evaluation
+ * queue does not touch the training pool: a handle can serve both, but a reader of one kind is the usual use. */
+
+/* Uploads the per-target-word tables the evaluation needs, computed on the host from the target vocabulary (host
+ * memory; copied before the call returns): word i's bytes are words[word_off[i], word_off[i + 1]), its normalize_word
+ * bytes norm[norm_off[i], norm_off[i + 1]), and legal[i] != 0 when legal_method_names_checker accepts it.  n_words must
+ * cover the target vocabulary, its OOV word included: an empty name stands for that word.  Replaces earlier tables. */
+int c2v_reader_eval_tables(c2v_reader* r, int32_t n_words, const char* words, const int64_t* word_off, const char* norm,
+                           const int64_t* norm_off, const uint8_t* legal, void* stream);
+
+/* Parses the complete lines of text[0, nbytes) (device memory) with c2v_reader_parse_chunk's rules but the evaluate
+ * filter -- a record is kept when any of its contexts is valid, whatever its target -- and appends the kept rows, in
+ * file order, to the evaluation queue.  Each row keeps its name: field 0's bytes (commas included), or the target OOV
+ * word's when field 0 is empty.  Needs the tables (C2V_ERR_STATE otherwise).  Synchronises `stream`; *appended = the rows
+ * added, *name_bytes = the name bytes the queue holds now (a bound on the names of any take before the next append).
+ * Errors as c2v_reader_parse_chunk, with nothing appended. */
+int c2v_reader_eval_append(c2v_reader* r, const char* text, int64_t nbytes, int64_t* appended, int64_t* name_bytes,
+                           int64_t* bad_line, int32_t* bad_kind, void* stream);
+
+/* Moves the next b queued rows (1 <= b <= c2v_reader_eval_queued) into src / path / tgt / mask [b, max_contexts] and
+ * target [b] (device memory), and their names into names (device memory of names_cap bytes, at least the *name_bytes
+ * the last append reported) with row j's name at names[name_off[j], name_off[j + 1]) (name_off: device, [b + 1]).
+ * Asynchronous on `stream`. */
+int c2v_reader_eval_take(c2v_reader* r, int32_t b, int32_t* src, int32_t* path, int32_t* tgt, float* mask,
+                         int32_t* target, int64_t* name_off, char* names, int64_t names_cap, void* stream);
+
+/* Rows queued and not yet taken (-1 for a NULL handle). */
+int64_t c2v_reader_eval_queued(const c2v_reader* r);
+
+/* Scores n rows: ids [n, k] (device; the engine's top-k word ids, best first) against the names
+ * names[name_off[j], name_off[j + 1]) (device, as c2v_reader_eval_take writes them).  Per row (device outputs [n]):
+ * rank[j] = the rank of the first word whose normalize_word equals the name's among the legal words of the top-k (not
+ * among all k), or -1; first[j] = the id of the first legal word, or -1; flags[j] = 1 when the name has a byte >= 0x80
+ * (the host scores it: normalize_word and the UTF-8 decoding are Unicode), 2 when no word of the top-k is legal (the host
+ * raises, as the host metric does), else 0.  acc (device int64 [k + 4], zeroed here) sums the unflagged rows: a histogram
+ * of their ranks over [0, k), then their number, and the subtoken true positives, false positives and false negatives of
+ * the first legal word against the name ('|'-separated, empty subtokens included, multiset counts).  Integer sums: the
+ * result does not depend on the order rows are added.  Only reads the handle's tables, so it may run on another host
+ * thread than append / take.  Asynchronous on `stream`. */
+int c2v_reader_eval_score(const c2v_reader* r, const int32_t* ids, int32_t n, int32_t k, const int64_t* name_off,
+                          const char* names, int32_t* rank, int32_t* first, int32_t* flags, int64_t* acc, void* stream);
 
 #ifdef __cplusplus
 }
