@@ -34,6 +34,7 @@ from .multi_rank import (CKPT_MAGIC, CKPT_SUFFIX, batch_split, check_checkpoint_
                          write_checkpoint, write_checkpoint_part)
 from . import device_reader as _device_reader_mod
 from .device_reader import device_eval_flag, device_reader_flag, sharded_reader_flag
+from .text_export import DeviceTextWriter, device_text_flag
 from .trainer import Trainer, make_fully_sharded_engine
 from .vocabularies import VocabType
 
@@ -157,6 +158,8 @@ class Code2VecModel(Code2VecModelBase):
         if self._device_eval and config.DL_FRAMEWORK == "b200-keras":
             raise ValueError("C2V_DEVICE_EVAL=1 is not available with --framework b200-keras: its evaluation has its own "
                              "metrics and loss on the host; unset C2V_DEVICE_EVAL or evaluate with --framework b200")
+        # C2V_DEVICE_TEXT=1: `.vectors` and word2vec files are formatted on the GPU (text_export.py, DESIGN.md §6f)
+        self._device_text = device_text_flag(os.environ)
         self._device_vocabs = None               # device_reader.DeviceVocabs, shared by the training and evaluation readers
         self._eval_tables = None                 # device_reader.eval_tables of the target vocabulary
         self._dev_eval_reader = None
@@ -256,6 +259,8 @@ class Code2VecModel(Code2VecModelBase):
         self.log("b200 backend evaluation: %s (C2V_DEVICE_EVAL=%d)" % (
             "read, predicted and scored on the GPU" if self._device_eval else "read and scored on the host",
             self._device_eval))
+        self.log("b200 backend text export: `.vectors` and word2vec files formatted %s (C2V_DEVICE_TEXT=%d)" % (
+            "on the GPU" if self._device_text else "on the host", self._device_text))
         if self.world > 1:
             # every multi-GPU run, evaluate-only ones too: the row shards and Trainer.predict live in the Trainer.
             # C2V_DETERMINISTIC=1 sends the embedding gradients through the ordered exchange (DESIGN.md §5.1)
@@ -592,7 +597,7 @@ class Code2VecModel(Code2VecModelBase):
         total_predictions, total_batches = 0, 0
         # several GPUs: every rank predicts its slice of each batch, rank 0 gathers the rows and writes every file
         writer = self.rank == 0
-        code_vectors_file = open(cfg.TEST_DATA_PATH + ".vectors", "w") if cfg.EXPORT_CODE_VECTORS and writer else None
+        code_vectors_file, text = self._open_code_vectors(writer)
         with (open("log.txt", "w") if writer else contextlib.nullcontext()) as log_output_file:
             start_time = time.time()
             self.log("Starting evaluation")
@@ -614,14 +619,14 @@ class Code2VecModel(Code2VecModelBase):
                 total_predictions += len(original_names)
                 total_batches += 1
                 if code_vectors_file is not None:
-                    self._write_code_vectors(code_vectors_file, code_vectors)
+                    self._export_code_vectors(code_vectors_file, text, code_vectors)
                 if total_batches % cfg.NUM_BATCHES_TO_LOG_PROGRESS == 0:
                     self._trace_evaluation(total_predictions, time.time() - start_time)
             self.log("Done evaluating, epoch reached")
             if writer:
                 log_output_file.write(str(topk_metric.topk_correct_predictions) + "\n")
         if code_vectors_file is not None:
-            code_vectors_file.close()
+            self._close_code_vectors(code_vectors_file, text)
         elapsed = int(time.time() - eval_start_time)
         self.log("Evaluation time: %sH:%sM:%sS" % ((elapsed // 60 // 60), (elapsed // 60) % 60, elapsed % 60))
         results = None
@@ -671,7 +676,7 @@ class Code2VecModel(Code2VecModelBase):
         total_predictions, total_batches = 0, 0
         writer = self.rank == 0
         reader = self._device_eval_reader()
-        code_vectors_file = open(cfg.TEST_DATA_PATH + ".vectors", "w") if cfg.EXPORT_CODE_VECTORS and writer else None
+        code_vectors_file, text = self._open_code_vectors(writer)
         try:
             with (open("log.txt", "w") if writer else contextlib.nullcontext()) as log_output_file:
                 start_time = time.time()
@@ -686,7 +691,8 @@ class Code2VecModel(Code2VecModelBase):
                         ids, _ = self.engine.topk(code, normalize=False)
                     if writer:
                         sc = reader.score(batch, ids)              # synchronises the current stream
-                        code_vectors = code.cpu().numpy() if code_vectors_file is not None else None
+                        if code_vectors_file is not None:
+                            code_vectors = code if text is not None else code.cpu().numpy()
                     batch.release()
                     total_predictions += n
                     total_batches += 1
@@ -697,7 +703,7 @@ class Code2VecModel(Code2VecModelBase):
                         self._log_and_score_host_rows(sc, n, index_to_word, log_output_file, subtokens_metric,
                                                       topk_metric)
                         if code_vectors_file is not None:
-                            self._write_code_vectors(code_vectors_file, code_vectors)
+                            self._export_code_vectors(code_vectors_file, text, code_vectors)
                     if total_batches % cfg.NUM_BATCHES_TO_LOG_PROGRESS == 0:
                         self._trace_evaluation(total_predictions, time.time() - start_time)
                 self.log("Done evaluating, epoch reached")
@@ -715,7 +721,7 @@ class Code2VecModel(Code2VecModelBase):
             raise
         finally:
             if code_vectors_file is not None:
-                code_vectors_file.close()
+                self._close_code_vectors(code_vectors_file, text)
         self.log("Device evaluation: %.1f MB of text uploaded, %.1f MB of device memory held" % (
             reader.h2d_bytes / 1e6, reader.device_bytes() / 1e6))
         elapsed = int(time.time() - eval_start_time)
@@ -731,6 +737,36 @@ class Code2VecModel(Code2VecModelBase):
             dist.all_gather_object(gathered, results)
             results = gathered[0]
         return results
+
+    # ---- `.vectors` and word2vec files (C2V_DEVICE_TEXT=1 formats them on the GPU, DESIGN.md §6f) ----------------------
+    def _open_code_vectors(self, writer: bool):
+        """(`<test file>.vectors` opened for this evaluation, or None when it exports none or is not the writing rank;
+        with C2V_DEVICE_TEXT=1 the DeviceTextWriter that fills it, else None)."""
+        cfg = self.config
+        if not (cfg.EXPORT_CODE_VECTORS and writer):
+            return None, None
+        if not self._device_text:
+            return open(cfg.TEST_DATA_PATH + ".vectors", "w"), None
+        f = open(cfg.TEST_DATA_PATH + ".vectors", "wb")
+        return f, DeviceTextWriter(f, self.engine.dev)
+
+    def _export_code_vectors(self, file, text: Optional[DeviceTextWriter], code_vectors):
+        """One batch's lines of the `.vectors` file: _write_code_vectors, or formatted on the GPU from the device tensor
+        (a host array is uploaded again)."""
+        if text is None:
+            self._write_code_vectors(file, code_vectors)
+            return
+        import torch
+        text.write_rows(code_vectors if isinstance(code_vectors, torch.Tensor) else
+                        self.engine.to_device(code_vectors, torch.float32))
+
+    def _close_code_vectors(self, file, text: Optional[DeviceTextWriter]):
+        try:
+            if text is not None:
+                text.close()
+                self.log("Device text: %s" % text.report())
+        finally:
+            file.close()
 
     def _log_and_score_host_rows(self, sc, n: int, index_to_word, output_file, subtokens_metric, topk_metric):
         """log.txt lines of one scored batch, in row order: the three line forms of _log_predictions_during_evaluation
@@ -830,14 +866,18 @@ class Code2VecModel(Code2VecModelBase):
 
     def _get_vocab_embedding_as_np_array(self, vocab_type: VocabType) -> np.ndarray:
         assert vocab_type in VocabType
+        return self._vocab_embedding_on_device(vocab_type).cpu().numpy()
+
+    def _vocab_embedding_on_device(self, vocab_type: VocabType):
+        """The whole table of `vocab_type` as a device tensor; on several GPUs gathered on every rank (a collective)."""
         if self.world > 1:
             return self._gather_table(self._param_of_vocab[vocab_type])
         self.engine.sync_tables()
-        return self.engine.params[self._param_of_vocab[vocab_type]].detach().cpu().numpy()
+        return self.engine.params[self._param_of_vocab[vocab_type]].detach()
 
-    def _gather_table(self, name: str) -> np.ndarray:
-        """The whole table `name` on every rank (a collective): the embedding shards all-gathered and interleaved back
-        (global row = local row * world + rank), or the target blocks all-gathered and concatenated."""
+    def _gather_table(self, name: str):
+        """The whole table `name` on every rank (a collective), in device memory: the embedding shards all-gathered and
+        interleaved back (global row = local row * world + rank), or the target blocks all-gathered and concatenated."""
         import torch
         import torch.distributed as dist
         e, W = self.engine, self.world
@@ -846,19 +886,28 @@ class Code2VecModel(Code2VecModelBase):
             whole = torch.empty((W,) + tuple(shard.shape), dtype=shard.dtype, device=e.dev)
             dist.all_gather_into_tensor(whole, shard)
             n_rows = self._engine_dims().shapes()[name][0]
-            return whole.transpose(0, 1).reshape(-1, shard.shape[1])[:n_rows].cpu().numpy()
+            return whole.transpose(0, 1).reshape(-1, shard.shape[1])[:n_rows]
         Y, per = e.global_target_vocab, -(-e.global_target_vocab // W)     # blocks of `per` rows, the last one shorter
         block = torch.zeros((per, e.dims.code_dim), dtype=torch.float32, device=e.dev)
         block[:e.dims.target_vocab].copy_(e.params["tgt"])
         whole = torch.empty((W * per, e.dims.code_dim), dtype=torch.float32, device=e.dev)
         dist.all_gather_into_tensor(whole, block)
-        return whole[:Y].cpu().numpy()
+        return whole[:Y]
 
     def save_word2vec_format(self, dest_save_path: str, vocab_type: VocabType):
         if self.world > 1 and self.rank != 0:
-            self._get_vocab_embedding_as_np_array(vocab_type)        # the gather is a collective; rank 0 writes the file
+            self._vocab_embedding_on_device(vocab_type)              # the gather is a collective; rank 0 writes the file
             return
-        super().save_word2vec_format(dest_save_path, vocab_type)
+        if not self._device_text:
+            return super().save_word2vec_format(dest_save_path, vocab_type)
+        if vocab_type not in VocabType:
+            raise ValueError("`vocab_type` should be `VocabType.Token`, `VocabType.Target` or `VocabType.Path`.")
+        from . import text_export
+        vocab = self.vocabs.get(vocab_type)
+        table = self._vocab_embedding_on_device(vocab_type)
+        with open(dest_save_path, "w") as out:
+            text = text_export.save_word2vec_file(out, vocab.index_to_word, table)
+        self.log("Device text: %s" % text.report())
 
     # ---- logging helpers (tensorflow_model.py:411-437) ------------------------------------------------------
     def _log_predictions_during_evaluation(self, results, output_file):

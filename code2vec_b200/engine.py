@@ -132,6 +132,10 @@ _SIGNATURES = {
     "c2v_reader_eval_take": (C.c_int, [_P, _I32, _P, _P, _P, _P, _P, _P, _P, C.c_int64, _P]),
     "c2v_reader_eval_queued": (C.c_int64, [_P]),
     "c2v_reader_eval_score": (C.c_int, [_P, _P, _I32, _I32, _P, _P, _P, _P, _P, _P, _P]),
+    # text of float32 matrices (text_export.py)
+    "c2v_text_format_rows": (C.c_int, [_P, C.c_int64, _I32, C.c_int64, _P, _P, _P, C.c_size_t, _P, C.c_int64, _P, _P,
+                                       _P]),
+    "c2v_selftest_format_floats": (C.c_int, [_P, C.c_int64, _P, _P]),
 }
 
 _lib = None

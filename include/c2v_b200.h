@@ -585,6 +585,30 @@ int64_t c2v_reader_eval_queued(const c2v_reader* r);
 int c2v_reader_eval_score(const c2v_reader* r, const int32_t* ids, int32_t n, int32_t k, const int64_t* name_off,
                           const char* names, int32_t* rank, int32_t* first, int32_t* flags, int64_t* acc, void* stream);
 
+/* ---- Text of float32 matrices (DESIGN.md §6f) -----------------------------------------------------------------------
+ * The lines of `<test file>.vectors` (model_base._write_code_vectors) and of word2vec files (common.save_word2vec_file),
+ * formatted on the device.  Every value is written as numpy's str(np.float32(x)) writes it: "nan", "inf", "-inf",
+ * "0.0", "-0.0"; positional ("0.5", "999999.0", "0.000100000005") for 1e-4 <= |x| < 1e6, compared exactly; otherwise
+ * scientific ("1e+07", "1.5e+08", "1.1754944e-38"); digits of Dragon4 in numpy's "unique" mode.  No engine handle is
+ * needed; failures return a negative c2v_status with the message in c2v_last_error(NULL). */
+
+/* Bytes one value's text and the separator after it take at most (a value is at most 15 bytes long). */
+#define C2V_TEXT_VALUE_BYTES 16
+
+/* Formats rows [0, rows) of the row-major float32 matrix x (device; row r at x + r * ld, cols values) as lines: row r's
+ * prefix bytes prefix[prefix_off[r], prefix_off[r + 1]) (device; both NULL for no prefix), then its values joined by
+ * single spaces, then '\n'.  stage (device, stage_bytes >= rows * cols * C2V_TEXT_VALUE_BYTES) is scratch.  row_end
+ * (device, [rows]) receives each line's end offset in out, lines back to back from out[0]; *rows_done (device) = the
+ * lines that end within out_cap bytes, which are written to out (device); the others are left for the next call.
+ * Asynchronous on `stream`. */
+int c2v_text_format_rows(const float* x, int64_t rows, int32_t cols, int64_t ld, const char* prefix,
+                         const int64_t* prefix_off, void* stage, size_t stage_bytes, char* out, int64_t out_cap,
+                         int64_t* row_end, int64_t* rows_done, void* stream);
+
+/* Test hook: formats x[0, n) (host) on the CPU with the function the device runs.  Value i's text goes to
+ * out[i * C2V_TEXT_VALUE_BYTES, ...) followed by NUL bytes up to the next value, and its length to len[i] (host). */
+int c2v_selftest_format_floats(const float* x, int64_t n, char* out, int32_t* len);
+
 #ifdef __cplusplus
 }
 #endif
