@@ -614,15 +614,15 @@ int transpose_operand(c2v_engine* e, cudaStream_t st, const float* x, int rows, 
   return C2V_OK;
 }
 
-// Ytab^T for dv, from the current target table (every row must be current: callers run end_target_lazy first).  3xTF32: as
-// its transposed split, and with with_split also the untransposed split into tgt_hi / tgt_lo that the logits GEMM reads.
-int transpose_table(c2v_engine* e, cudaStream_t st, bool with_split) {
+// Ytab^T for dv, from the current target table (every row must be current: callers run end_target_lazy first); 3xTF32: as
+// its transposed split.  A training step's logits GEMM writes it from its B tiles (launch_logits, for_dv); this pass is for
+// a dv that no such logits pass preceded.
+int transpose_table(c2v_engine* e, cudaStream_t st) {
   const int Y = e->dims.target_vocab, D = e->dims.code_dim;
   int rc;
   if (is_3x(e)) {
     PhaseTimer pt(e, PH_SPLIT, st);
-    rc = transpose_operand(e, st, e->theta.tgt, Y, D, e->ws.ldS, e->ws.tgtT, true, e->ws.tgtT_lo,
-                           with_split ? wsp<float>(e, e->ws.tgt_hi) : nullptr, with_split ? wsp<float>(e, e->ws.tgt_lo) : nullptr);
+    rc = transpose_operand(e, st, e->theta.tgt, Y, D, e->ws.ldS, e->ws.tgtT, true, e->ws.tgtT_lo);
   } else {
     PhaseTimer pt(e, PH_DV, st);
     rc = transpose_operand(e, st, e->theta.tgt, Y, D, e->ws.ldS, e->ws.tgtT, false);
@@ -885,7 +885,8 @@ inline TopkCandidates topk_candidates(c2v_engine* e, int B, int k) {
   return {S, reinterpret_cast<int32_t*>(S + (size_t)B * umma::lse_slots(e->dims.target_vocab) * k)};
 }
 
-// for_dv: a dv GEMM of this step follows, so Ytab^T is made here (transpose_table), before the GEMM and from the same table
+// for_dv: a dv GEMM of this step follows, so the GEMM also writes Ytab^T (3xTF32: its transposed split) from the Ytab tiles it
+// streams, from the same table (umma::BTransposed).  Only the first logits pass of a step, whose epilogues take go_dv, does.
 template <bool X3>
 int launch_logits(c2v_engine* e, cudaStream_t st, const float* v, int B, LogitsOut out, const LogitsArgs& a, bool for_dv) {
   const int D = e->dims.code_dim, Y = e->dims.target_vocab;
@@ -895,14 +896,10 @@ int launch_logits(c2v_engine* e, cudaStream_t st, const float* v, int B, LogitsO
   if (X3) {      // fp32-faithful: both operands as tf32 (hi, lo) pairs; the gated fallback reuses the previous pass's splits
     if (out != LOGITS_STORE_LSE_GATED) {
       if ((rcs = split_small(e, st, v, (size_t)B * D, e->ws.v_hi, e->ws.v_lo))) return rcs;
-      if (for_dv) rcs = transpose_table(e, st, true);
-      else rcs = split_small(e, st, e->theta.tgt, (size_t)Y * D, e->ws.tgt_hi, e->ws.tgt_lo);
-      if (rcs) return rcs;
+      if ((rcs = split_small(e, st, e->theta.tgt, (size_t)Y * D, e->ws.tgt_hi, e->ws.tgt_lo))) return rcs;
     }
     opA.base = wsp<float>(e, e->ws.v_hi); opA.lo = wsp<float>(e, e->ws.v_lo);
     opB.base = wsp<float>(e, e->ws.tgt_hi); opB.lo = wsp<float>(e, e->ws.tgt_lo);
-  } else if (for_dv && (rcs = transpose_table(e, st, false))) {
-    return rcs;
   }
   PhaseTimer pt(e, PH_LOGITS, st);
   float* S = wsp<float>(e, e->ws.S);
@@ -913,13 +910,21 @@ int launch_logits(c2v_engine* e, cudaStream_t st, const float* v, int B, LogitsO
     C2V_LAUNCH(e, C2V_CUDA(e, (umma::launch_cfg<false, false, decltype(ep)>(st, B, Y, D, 1, opA, opB, ep, e->num_sms))));
     return C2V_OK;
   };
+  auto go_dv = [&](auto ep) -> int {
+    if (!for_dv) return go(ep);
+    const umma::BTransposed bt{wsp<float>(e, e->ws.tgtT), X3 ? wsp<float>(e, e->ws.tgtT_lo) : nullptr, e->ws.ldS};
+    C2V_LAUNCH(e, C2V_CUDA(e, (umma::launch_cfg<false, false, decltype(ep), umma::AXNone, true>(st, B, Y, D, 1, opA, opB, ep, e->num_sms,
+                                                                                                umma::AXNone{}, bt))));
+    e->tgt_t_valid = true;
+    return C2V_OK;
+  };
   switch (out) {
-    case LOGITS_STORE: return go(umma::EpiStore{S, ld, 0});
-    case LOGITS_STORE_LSE: return go(lse);
-    case LOGITS_LSE_ONLY: return go(umma::EpiLseOnlyT<X3>{lse});
+    case LOGITS_STORE: return go_dv(umma::EpiStore{S, ld, 0});
+    case LOGITS_STORE_LSE: return go_dv(lse);
+    case LOGITS_LSE_ONLY: return go_dv(umma::EpiLseOnlyT<X3>{lse});
     case LOGITS_SOFTMAX_GRAD:
       return go(umma::EpiSoftmaxGradT<X3, X3>{S, S_lo, ld, a.sg.lse, a.sg.target, a.sg.row0, a.sg.inv_batch, B});
-    case LOGITS_EXP_SUM: return go(umma::EpiExpSumT<X3, X3>{S, S_lo, ld, a.exp_offset, lse.partial, lse.slots});
+    case LOGITS_EXP_SUM: return go_dv(umma::EpiExpSumT<X3, X3>{S, S_lo, ld, a.exp_offset, lse.partial, lse.slots});
     case LOGITS_STORE_LSE_GATED: return go(umma::EpiStoreLseGatedT<X3>{lse, a.gate});
     case LOGITS_TOPK:
     case LOGITS_TOPK_LSE: {
@@ -1159,7 +1164,7 @@ int run_dv(c2v_engine* e, cudaStream_t st, int B, float* dv, const SlabDesc& sla
   if (is_tc(e)) {
     // B = Ytab^T, K-major, made by this step's logits pass (3xTF32: as the table's split; P was written as its split by
     // softmax_grad_kernel)
-    if (!e->tgt_t_valid) { int rct = transpose_table(e, st, false); if (rct) return rct; }
+    if (!e->tgt_t_valid) { int rct = transpose_table(e, st); if (rct) return rct; }
     umma::Operand opA{S, e->ws.ldS, false};
     umma::Operand opB{wsp<float>(e, e->ws.tgtT), e->ws.ldS, false};
     if (is_3x(e)) {
@@ -2332,6 +2337,19 @@ int c2v_selftest_gemm3(c2v_engine* e, int32_t a_mn, int32_t b_mn, int32_t bn, in
   return umma::effective_splits(K, splits);
 }
 
+int c2v_selftest_gemm_bt(c2v_engine* e, int32_t M, int32_t N, int32_t K, const float* A, size_t lda, const float* Bm, size_t ldb,
+                         float* C, size_t ldc, float* BT, size_t ldbt, void* stream) {
+  if (!e || !A || !Bm || !C || !BT) return C2V_ERR_INVALID;
+  C2V_CUDA(e, cudaSetDevice(e->device));
+  const umma::Operand opA{A, lda, false}, opB{Bm, ldb, false};
+  if (!umma::operand_ok(opA) || !umma::operand_ok(opB)) return fail(e, C2V_ERR_INVALID, "operand not TMA-compatible");
+  const umma::EpiStore ep{C, ldc, 0};
+  C2V_LAUNCH(e, C2V_CUDA(e, (umma::launch_cfg<false, false, umma::EpiStore, umma::AXNone, true>((cudaStream_t)stream, M, N, K, 1, opA, opB,
+                                                                                                ep, e->num_sms, umma::AXNone{},
+                                                                                                umma::BTransposed{BT, nullptr, ldbt}))));
+  return C2V_OK;
+}
+
 int c2v_selftest_split(c2v_engine* e, const float* x, float* hi, float* lo, size_t count, void* stream) {
   if (!e || !x || !hi || !lo) return C2V_ERR_INVALID;
   if (count % 4 || ((uintptr_t)x | (uintptr_t)hi | (uintptr_t)lo) % 16) return fail(e, C2V_ERR_INVALID, "count % 4 and 16-byte alignment");
@@ -2352,6 +2370,13 @@ int c2v_selftest_transpose(c2v_engine* e, const float* x, int32_t rows, int32_t 
   cudaStream_t st = (cudaStream_t)stream;
   if (xT_lo) C2V_LAUNCH(e, (transpose_kernel<true><<<grid, 256, 0, st>>>(x, rows, cols, xT, xT_lo, ldT, nullptr, nullptr)));
   else C2V_LAUNCH(e, (transpose_kernel<false><<<grid, 256, 0, st>>>(x, rows, cols, xT, nullptr, ldT, nullptr, nullptr)));
+  return C2V_OK;
+}
+
+int c2v_selftest_target_t(const c2v_engine* e, int32_t lo, size_t* offset, size_t* ld) {
+  if (!e || !offset || !ld) return C2V_ERR_INVALID;
+  *offset = lo ? e->ws.tgtT_lo : e->ws.tgtT;
+  *ld = e->ws.ldS;
   return C2V_OK;
 }
 

@@ -8,6 +8,7 @@
 //                     the four producer warps then transpose in place (transpose_box); the loads of the next
 //                     steps stay in flight meanwhile.  An A-operand policy (AX*) may instead compute the A
 //                     tile (softmax gradient of a logits tile, embedding gather).
+//                     With B_T (the logits GEMM), warps 1-3 also write each B tile out transposed (store_b_transposed).
 //   warpgroups 1, 2 : consumers -- each owns 64 rows of the 128-row tile and issues
 //                     wgmma.mma_async m64n128k8 (tf32) into a 64-register accumulator per thread;
 //                     then writes the accumulator to its shared-memory staging blocks and goes on to its
@@ -736,6 +737,50 @@ __device__ __forceinline__ void transpose_box(uint8_t* box, int lane, const F& f
                  "f"(v[4 * c + 3]) : "memory");
 }
 
+// Where a GEMM with B_T writes its B operand's K-major transpose [K, ld] (element (n, k) at hi[k * ld + n]; 3xTF32: the
+// transposed high parts to hi and the residuals to lo): the logits GEMM makes Ytab^T for dv from the Ytab tiles it streams
+// anyway, instead of a separate pass that reads the table again.
+struct BTransposed {
+  float* hi;
+  float* lo;
+  size_t ld;
+};
+
+// The B tile of a full stage (rows n0 .. n0+127, k0 .. k0+31; chunk c of row r at (c ^ (r & 7)) * 16) to dst[k * ld + n] for
+// n < N, k < K (K % 4 == 0: a chunk lies wholly inside K or outside it).  Copying warp cw in [0, 3) takes chunks cw, cw + 3,
+// ...; lane l rows 4l .. 4l+3, so each of a chunk's four float4 stores writes 512 consecutive bytes of one row of dst.  At
+// step j lane l reads row 4l + (j ^ s), s = (l >> 1) & 3: the 8 lanes of a quarter-warp then read rows that differ in
+// (r & 7), i.e. 8 distinct 16-byte bank groups, and two conditional swaps put the four rows back in order.  The stores
+// stream (evict-first): dst is read by a later GEMM, and L2 is better spent on the B tiles the other m-tiles still read.
+__device__ __forceinline__ void store_b_transposed(const uint8_t* sb, float* dst, size_t ld, int n0, int N, int k0, int K, int cw,
+                                                   int lane) {
+  const int s = (lane >> 1) & 3, n = n0 + 4 * lane;
+#pragma unroll 1
+  for (int c = cw; c < BK / 4 && k0 + 4 * c < K; c += 3) {
+    float4 v[4];
+#pragma unroll
+    for (int j = 0; j < 4; ++j) {
+      const int r = 4 * lane + (j ^ s);
+      v[j] = *reinterpret_cast<const float4*>(sb + r * 128 + ((c ^ (r & 7)) << 4));
+    }
+    if (s & 1) { const float4 t0 = v[0], t2 = v[2]; v[0] = v[1]; v[1] = t0; v[2] = v[3]; v[3] = t2; }
+    if (s & 2) { const float4 t0 = v[0], t1 = v[1]; v[0] = v[2]; v[1] = v[3]; v[2] = t0; v[3] = t1; }
+    const float4 o[4] = {make_float4(v[0].x, v[1].x, v[2].x, v[3].x), make_float4(v[0].y, v[1].y, v[2].y, v[3].y),
+                         make_float4(v[0].z, v[1].z, v[2].z, v[3].z), make_float4(v[0].w, v[1].w, v[2].w, v[3].w)};
+    float* p = dst + (size_t)(k0 + 4 * c) * ld + n;
+#pragma unroll
+    for (int i = 0; i < 4; ++i, p += ld) {
+      if (n + 3 < N) {
+        __stcs(reinterpret_cast<float4*>(p), o[i]);
+      } else {          // the last n-tile: columns n >= N are TMA's zero fill, and dst's padding there stays as it is
+        if (n < N) __stcs(p, o[i].x);
+        if (n + 1 < N) __stcs(p + 1, o[i].y);
+        if (n + 2 < N) __stcs(p + 2, o[i].z);
+      }
+    }
+  }
+}
+
 // gather(cs)[m0 .. m0+127, k-block kb] with dropout, as load_tile_k lays it out (d % 32 == 0: a k-block lies in one
 // of the three segments source token | path | target token)
 __device__ __forceinline__ void load_tile_gather(uint8_t* dst, const AXGather& g, int m0, int M, int kb, bool write_x, int t) {
@@ -790,16 +835,19 @@ struct SmemLayout {
   static_assert(kTotal <= 232448, "exceeds the 227 KB of shared memory a CTA can opt into");
 };
 
-template <bool A_MN, bool B_MN, class Epi, class AX = AXNone>
+// B_T: the GEMM also writes its B operand transposed to bt (store_b_transposed) -- each B tile once, from a stage that holds
+// it for the product anyway.
+template <bool A_MN, bool B_MN, class Epi, class AX = AXNone, bool B_T = false>
 __global__ void __launch_bounds__(kThreads, 1)
 umma_gemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB,
                  const __grid_constant__ CUtensorMap tmAlo, const __grid_constant__ CUtensorMap tmBlo, GemmShape gs,
-                 GemmPtrs ptr, Epi epi, AX ax = AX{}) {
+                 GemmPtrs ptr, Epi epi, AX ax = AX{}, BTransposed bt = {}) {
   if (epi_gate_closed(epi, 0)) return;      // gated fallback pass: nothing to do (uniform over the grid)
   using L = SmemLayout;
   static_assert(!(A_MN && AX::kKind == 2), "the gathered A tile is K-major");
   constexpr bool kTmaA = !A_MN && AX::kKind == 0;     // K-major tiles TMA writes as wgmma reads them
   constexpr bool kTmaB = !B_MN;
+  static_assert(!B_T || (kTmaA && kTmaB), "the B tile is copied out of all-K-major TMA stages");
   constexpr uint32_t kTxBytes = (kTmaA ? L::kABytes : 0) + (kTmaB ? L::kBBytes : 0);
   constexpr uint32_t kMnTxBytes = (A_MN ? L::kABytes : 0) + (B_MN ? L::kBBytes : 0);    // MN-major tiles, transposed after landing
   // How many steps the producer's TMA loads run ahead of the step it completes (transposes and publishes).  The
@@ -820,7 +868,12 @@ umma_gemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant_
   const int total_kblocks = (gs.K + BK - 1) / BK;
 
   if (threadIdx.x == 0) {
-    for (int s = 0; s < STAGES; ++s) { mbar_init(&full_bar[s], 128); mbar_init(&empty_bar[s], 8); mbar_init(&landed_bar[s], 1); }
+    // B_T: producer warp 0 alone publishes a stage, and warps 1-3 release it like three more consumer warps
+    for (int s = 0; s < STAGES; ++s) {
+      mbar_init(&full_bar[s], B_T ? 32 : 128);
+      mbar_init(&empty_bar[s], B_T ? 8 + 3 : 8);
+      mbar_init(&landed_bar[s], 1);
+    }
     mbar_init(epi_full, 256);
     mbar_init(epi_empty, 128);
     asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
@@ -927,7 +980,26 @@ umma_gemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant_
     };
     Cursor ld{static_cast<int>(blockIdx.x), 0, 0, 0, 0, 0, 0, 0, 0u};
     seek(ld);
-    if constexpr (kLag == 0) {
+    if constexpr (B_T) {
+      if (warp == 0) {          // the loads, never held up by the copy
+        for (; ld.item < total_items; next(ld)) { issue(ld); complete(ld); }
+      } else {
+        // warps 1-3 walk the same steps: wait for the stage, copy its B tile out if this m-tile is the one that copies it
+        // (3xTF32: B_lo of pass 1 to bt.lo, B_hi of pass 2 to bt.hi; pass 0 reads B_hi too), then release it -- in every
+        // step, so that empty_bar's count holds whichever item a stage belongs to.  K block kb of n-tile nt is copied by
+        // m-tile (nt + kb) % m_tiles: every work item, and so every CTA, copies its share of the blocks.  (Copying all of
+        // them in m-tile 0 loaded the copy onto the quarter of the CTAs that run m-tile 0 items, and cost the logits GEMM
+        // of the java14m step as much time as the separate pass it replaced.)
+        for (; ld.item < total_items; next(ld)) {
+          mbar_wait(&full_bar[ld.stage], ld.phase);
+          if (ld.pass > 0 && (ld.nt + ld.kb) % gs.m_tiles == ld.mt)
+            store_b_transposed(smem + ld.stage * L::kStageBytes + L::kABytes, ld.pass == 2 ? bt.hi : bt.lo, bt.ld, ld.nt * BN,
+                               gs.N, ld.kb * BK, gs.K, warp - 1, lane);
+          __syncwarp();
+          if (lane == 0) mbar_arrive(&empty_bar[ld.stage]);
+        }
+      }
+    } else if constexpr (kLag == 0) {
       // all-K-major: one cursor (the lagging loop below, run with kLag = 0, was 10-19% slower on these GEMMs on an H100)
       for (; ld.item < total_items; next(ld)) { issue(ld); complete(ld); }
     } else {
@@ -1130,26 +1202,31 @@ inline GemmShape make_shape(int M, int N, int K, int splits, int terms) {
   return gs;
 }
 
-template <bool A_MN, bool B_MN, class Epi, class AX>
+template <bool A_MN, bool B_MN, class Epi, class AX, bool B_T = false>
 inline cudaError_t launch_kernel(cudaStream_t st, const CUtensorMap& tmA, const CUtensorMap& tmB, const CUtensorMap& tmAlo,
                                  const CUtensorMap& tmBlo, const GemmShape& gs, const GemmPtrs& ptr, const Epi& epi, int num_sms,
-                                 const AX& ax) {
-  auto kern = umma_gemm_kernel<A_MN, B_MN, Epi, AX>;
+                                 const AX& ax, const BTransposed& bt = {}) {
+  auto kern = umma_gemm_kernel<A_MN, B_MN, Epi, AX, B_T>;
   cudaError_t e = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, SmemLayout::kTotal);
   if (e != cudaSuccess) return e;
   int grid = gs.m_tiles * gs.n_tiles * gs.splits;
   if (grid > num_sms) grid = num_sms;
-  kern<<<grid, kThreads, SmemLayout::kTotal, st>>>(tmA, tmB, tmAlo, tmBlo, gs, ptr, epi, ax);
+  kern<<<grid, kThreads, SmemLayout::kTotal, st>>>(tmA, tmB, tmAlo, tmBlo, gs, ptr, epi, ax, bt);
   return cudaGetLastError();
 }
 
-template <bool A_MN, bool B_MN, class Epi, class AX = AXNone>
+// B_T: B^T [K, bt.ld] is written to bt as well (umma_gemm_kernel); bt.ld >= N, both 16-byte aligned with a pitch of a
+// multiple of 4 floats, K % 4 == 0.
+template <bool A_MN, bool B_MN, class Epi, class AX = AXNone, bool B_T = false>
 inline cudaError_t launch_cfg(cudaStream_t st, int M, int N, int K, int splits, const Operand& A, const Operand& B, const Epi& epi,
-                              int num_sms, const AX& ax = AX{}) {
+                              int num_sms, const AX& ax = AX{}, const BTransposed& bt = {}) {
   CUtensorMap tmA{}, tmB{}, tmAlo{}, tmBlo{};
   const bool three = A.lo != nullptr && B.lo != nullptr;
   if ((A.lo != nullptr) != (B.lo != nullptr)) return cudaErrorInvalidValue;
   if (AX::kKind != 0 && three) return cudaErrorInvalidValue;      // the transforms rewrite a single fp32 tile
+  if (B_T && (!bt.hi || (three && !bt.lo) || bt.ld < (size_t)N || bt.ld % 4 || K % 4 ||
+              ((reinterpret_cast<uintptr_t>(bt.hi) | reinterpret_cast<uintptr_t>(bt.lo)) % 16)))
+    return cudaErrorInvalidValue;
   if (A_MN || AX::kKind == 0) {
     if (!operand_map(&tmA, A.base, A_MN, M, K, A.ld)) return cudaErrorInvalidValue;
     if (three && !operand_map(&tmAlo, A.lo, A_MN, M, K, A.ld)) return cudaErrorInvalidValue;
@@ -1157,8 +1234,8 @@ inline cudaError_t launch_cfg(cudaStream_t st, int M, int N, int K, int splits, 
   if (!operand_map(&tmB, B.base, B_MN, N, K, B.ld)) return cudaErrorInvalidValue;
   if (three && !operand_map(&tmBlo, B.lo, B_MN, N, K, B.ld)) return cudaErrorInvalidValue;
   const GemmPtrs ptr{A.base, A.ld};
-  return launch_kernel<A_MN, B_MN, Epi, AX>(st, tmA, tmB, tmAlo, tmBlo, make_shape(M, N, K, splits, three ? 3 : 1), ptr, epi,
-                                            num_sms, ax);
+  return launch_kernel<A_MN, B_MN, Epi, AX, B_T>(st, tmA, tmB, tmAlo, tmBlo, make_shape(M, N, K, splits, three ? 3 : 1), ptr, epi,
+                                                 num_sms, ax, bt);
 }
 
 // number of split-K slices launch_cfg will actually produce

@@ -97,8 +97,11 @@ _SIGNATURES = {
                                     _P, C.c_size_t, _P]),
     "c2v_selftest_gemm3": (C.c_int, [_P, _I32, _I32, _I32, _I32, _I32, _I32, _I32, _P, _P, C.c_size_t, _P, _P, C.c_size_t,
                                      _P, C.c_size_t, _P]),
+    "c2v_selftest_gemm_bt": (C.c_int, [_P, _I32, _I32, _I32, _P, C.c_size_t, _P, C.c_size_t, _P, C.c_size_t, _P, C.c_size_t,
+                                       _P]),
     "c2v_selftest_split": (C.c_int, [_P, _P, _P, _P, C.c_size_t, _P]),
     "c2v_selftest_transpose": (C.c_int, [_P, _P, _I32, _I32, _P, _P, C.c_size_t, _P]),
+    "c2v_selftest_target_t": (C.c_int, [_P, _I32, C.POINTER(C.c_size_t), C.POINTER(C.c_size_t)]),
     "c2v_selftest_row_sum": (C.c_int, [_P, _I32, _P, _P, _I32, _P, _P]),
     "c2v_selftest_exchange_push": (C.c_int, [_P, _P, _P, _I32, _P, _P, _I32, _P]),
     "c2v_set_event": (C.c_int, [_P, C.c_char_p, _P]),
@@ -331,6 +334,24 @@ class PathAttentionEngine:
         self._check(self.lib.c2v_selftest_transpose(self.h, x.data_ptr(), rows, cols, out[0].data_ptr(),
                                                     out[1].data_ptr() if split else None, ld_t, self._stream()))
         return tuple(out) if split else out[0]
+
+    def selftest_gemm_bt(self, A, B, M: int, N: int, K: int, BT, C_out=None):
+        """Test hook: C[M,N] = A.B (tf32) with A [M,K] and B [N,K] row-major, and B^T written into BT [K, >= N] by the same
+        kernel (c2v_selftest_gemm_bt); returns C."""
+        if C_out is None:          # the epilogue stores float4s: 16-byte row pitch
+            C_out = self.torch.empty((M, (N + 3) // 4 * 4), dtype=self.torch.float32, device=self.dev)[:, :N]
+        out = C_out
+        self._check(self.lib.c2v_selftest_gemm_bt(self.h, M, N, K, A.data_ptr(), A.stride(0), B.data_ptr(), B.stride(0),
+                                                  out.data_ptr(), out.stride(0), BT.data_ptr(), BT.stride(0), self._stream()))
+        return out
+
+    def selftest_target_t(self, lo: bool = False):
+        """Test hook: the workspace's K-major copy of the target table that dv reads (c2v_selftest_target_t), as a
+        [code_dim, ld] view: the table (tf32) or its transposed high parts (3xTF32); lo: the transposed residuals."""
+        off, ld = C.c_size_t(), C.c_size_t()
+        self._check(self.lib.c2v_selftest_target_t(self.h, int(lo), C.byref(off), C.byref(ld)))
+        n = self.dims.code_dim * ld.value
+        return self.workspace[off.value:off.value + 4 * n].view(self.torch.float32).view(self.dims.code_dim, ld.value)
 
     def selftest_gemm(self, A, B, a_mn: bool, b_mn: bool, M: int, N: int, K: int, bn: int = 192, splits: int = 1,
                       three: bool = False):

@@ -415,11 +415,22 @@ int c2v_selftest_gemm3(c2v_engine* e, int32_t a_mn, int32_t b_mn, int32_t bn, in
                        void* stream);
 int c2v_selftest_split(c2v_engine* e, const float* x, float* hi, float* lo, size_t count, void* stream);
 
+/* The same product with both operands K contiguous (tf32, no split-K) that also writes B transposed, as the logits GEMM
+ * writes the target table's K-major copy for dv: BT[k * ldbt + n] = B[n * ldb + k] for n < N, k < K (columns N .. ldbt-1
+ * are not written).  K % 4 == 0, ldbt >= N and ldbt % 4 == 0, BT 16-byte aligned. */
+int c2v_selftest_gemm_bt(c2v_engine* e, int32_t M, int32_t N, int32_t K, const float* A, size_t lda, const float* B,
+                         size_t ldb, float* C, size_t ldc, float* BT, size_t ldbt, void* stream);
+
 /* Test hook for the K-major copies the engine makes of its MN-major GEMM operands: xT[c, r] = x[r, c] for a row-major
  * x [rows, cols] (pitch cols) into xT [cols, ldT] (ldT >= rows; columns rows .. ldT-1 are not written).  With xT_lo
  * non-NULL, xT / xT_lo receive the transposed 3xTF32 split of x instead.  Device pointers. */
 int c2v_selftest_transpose(c2v_engine* e, const float* x, int32_t rows, int32_t cols, float* xT, float* xT_lo, size_t ldT,
                            void* stream);
+
+/* Test hook: where the bound workspace holds the K-major copy of the target table that the dv GEMM reads, Ytab^T
+ * [code_dim, *ld] (columns target_vocab .. *ld-1 are padding): lo = 0 the table itself (tf32) or its transposed high parts
+ * (3xTF32), lo = 1 the transposed residuals (3xTF32).  *offset is in bytes from the workspace base. */
+int c2v_selftest_target_t(const c2v_engine* e, int32_t lo, size_t* offset, size_t* ld);
 
 /* Test hook for option "deterministic": the sort + chunked reduce of a train step's embedding-gradient scatter, on
  * `count` caller-given contributions instead of dX' (no dropout, no scaling): row rows[i] of table table_id (0 = token

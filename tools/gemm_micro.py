@@ -3,7 +3,8 @@ java14m train step (B = 1024, C = 200), each product in the operand layout the e
 copies made by torch, in the all-K-major layout.  The all-K-major time is the ceiling to compare against: there
 both operands go from TMA straight to wgmma, with no transpose in shared memory.  Where the engine now feeds a
 K-major copy of an operand it stores MN-major (W^T, v^T, Ytab^T), the layout it used before is timed as well, and
-so are the copies themselves (c2v_selftest_transpose; plain, and as the 3xTF32 split).
+so are the copies themselves (c2v_selftest_transpose; plain, and as the 3xTF32 split).  The logits GEMM is also timed
+writing Ytab^T from its B tiles, as the train step runs it (c2v_selftest_gemm_bt), alternating with the plain product.
 
     python tools/gemm_micro.py [--reps 20]
 """
@@ -86,6 +87,21 @@ def main():
         print(line, flush=True)
         del out
         torch.cuda.empty_cache()
+
+    # the logits GEMM with and without the Ytab^T write, alternated so that clock drift falls on both arms alike
+    A, Bm = padded(B, D), padded(Y, D)
+    out = torch.empty((B, (Y + 3) // 4 * 4), device="cuda")
+    bt = torch.empty((D, (Y + 63) // 64 * 64), device="cuda")
+    plain, write = [], []
+    for _ in range(5):
+        plain.append(time_gemm(A, Bm, False, False, B, Y, D, 1, out[None]))
+        write.append(time_fn(lambda: eng.selftest_gemm_bt(A, Bm, B, Y, D, bt, out)))
+    med = lambda xs: sorted(xs)[len(xs) // 2]
+    print("%-20s plain: %s ms   + Ytab^T write: %s ms   median %.3f -> %.3f ms (+%.3f)" % (
+        "logits   v.Ytab^T", " ".join("%.3f" % x for x in plain), " ".join("%.3f" % x for x in write), med(plain), med(write),
+        med(write) - med(plain)), flush=True)
+    del A, Bm, out, bt
+    torch.cuda.empty_cache()
 
     for name, rows, cols, ld_t in COPIES:
         x = torch.empty((rows, cols), device="cuda").normal_()
