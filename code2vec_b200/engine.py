@@ -45,6 +45,11 @@ class c2v_reader_share_status(C.Structure):
                 ("bad_line", C.c_int64), ("bad_kind", C.c_int32), ("overflow", C.c_int32)]
 
 
+class c2v_prep_status(C.Structure):
+    _fields_ = [(n, C.c_int64) for n in ("lines", "bad_utf8", "bad_line", "long_lines", "seen", "kept", "written", "empty",
+                                         "longest", "keys", "slots", "rehashes")]
+
+
 class _DeviceArray:
     """A raw device allocation presented through __cuda_array_interface__ so torch can view it."""
 
@@ -139,6 +144,16 @@ _SIGNATURES = {
     "c2v_text_format_rows": (C.c_int, [_P, C.c_int64, _I32, C.c_int64, _P, _P, _P, C.c_size_t, _P, C.c_int64, _P, _P,
                                        _P]),
     "c2v_selftest_format_floats": (C.c_int, [_P, C.c_int64, _P, _P]),
+    # preprocessing (device_preprocess.py)
+    "c2v_prep_create": (C.c_int, [C.c_int, C.POINTER(_P)]),
+    "c2v_prep_destroy": (None, [_P]),
+    "c2v_prep_device_bytes": (C.c_size_t, [_P]),
+    "c2v_prep_count_chunk": (C.c_int, [_P, _P, C.c_int64, C.c_int64, C.POINTER(c2v_prep_status), _P]),
+    "c2v_prep_histogram": (C.c_int, [_P, _I32, C.POINTER(_P), C.POINTER(C.c_int64), _P]),
+    "c2v_prep_classify_chunk": (C.c_int, [_P, _P, C.c_int64, _I32, C.POINTER(c2v_reader_vocab), C.POINTER(c2v_reader_vocab),
+                                          C.POINTER(c2v_prep_status), _P]),
+    "c2v_prep_long_lines": (C.c_int, [_P, _P, _P, _P, _P]),
+    "c2v_prep_assemble": (C.c_int, [_P, _P, _P, C.POINTER(_P), C.POINTER(C.c_int64), _P]),
 }
 
 _lib = None

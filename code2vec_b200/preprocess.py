@@ -10,6 +10,7 @@ MAX_CONTEXTS context fields, padded with empty ones (SURVEY A.5).
 """
 from __future__ import annotations
 
+import os
 import pickle
 import random
 from argparse import ArgumentParser
@@ -112,13 +113,19 @@ def process_file(file_path: str, data_file_role: str, dataset_name: str, word_to
             kept_contexts += len(contexts)
             out.write(target + " " + " ".join(contexts) + " " * (max_contexts - len(contexts)) + "\n")
             written += 1
+    log_file_stats(file_path, seen_contexts, kept_contexts, written, empty, longest, log)
+    return written
+
+
+def log_file_stats(file_path: str, seen_contexts: int, kept_contexts: int, written: int, empty: int, longest: int,
+                   log=print):
+    """process_file's report (preprocess.py:68-74); ZeroDivisionError when no example was written, as upstream."""
     log("File: " + file_path)
     log("Average total contexts: " + str(float(seen_contexts) / written))
     log("Average final (after sampling) contexts: " + str(float(kept_contexts) / written))
     log("Total examples: " + str(written))
     log("Empty examples: " + str(empty))
     log("Max number of contexts per word: " + str(longest))
-    return written
 
 
 def save_dictionaries(dataset_name: str, word_to_count, path_to_count, target_to_count, num_training_examples: int,
@@ -152,6 +159,12 @@ def arguments_parser() -> ArgumentParser:
 
 
 def main(argv: Optional[Iterable[str]] = None, rng=random, log=print) -> int:
+    """C2V_DEVICE_PREPROCESS=1 runs the same command line on the GPU (device_preprocess.main); the files, the log lines
+    of process_file and the state `rng` is left in are the same."""
+    from .device_preprocess import device_preprocess_flag
+    if device_preprocess_flag(os.environ):
+        from . import device_preprocess
+        return device_preprocess.main(argv, rng, log)
     args = arguments_parser().parse_args(None if argv is None else list(argv))
     histos = {"word": args.word_histogram, "path": args.path_histogram, "target": args.target_histogram}
     if not all(histos.values()):

@@ -620,6 +620,68 @@ int c2v_text_format_rows(const float* x, int64_t rows, int32_t cols, int64_t ld,
  * out[i * C2V_TEXT_VALUE_BYTES, ...) followed by NUL bytes up to the next value, and its length to len[i] (host). */
 int c2v_selftest_format_floats(const float* x, int64_t n, char* out, int32_t* len);
 
+/* ---- Preprocessing on the device (DESIGN.md §6g) ----------------------------------------------------------------------
+ * Raw extractor output (`target ctx ctx ...` lines) in device memory -> what preprocess.py's count_histograms and
+ * process_file write, byte for byte (device_preprocess.py).  A chunk is whole lines of a file under universal newlines:
+ * it ends after '\n', after a '\r' that the file does not follow with '\n', or at the end of the file.  Lines are split
+ * on ' ' into fields (field 0 the target, the others contexts, empty ones included) and contexts on ','.  A handle is
+ * independent of any engine or reader handle.  Failures return a negative c2v_status with the message in
+ * c2v_last_error(NULL).  Calls on one handle run on one caller stream, one host thread at a time; each call below that
+ * reports a status synchronises the stream. */
+typedef struct c2v_prep c2v_prep;
+
+typedef struct c2v_prep_status {
+  int64_t lines;       /* lines of the chunk, blank ones included                                                   */
+  int64_t bad_utf8;    /* offset in the chunk of the first byte Python's strict UTF-8 decoder rejects, or -1; the
+                          chunk is not processed further when it is set                                             */
+  int64_t bad_line;    /* classify: the first line (0-based in the chunk) with more than max_contexts contexts and a
+                          context of fewer than 3 parts (process_file raises IndexError there), or -1             */
+  int64_t long_lines;  /* classify: lines with more than max_contexts contexts                                     */
+  int64_t seen, kept, written, empty, longest;   /* classify: process_file's statistics over the chunk's lines      */
+  int64_t keys;        /* count: distinct keys in the histogram table (all three kinds)                             */
+  int64_t slots;       /* count: slots of the table                                                                 */
+  int64_t rehashes;    /* count: times the table was doubled with keys in it                                        */
+} c2v_prep_status;
+
+int c2v_prep_create(int device, c2v_prep** out);
+void c2v_prep_destroy(c2v_prep* h);          /* synchronises the device, then frees the handle's buffers */
+size_t c2v_prep_device_bytes(const c2v_prep* h);     /* device memory the handle holds (table, arena, scratch) */
+
+/* count_histograms over the chunk text[0, nbytes) (device memory, nbytes < 2^31) that starts at byte file_offset of
+ * the file: per line tokens[p0], paths[p1], tokens[p2] of every context of 3 parts or more (later parts ignored),
+ * tokens[p0] and, with a second part, paths[p1] of the others, and targets[field 0].  Counts add up across calls; each
+ * key keeps the file offset of its first occurrence.  The table doubles (rehash) before a chunk whose inserts could
+ * take it past half full; key bytes are copied to an arena, so the text may be reused once this returns. */
+int c2v_prep_count_chunk(c2v_prep* h, const char* text, int64_t nbytes, int64_t file_offset, c2v_prep_status* st,
+                         void* stream);
+
+/* The histogram of kind 0 (tokens), 1 (paths) or 2 (targets) as write_histogram writes a Counter: `word count\n` per
+ * key, keys in the order of their first occurrence.  *text (device memory of the handle, valid until the next call on
+ * it) and *nbytes receive the text. */
+int c2v_prep_histogram(c2v_prep* h, int32_t kind, const char** text, int64_t* nbytes, void* stream);
+
+/* The down-sampling decisions of process_file for the chunk text[0, nbytes) (device memory, kept unchanged until
+ * c2v_prep_assemble has run): every context's bytes, and for each line of more than max_contexts contexts its full
+ * (all three parts in the vocabularies: token and path are membership tables built as c2v_reader_vocab, a word is in
+ * when its index is not oov) and partial contexts in file order.  st gets the chunk's statistics. */
+int c2v_prep_classify_chunk(c2v_prep* h, const char* text, int64_t nbytes, int32_t max_contexts,
+                            const c2v_reader_vocab* token, const c2v_reader_vocab* path, c2v_prep_status* st,
+                            void* stream);
+
+/* Per line of more than max_contexts contexts of the classified chunk, in file order (host outputs [st.long_lines]):
+ * its line in the chunk, its full and its partial context counts. */
+int c2v_prep_long_lines(c2v_prep* h, int64_t* line, int32_t* n_full, int32_t* n_partial, void* stream);
+
+/* The lines process_file writes for the classified chunk: long line r (in c2v_prep_long_lines order) takes
+ * picks[pick_off[r], pick_off[r + 1]) (host memory): with n_full > max_contexts, max_contexts indices into its full
+ * contexts (rng.sample(range(n_full), max_contexts)); with n_full + n_partial > max_contexts, max_contexts - n_full
+ * indices into its partial contexts after all the full ones; otherwise none (its full, then its partial contexts).
+ * Output contexts keep the pick order; a line is `target ctx ... ctx` + the padding spaces up to max_contexts contexts
+ * + '\n', and lines left with no context are skipped.  *text (device memory of the handle, valid until the next call)
+ * and *nbytes receive the chunk's lines; the copy is ordered on `stream`.  C2V_ERR_STATE when bad_line was set. */
+int c2v_prep_assemble(c2v_prep* h, const int32_t* picks, const int64_t* pick_off, const char** text, int64_t* nbytes,
+                      void* stream);
+
 #ifdef __cplusplus
 }
 #endif
