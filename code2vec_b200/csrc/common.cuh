@@ -22,15 +22,18 @@ __device__ __forceinline__ float warp_max(float v) {
 // ---------------------------------------------------------------------------------------------
 // theta <- theta - (lr_t m) / (sqrt(v) + eps): the parameter move of TF1 Adam in correctly rounded fp32 operations, shared by
 // every kernel that applies it (adam_kernel, the lazy row replay, the dY epilogue) so that they stay bit-identical.
+// tests/adam_model.py states the step; tests/test_gpu_adam_model.py holds every path to it bit for bit.
 // A ZERO numerator -- an element whose gradient has been exactly zero so far (dropout masks a quarter of every row; rows
 // no batch has touched), or lr_t m underflowing -- makes the correctly rounded quotient a zero of the numerator's sign
-// (the denominator is positive), so theta - num is the same bits as theta - num / den.  Dividing anyway sends div.rn.f32
+// when the denominator is positive, so theta - num is the same bits as theta - num / den.  Dividing anyway sends div.rn.f32
 // through its out-of-line slow path (zero / denormal operands), which a profile of the row replay showed on 46 % of the
-// divisions of a 25-step run; the branch keeps it for genuinely denormal numerators only.
+// divisions of a 25-step run; the branch keeps it for genuinely denormal numerators only.  The denominator is positive
+// for every v >= 0 only when eps > 0 (pos_eps, decided by the caller from the step's eps): with eps = 0 an element with
+// m = v = 0 divides 0 / 0 into NaN, and a negative eps can flip the zero's sign, exactly as the dense kernel does.
 // ---------------------------------------------------------------------------------------------
-__device__ __forceinline__ float adam_move(float theta, float lr_t, float m, float v, float eps) {
+__device__ __forceinline__ float adam_move(float theta, float lr_t, float m, float v, float eps, bool pos_eps) {
   const float num = __fmul_rn(lr_t, m);
-  if (num == 0.f) return __fsub_rn(theta, num);
+  if (pos_eps && num == 0.f) return __fsub_rn(theta, num);
   return __fsub_rn(theta, __fdiv_rn(num, __fadd_rn(__fsqrt_rn(v), eps)));
 }
 // exp_slab schedule (umma::EpiExpSumT, expsum_combine_kernel): a row's largest U = exp(logit - c_row) must stay inside this
@@ -44,7 +47,8 @@ constexpr float kExpSlabMin = 1e-26f, kExpSlabMax = 1e30f;
 constexpr float kExpSlabMinOperand = 0x1p-112f;
 
 // The same move without the test, for dense gradients (the target table's update in the dY epilogue, adam_kernel): zero
-// numerators are rare there and the branch costs more than the occasional slow path.  Identical bits by the argument above.
+// numerators are rare there and the branch costs more than the occasional slow path.  Identical bits to adam_move, for
+// every eps, by the argument above.
 __device__ __forceinline__ float adam_move_dense(float theta, float lr_t, float m, float v, float eps) {
   return __fsub_rn(theta, __fdiv_rn(__fmul_rn(lr_t, m), __fadd_rn(__fsqrt_rn(v), eps)));
 }

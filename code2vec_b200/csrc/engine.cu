@@ -326,6 +326,8 @@ struct PhaseTimer {
 inline int rest_ok(const c2v_engine* e) {
   return (e->rest_shortcut && e->hp_b1 > 0.f && e->hp_b1 <= 0.95f && e->hp_b2 >= 0.99f && e->hp_b2 < 1.f && e->hp_eps > 0.f) ? 1 : 0;
 }
+// adam_move's zero-numerator exit (common.cuh) matches the division only while sqrt(v) + eps > 0, i.e. for eps > 0
+inline int pos_eps(const c2v_engine* e) { return e->hp_eps > 0.f ? 1 : 0; }
 inline bool is_tc(const c2v_engine* e) { return e->math_mode != C2V_MATH_FP32; }          // tensor-core (wgmma) GEMMs
 inline bool is_3x(const c2v_engine* e) { return e->math_mode == C2V_MATH_3XTF32; }        // ... as 3xTF32
 inline bool aligned16(const void* p) { return reinterpret_cast<uintptr_t>(p) % 16 == 0; }
@@ -481,10 +483,10 @@ int prepare_rows(c2v_engine* e, cudaStream_t st, const ContextSource& cs) {
     const float* lr_tab = wsp<float>(e, e->ws.lr_tab);
     C2V_ADAM_ROWS(e, ADAM_ROWS_CATCHUP, st,
                   e->theta.tok, e->grad.tok, e->am.tok, e->av.tok, d.token_vocab, d.embed_dim, stamp_tok, e->mark_epoch,
-                      wsp<int32_t>(e, e->ws.last_tok), (int32_t)e->adam_t_done, lr_tab, e->hp_b1, e->hp_b2, e->hp_eps, rest_ok(e));
+                      wsp<int32_t>(e, e->ws.last_tok), (int32_t)e->adam_t_done, lr_tab, e->hp_b1, e->hp_b2, e->hp_eps, rest_ok(e), pos_eps(e));
     C2V_ADAM_ROWS(e, ADAM_ROWS_CATCHUP, st,
                   e->theta.path, e->grad.path, e->am.path, e->av.path, d.path_vocab, d.embed_dim, stamp_path, e->mark_epoch,
-                      wsp<int32_t>(e, e->ws.last_path), (int32_t)e->adam_t_done, lr_tab, e->hp_b1, e->hp_b2, e->hp_eps, rest_ok(e));
+                      wsp<int32_t>(e, e->ws.last_path), (int32_t)e->adam_t_done, lr_tab, e->hp_b1, e->hp_b2, e->hp_eps, rest_ok(e), pos_eps(e));
   }
   return C2V_OK;
 }
@@ -495,7 +497,7 @@ int launch_sweep(c2v_engine* e, cudaStream_t st, float* p, float* g, float* m, f
   int blocks = (rows + 7) / 8;
   if (blocks > e->num_sms * 4) blocks = e->num_sms * 4;
   C2V_LAUNCH(e, (adam_sweep_kernel<4><<<blocks, 256, 0, st>>>(p, g, m, v, rows, dim, last, (int32_t)t, wsp<float>(e, e->ws.lr_tab), e->hp_b1,
-                                                             e->hp_b2, e->hp_eps, rest_ok(e))));
+                                                             e->hp_b2, e->hp_eps, rest_ok(e), pos_eps(e))));
   return C2V_OK;
 }
 
@@ -582,10 +584,10 @@ int early_catchup(c2v_engine* e, cudaStream_t side) {
   C2V_LAUNCH(e, (mark_rows_kernel<<<(rows + 255) / 256, 256, 0, side>>>(hs, hp, ht, rows, stamp_tok, stamp_path, e->mark_epoch)));
   C2V_ADAM_ROWS(e, ADAM_ROWS_CATCHUP, side,
                   e->theta.tok, e->grad.tok, e->am.tok, e->av.tok, d.token_vocab, d.embed_dim, stamp_tok, e->mark_epoch,
-                    wsp<int32_t>(e, e->ws.last_tok), (int32_t)t, lr_tab, e->hp_b1, e->hp_b2, e->hp_eps, rest_ok(e));
+                    wsp<int32_t>(e, e->ws.last_tok), (int32_t)t, lr_tab, e->hp_b1, e->hp_b2, e->hp_eps, rest_ok(e), pos_eps(e));
   C2V_ADAM_ROWS(e, ADAM_ROWS_CATCHUP, side,
                   e->theta.path, e->grad.path, e->am.path, e->av.path, d.path_vocab, d.embed_dim, stamp_path, e->mark_epoch,
-                    wsp<int32_t>(e, e->ws.last_path), (int32_t)t, lr_tab, e->hp_b1, e->hp_b2, e->hp_eps, rest_ok(e));
+                    wsp<int32_t>(e, e->ws.last_path), (int32_t)t, lr_tab, e->hp_b1, e->hp_b2, e->hp_eps, rest_ok(e), pos_eps(e));
   e->early_t = t;
   e->early_count++;
   return C2V_OK;
@@ -1449,7 +1451,7 @@ int sampled_train_step_impl(c2v_engine* e, cudaStream_t st, const int32_t* src, 
     if (e->adam_t_done > 0)
       C2V_ADAM_ROWS(e, ADAM_ROWS_CATCHUP, st,
                     e->theta.tgt, e->grad.tgt, e->am.tgt, e->av.tgt, d.target_vocab, d.code_dim, stamp, e->mark_epoch, last,
-                    (int32_t)e->adam_t_done, wsp<float>(e, e->ws.lr_tab), e->hp_b1, e->hp_b2, e->hp_eps, rest_ok(e));
+                    (int32_t)e->adam_t_done, wsp<float>(e, e->ws.lr_tab), e->hp_b1, e->hp_b2, e->hp_eps, rest_ok(e), pos_eps(e));
   }
   {
     PhaseTimer pt(e, PH_SAMPLED, st);

@@ -967,9 +967,10 @@ __global__ void __launch_bounds__(kTopkThreads) topk_merge_iter_kernel(TopkMerge
 
 // ---------------------------------------------------------------------------------------------
 // tf.compat.v1.train.AdamOptimizer dense apply (tensorflow_model.py:232; SURVEY A.3).  Every
-// element is visited (TF1's sparse apply decays m, v and moves theta on all rows).  Rounding
-// order matches oracle.adam_step.  zero_grad: clear g after use, so the next step's scatter-add
-// starts from zero without a separate memset pass.
+// element is visited (TF1's sparse apply decays m, v and moves theta on all rows).  The operations
+// and their order are the float32 step of tests/adam_model.py, with lr_t computed on the host as
+// oracle.adam_lr_t states it; tests/test_gpu_adam_model.py compares the bits.  zero_grad: clear g
+// after use, so the next step's scatter-add starts from zero without a separate memset pass.
 // ---------------------------------------------------------------------------------------------
 __global__ void __launch_bounds__(256)
 adam_kernel(float* __restrict__ p, float* __restrict__ g, float* __restrict__ m, float* __restrict__ v, size_t n4,
@@ -1358,11 +1359,13 @@ constexpr int kLrRingMask = kLrRing - 1;
 // delta_s = lr_s m_s / (sqrt(v_s) + eps) shrinks monotonically in magnitude and keeps its sign.  Rounding is
 // monotone, so once fl(theta - delta_s) == theta for EVERY element of the row it stays so for all later steps:
 // theta is left alone and only m <- fl(m b1), v <- fl(v b2) continue, without the division and square root.
-// Bit-identical to the dense kernel (tests/test_lazy_adam_model.py on the CPU, tests/test_gpu_lazy_adam.py on
-// the GPU); the engine enables it only for 0 < b1 <= 0.95, 0.99 <= b2 < 1.
+// Bit-identical to the dense kernel: tests/test_lazy_adam_model.py checks the scheme on the CPU and
+// tests/test_gpu_adam_model.py every element of the replayed tables against the float32 step on the GPU; the engine
+// enables it only for 0 < b1 <= 0.95, 0.99 <= b2 < 1, eps > 0.  pos_eps: eps > 0 (adam_move's zero-numerator exit).
 __device__ __forceinline__ void replay_row(float* __restrict__ p, float* __restrict__ g, float* __restrict__ m, float* __restrict__ v,
                                            size_t row_off, int d, int32_t from, int32_t t_done, const float* __restrict__ lr_tab,
-                                           float b1, float b2, float eps, float omb1, float omb2, int lane, bool rest_ok) {
+                                           float b1, float b2, float eps, float omb1, float omb2, int lane, bool rest_ok,
+                                           bool pos_eps) {
   for (int j0 = 0; j0 < d; j0 += 128) {          // every lane walks every slice: the vote below needs all 32
     const int j = j0 + lane * 4;
     const bool act = j < d;
@@ -1382,7 +1385,7 @@ __device__ __forceinline__ void replay_row(float* __restrict__ p, float* __restr
       for (int q = 0; q < 4; ++q) {
         mm[q] = __fadd_rn(__fmul_rn(mm[q], b1), __fmul_rn(omb1, gg[q]));
         vv[q] = __fadd_rn(__fmul_rn(vv[q], b2), __fmul_rn(omb2, __fmul_rn(gg[q], gg[q])));
-        pp[q] = adam_move(pp[q], lr_s, mm[q], vv[q], eps);
+        pp[q] = adam_move(pp[q], lr_s, mm[q], vv[q], eps, pos_eps);
       }
     }
     // the zero-gradient steps after it: m*b1 + (1-b1)*0, v*b2 + (1-b2)*(0*0)
@@ -1394,7 +1397,7 @@ __device__ __forceinline__ void replay_row(float* __restrict__ p, float* __restr
       for (int q = 0; q < 4; ++q) {
         mm[q] = __fadd_rn(__fmul_rn(mm[q], b1), __fmul_rn(omb1, 0.f));
         vv[q] = __fadd_rn(__fmul_rn(vv[q], b2), __fmul_rn(omb2, 0.f));
-        const float np = adam_move(pp[q], lr_s, mm[q], vv[q], eps);
+        const float np = adam_move(pp[q], lr_s, mm[q], vv[q], eps, pos_eps);
         moved |= (__float_as_uint(np) != __float_as_uint(pp[q]));
         pp[q] = np;
       }
@@ -1427,7 +1430,7 @@ template <int MODE, int OCC>
 __global__ void __launch_bounds__(256, OCC)
 adam_rows_kernel(float* __restrict__ p, float* __restrict__ g, float* __restrict__ m, float* __restrict__ v, int rows, int d,
                  const int32_t* __restrict__ stamp, int32_t epoch, int32_t* __restrict__ last, int32_t t_done,
-                 const float* __restrict__ lr_tab, float b1, float b2, float eps, int rest_ok) {
+                 const float* __restrict__ lr_tab, float b1, float b2, float eps, int rest_ok, int pos_eps) {
   const int lane = threadIdx.x & 31;
   const int warp_global = (blockIdx.x * 256 + threadIdx.x) >> 5;
   const int total_warps = (gridDim.x * 256) >> 5;
@@ -1459,7 +1462,8 @@ adam_rows_kernel(float* __restrict__ p, float* __restrict__ g, float* __restrict
       todo &= todo - 1;
       if (todo) prefetch_row(base + __ffs(todo) - 1);
       const int32_t from = __shfl_sync(0xffffffffu, from_l, b);
-      replay_row(p, g, m, v, (size_t)(base + b) * d, d, from, t_done, lr_tab, b1, b2, eps, omb1, omb2, lane, rest_ok != 0);
+      replay_row(p, g, m, v, (size_t)(base + b) * d, d, from, t_done, lr_tab, b1, b2, eps, omb1, omb2, lane, rest_ok != 0,
+                 pos_eps != 0);
     }
     if (hit) last[r] = t_done;
   }
@@ -1471,7 +1475,7 @@ template <int OCC>
 __global__ void __launch_bounds__(256, OCC)
 adam_sweep_kernel(float* __restrict__ p, float* __restrict__ g, float* __restrict__ m, float* __restrict__ v, int rows, int d,
                   int32_t* __restrict__ last, int32_t t_done, const float* __restrict__ lr_tab, float b1, float b2, float eps,
-                  int rest_ok) {
+                  int rest_ok, int pos_eps) {
   const int lane = threadIdx.x & 31;
   const int warp_global = (blockIdx.x * 256 + threadIdx.x) >> 5;
   const int total_warps = (gridDim.x * 256) >> 5;
@@ -1479,7 +1483,7 @@ adam_sweep_kernel(float* __restrict__ p, float* __restrict__ g, float* __restric
   for (int row = warp_global; row < rows; row += total_warps) {
     const int32_t from = last[row];
     if (from >= t_done) continue;
-    replay_row(p, g, m, v, (size_t)row * d, d, from, t_done, lr_tab, b1, b2, eps, omb1, omb2, lane, rest_ok != 0);
+    replay_row(p, g, m, v, (size_t)row * d, d, from, t_done, lr_tab, b1, b2, eps, omb1, omb2, lane, rest_ok != 0, pos_eps != 0);
     __syncwarp();
     if (lane == 0) last[row] = t_done;
   }

@@ -1,6 +1,6 @@
 """The deferred-update scheme of `lazy_adam` (DESIGN.md section 4.4) as a numpy model, against the dense TF1 Adam of
-the oracle (SURVEY A.3), in float32 with the same operation order as adam_kernel / replay_row.  This pins the
-ALGORITHM on the CPU (the CUDA kernels are pinned against it on the GPU by tests/test_gpu_lazy_adam.py):
+the oracle (SURVEY A.3), in float32 with the same operation order as adam_kernel / replay_row (tests/adam_model.py).
+This pins the ALGORITHM on the CPU (tests/test_gpu_adam_model.py pins the CUDA kernels to the same float32 step):
   * a row that is only brought up to date when a batch references it again, when the periodic sweep reaches it or at
     a flush -- one step with the gradient that was left in its gradient row, then zero-gradient steps -- ends with
     the same bits as a row updated densely;
@@ -10,19 +10,19 @@ ALGORITHM on the CPU (the CUDA kernels are pinned against it on the GPU by tests
 """
 import numpy as np
 
+from oracle.path_attention_oracle import adam_lr_t
+from tests import adam_model
+
 F = np.float32
 
 
 def lr_at(t, lr=1e-3, b1=0.9, b2=0.999):
-    return F(float(lr) * np.sqrt(1.0 - float(b2) ** t) / (1.0 - float(b1) ** t))      # computed in double on the host, as the engine does
+    return adam_lr_t(t, lr, b1, b2)
 
 
 def dense_step(p, m, v, g, t, b1, b2, eps, lr=1e-3):
     """adam_kernel: every element, every step (correctly rounded fp32 operations in this order)."""
-    b1, b2, eps = F(b1), F(b2), F(eps)
-    m[:] = m * b1 + (F(1) - b1) * g
-    v[:] = v * b2 + (F(1) - b2) * (g * g)
-    p[:] = p - (lr_at(t, lr, float(b1), float(b2)) * m) / (np.sqrt(v) + eps)
+    adam_model.step(p, m, v, g, lr_at(t, lr, b1, b2), b1, b2, eps)
 
 
 class LazyTable:
