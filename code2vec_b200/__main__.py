@@ -11,12 +11,16 @@ them as extractor.py:22-38 does (first MAX_CONTEXTS contexts, path strings repla
 """
 from __future__ import annotations
 
+import os
 import sys
 from typing import Iterable, Optional
 
-from . import load_model_dynamically
+import numpy as np
+
+from . import load_model_dynamically, similarity
 from .common import common
 from .config import Config
+from .multi_rank import run_world
 from .vocabularies import VocabType
 
 SHOW_TOP_CONTEXTS = 10       # interactive_predict.py:6
@@ -74,6 +78,34 @@ def print_predictions(config: Config, model, lines: Iterable[str], out=None):
             out.write(" ".join(map(str, raw.code_vector)) + "\n")
 
 
+def print_most_similar(model, vocab_type: VocabType, lines: Iterable[str], topn: int, out=None):
+    """One block per query line (`pos1,pos2[ neg1,neg2]`): `Most similar to:\\t<line>`, then `\\t(%f) <word>` per result;
+    a query with a word outside the vocabulary prints `Not in vocabulary: <w>` instead."""
+    out = sys.stdout if out is None else out
+    for line in lines:
+        query = similarity.parse_query_line(line)
+        if query is None:
+            continue
+        missing = [w for w in query[0] + query[1] if w not in model.vocabs.get(vocab_type).word_to_index]
+        if missing:
+            out.write("Not in vocabulary: %s\n" % missing[0])
+            continue
+        out.write(similarity.format_most_similar(line, model.most_similar(query[0], query[1], topn=topn,
+                                                                          vocab_type=vocab_type)))
+
+
+def write_nearest(model, c2v_path: str, topn: int) -> str:
+    """`<c2v_path>.nearest`: line r is example r's name, then `\\t<row>,<name>,<similarity>` per nearest other example."""
+    names, _vectors, idx, val = model.nearest_code_vectors(c2v_path, topn)
+    out_path = c2v_path + ".nearest"
+    pad = np.iinfo(np.int32).max
+    with open(out_path, "w") as f:
+        for r, name in enumerate(names):
+            f.write(similarity.format_nearest_line(
+                name, [(int(j), names[j], float(v)) for j, v in zip(idx[r], val[r]) if j != pad]))
+    return out_path
+
+
 def main(argv: Optional[Iterable[str]] = None) -> int:
     argv = list(sys.argv[1:] if argv is None else argv)
     predict_input = None
@@ -81,6 +113,8 @@ def main(argv: Optional[Iterable[str]] = None) -> int:
         i = argv.index("--predict_input")
         predict_input = argv[i + 1]
         del argv[i:i + 2]
+    argv, sim = similarity.split_cli_flags(argv)       # --most_similar, --most_similar_input, --nearest, --topn
+    similarity.check_single_gpu(sim, run_world(os.environ)[0])
     config = Config(set_defaults=True)
     config.load_from_args(argv)
     config.verify()
@@ -106,6 +140,15 @@ def main(argv: Optional[Iterable[str]] = None) -> int:
                     print_predictions(config, model, f)
             else:
                 print_predictions(config, model, sys.stdin)
+        if sim.most_similar is not None:
+            vocab_type = {"target": VocabType.Target, "token": VocabType.Token, "path": VocabType.Path}[sim.most_similar]
+            if sim.most_similar_input:
+                with open(sim.most_similar_input, "r") as f:
+                    print_most_similar(model, vocab_type, f, sim.topn)
+            else:
+                print_most_similar(model, vocab_type, sys.stdin, sim.topn)
+        if sim.nearest is not None:
+            config.log("Nearest code vectors written to: %s" % write_nearest(model, sim.nearest, sim.topn))
     finally:
         model.close_session()
     return 0

@@ -295,6 +295,9 @@ class Code2VecModel(Code2VecModelBase):
             self._dev_eval_reader.close()
             self._dev_eval_reader = None
         self._device_vocabs = None
+        if getattr(self, "_knn_handle", None) is not None:
+            self._knn_handle.close()
+            self._knn_handle = None
         if self.engine is not None:
             if self.world > 1:
                 import torch
@@ -874,6 +877,69 @@ class Code2VecModel(Code2VecModelBase):
             return self._gather_table(self._param_of_vocab[vocab_type])
         self.engine.sync_tables()
         return self.engine.params[self._param_of_vocab[vocab_type]].detach()
+
+    # ---- nearest neighbours (similarity.py, DESIGN.md §6h) ------------------------------------------------------------
+    def _knn(self):
+        """The model's search handle, made once (one GPU only, as --predict)."""
+        from .similarity import NearestNeighbours
+        if self.world > 1:
+            raise ValueError("most_similar and nearest_code_vectors run on one GPU; this run has %d ranks" % self.world)
+        if getattr(self, "_knn_handle", None) is None:
+            self._knn_handle = NearestNeighbours(self.engine.dev)
+            self._knn_bound = None
+        return self._knn_handle
+
+    def most_similar(self, positive, negative=(), topn: int = 10, vocab_type: VocabType = VocabType.Target):
+        """gensim 4's KeyedVectors.most_similar(positive, negative, topn) on the table of `vocab_type`, on the GPU:
+        [(word, cosine similarity)], the query's own words left out.  KeyError for a word outside the vocabulary."""
+        from . import similarity
+        if isinstance(positive, str):
+            positive = [positive]
+        if isinstance(negative, str):
+            negative = [negative]
+        nn = self._knn()
+        vocab = self.vocabs.get(vocab_type)
+        for w in list(positive) + list(negative):
+            if w not in vocab.word_to_index:
+                raise KeyError("Key '%s' not present in vocabulary" % w)
+        # the table as it stands after the engine's last step: re-bound whenever a step has run since
+        stamp = (vocab_type, self._math_eval, self.engine.launch_count)
+        if self._knn_bound != stamp:
+            nn.bind(self._vocab_embedding_on_device(vocab_type), self._math_eval)
+            self._knn_bound = (vocab_type, self._math_eval, self.engine.launch_count)
+        return similarity.most_similar(nn, vocab.word_to_index, vocab.index_to_word, positive, negative, topn)
+
+    def nearest_code_vectors(self, c2v_path: str, topn: int = 10):
+        """The code vectors of the examples of `c2v_path` that evaluate() scores -- in its order and its batches of
+        TEST_BATCH_SIZE, equal to what --export_code_vectors writes -- and each one's topn nearest other examples by
+        cosine: (names [N], code vectors [N, D] on the host, neighbour rows [N, topn], similarities [N, topn]), rows
+        padded with (INT_MAX, -inf) when the corpus has fewer than topn + 1 examples."""
+        import copy
+        import torch
+        from . import similarity
+        nn = self._knn()
+        cfg = copy.copy(self.config)
+        cfg.TEST_DATA_PATH = c2v_path
+        reader = PathContextReader(vocabs=self.vocabs, model_input_tensors_former=_EvaluateInputFormer(), config=cfg,
+                                   estimator_action=EstimatorAction.Evaluate)
+        self.engine.set_option("math_mode", self._math_eval)
+        names, parts = [], []
+        for batch in reader.get_dataset():
+            t = _EvaluateInputFormer().from_model_input_form(batch)
+            _idx, _vals, code, _attn = self.engine.predict_batch_host(
+                t.path_source_token_indices, t.path_indices, t.path_target_token_indices, t.context_valid_mask,
+                normalize=False, want_code=True, want_attention=False)
+            names.extend(common.binary_to_string(n) for n in t.target_string)
+            parts.append(code)
+        D = self.config.CODE_VECTOR_SIZE
+        vectors = np.concatenate(parts) if parts else np.zeros((0, D), dtype=np.float32)
+        if vectors.shape[0] == 0:
+            return names, vectors, np.zeros((0, topn), np.int32), np.zeros((0, topn), np.float32)
+        self._knn_bound = None
+        idx, val = similarity.nearest_rows(nn, torch.from_numpy(vectors).to(self.engine.dev), topn, self._math_eval)
+        self.log("Nearest neighbours: %d code vectors, %.1f MB of device memory held" % (
+            vectors.shape[0], nn.device_bytes() / 1e6))
+        return names, vectors, idx, val
 
     def _gather_table(self, name: str):
         """The whole table `name` on every rank (a collective), in device memory: the embedding shards all-gathered and

@@ -1543,6 +1543,23 @@ int adam_impl(c2v_engine* e, cudaStream_t st, float lr, float b1, float b2, floa
 // failures of calls without an engine handle in other translation units (reader.cu): c2v_last_error(NULL) returns them
 namespace c2v {
 void set_global_error(const std::string& msg) { g_create_error = msg; }
+
+// The top-k kernels of this file for the nearest-neighbour search (knn.cu), which cannot include kernels.cuh a second
+// time.  Row r of `rows` keeps the best k of its L sorted candidate lists [L, k] at (idx, val) + r * L * k (k <= 16), or
+// of slab row S + r * ldS (k <= 64), in tf.nn.top_k's order, into idx_out / val_out [rows, k].
+cudaError_t knn_topk_merge(const int32_t* idx, const float* val, int L, int k, int rows, int32_t* idx_out, float* val_out,
+                           cudaStream_t st) {
+  const TopkMergeArgs ma{idx, val, L, (size_t)L * k, (size_t)k, k, 0, nullptr, nullptr, 1, rows, 0, idx_out, val_out};
+  topk_merge_kernel<16><<<rows, kTopkThreads, 0, st>>>(ma);
+  return cudaGetLastError();
+}
+cudaError_t knn_topk_slab(const float* S, size_t ldS, int N, int k, int rows, int32_t* idx_out, float* val_out, cudaStream_t st) {
+  if (k <= 16)
+    topk_kernel<16><<<rows, kTopkThreads, 0, st>>>(S, ldS, N, k, 0, idx_out, val_out);
+  else
+    topk_iter_kernel<<<rows, kTopkThreads, 0, st>>>(S, ldS, N, k, 0, idx_out, val_out);
+  return cudaGetLastError();
+}
 }
 
 // ================================== C ABI =======================================================

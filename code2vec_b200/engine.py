@@ -154,6 +154,14 @@ _SIGNATURES = {
                                           C.POINTER(c2v_prep_status), _P]),
     "c2v_prep_long_lines": (C.c_int, [_P, _P, _P, _P, _P]),
     "c2v_prep_assemble": (C.c_int, [_P, _P, _P, C.POINTER(_P), C.POINTER(C.c_int64), _P]),
+    # nearest neighbours (similarity.py)
+    "c2v_knn_create": (C.c_int, [C.c_int, C.POINTER(_P)]),
+    "c2v_knn_destroy": (None, [_P]),
+    "c2v_knn_device_bytes": (C.c_size_t, [_P]),
+    "c2v_knn_bind_table": (C.c_int, [_P, _P, C.c_int64, _I32, C.c_int64, _I32, _P]),
+    "c2v_knn_queries": (C.c_int, [_P, _P, _P, _P, _I32, _P, _P]),
+    "c2v_knn_search": (C.c_int, [_P, _P, _I32, C.c_int64, _I32, _P, _P, _I32, _P, _P, _P]),
+    "c2v_knn_profile": (C.c_int, [_P, _I32, C.POINTER(C.c_double), C.POINTER(C.c_double)]),
 }
 
 _lib = None

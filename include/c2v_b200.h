@@ -682,6 +682,50 @@ int c2v_prep_long_lines(c2v_prep* h, int64_t* line, int32_t* n_full, int32_t* n_
 int c2v_prep_assemble(c2v_prep* h, const int32_t* picks, const int64_t* pick_off, const char** text, int64_t* nbytes,
                       void* stream);
 
+/* ---- Nearest neighbours (DESIGN.md §6h) ------------------------------------------------------------------------------
+ * Cosine search over the rows of a float32 table T [rows, dim] in device memory: gensim 4's KeyedVectors.most_similar on
+ * the embedding tables, and the nearest methods of a corpus by code vector (similarity.py).  With norm_i = ||T_i||, row
+ * i scores s_i = (T_i . q) / norm_i against a query q; a row of zero norm (or with a NaN) scores NaN and is never
+ * returned.  Results are ordered as tf.nn.top_k orders them: value descending, exact ties to the lower row.  A handle is
+ * independent of any engine handle; failures return a negative c2v_status with the message in c2v_last_error(NULL).
+ * Calls on one handle run on one caller stream, one host thread at a time. */
+typedef struct c2v_knn c2v_knn;
+
+int c2v_knn_create(int device, c2v_knn** out);
+void c2v_knn_destroy(c2v_knn* h);          /* synchronises the device, then frees the handle's buffers */
+
+/* The most device memory the handle has held at once (norms, table copies, one query block's buffers). */
+size_t c2v_knn_device_bytes(const c2v_knn* h);
+
+/* Binds T (row r at table + r * ld; 1 <= dim <= ld, rows < 2^31) with the arithmetic of the searches (c2v_math_mode):
+ * computes the row norms (in double) and, in 3xTF32, the tf32 split of the table; a table without a 16-byte row pitch
+ * is also copied with one.  T must stay allocated while bound; once its contents change, bind it again (the norms and
+ * copies describe the contents at this call).  Asynchronous on `stream`. */
+int c2v_knn_bind_table(c2v_knn* h, const float* table, int64_t rows, int32_t dim, int64_t ld, int32_t math, void* stream);
+
+/* gensim's query vectors (KeyedVectors.get_mean_vector with pre- and post-normalisation): query j is the sum over
+ * e in [offsets[j], offsets[j + 1]) of weights[e] * T[word_ids[e]] / norm, computed in double and scaled to unit length
+ * (a zero sum stays zero), written as float to q_out [nq, dim] (pitch dim).  word_ids (in [0, rows)), weights
+ * (+1 positive, -1 negative), offsets [nq + 1] and q_out are device memory.  Asynchronous on `stream`. */
+int c2v_knn_queries(c2v_knn* h, const int32_t* word_ids, const float* weights, const int64_t* offsets, int32_t nq, float* q_out,
+                    void* stream);
+
+/* For each query j of q [nq, dim] (pitch ldq >= dim, device): the k + max_exclude best rows, then without the ids
+ * exclude[exclude_off[j], exclude_off[j + 1]) (device; NULL when max_exclude = 0; a list has at most max_exclude
+ * entries), the first k of the rest -> idx / val [nq, k] (device), padded with (INT_MAX, -inf) where fewer rows remain.
+ * That is gensim's exclusion of the query words from the top topn + len(words).  k + max_exclude <= 64.
+ * Routes: tf32 / 3xTF32 with k + max_exclude <= 16, the wgmma GEMM whose epilogue scales each column by 1 / norm and
+ * keeps candidate lists, merged per query; otherwise (fp32, or more candidates) the fp32 SIMT GEMM into a score slab
+ * and the top-k kernels.  Queries go in blocks whose candidate lists or slab take at most 512 MB and that hold at most
+ * 65536 queries, so the memory held does not grow with nq.  Asynchronous on `stream`. */
+int c2v_knn_search(c2v_knn* h, const float* q, int32_t nq, int64_t ldq, int32_t k, const int32_t* exclude,
+                   const int64_t* exclude_off, int32_t max_exclude, int32_t* idx, float* val, void* stream);
+
+/* Device time of the searches since the last call, split into the GEMM (with its candidate epilogue) and the selection
+ * (merge or slab top-k, exclusion), in ms; synchronises.  on != 0 times the searches that follow (CUDA events around
+ * each query block), 0 stops. */
+int c2v_knn_profile(c2v_knn* h, int32_t on, double* gemm_ms, double* select_ms);
+
 #ifdef __cplusplus
 }
 #endif
