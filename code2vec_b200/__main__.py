@@ -135,7 +135,20 @@ def main(argv: Optional[Iterable[str]] = None) -> int:
                 config.log(str(eval_results).replace("topk", "top{}".format(config.TOP_K_WORDS_CONSIDERED_DURING_PREDICTION)))
         if config.PREDICT:
             model.predict([])                          # the reference's warm-up call (interactive_predict.py:16)
-            if predict_input:
+            if getattr(model, "device_predict", False):
+                # C2V_DEVICE_PREDICT=1: the whole input as bytes, read with the source's newline rule on the GPU
+                if predict_input:
+                    with open(predict_input, "rb") as f:
+                        data, universal = f.read(), True
+                else:
+                    data, universal = sys.stdin.buffer.read(), False
+                sys.stdout.flush()
+                if model.print_predictions_device(data, universal, sys.stdout.buffer):
+                    sys.stdout.buffer.flush()
+                else:
+                    from .device_predict import split_source_lines
+                    print_predictions(config, model, split_source_lines(data, universal))
+            elif predict_input:
                 with open(predict_input, "r") as f:
                     print_predictions(config, model, f)
             else:

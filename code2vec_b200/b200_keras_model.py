@@ -206,6 +206,8 @@ class Code2VecModel(_TFNumericsModel):
         return ModelEvaluationResults(topk_acc=list(hits / n_examples), subtoken_precision=counts.precision,
                                       subtoken_recall=counts.recall, subtoken_f1=counts.f1, loss=loss_sum / n_examples)
 
+    _PREDICT_NORMALIZE = 2                     # the device predict route's scores: full-vocabulary probabilities
+
     # ---- predict (keras_model.py:196-232): scores are full-vocabulary probabilities ---------------------
     def predict(self, predict_data_lines: Iterable[str]) -> List[ModelPredictionResults]:
         if self.predict_reader is None:

@@ -34,6 +34,7 @@ from .multi_rank import (CKPT_MAGIC, CKPT_SUFFIX, batch_split, check_checkpoint_
                          write_checkpoint, write_checkpoint_part)
 from . import device_reader as _device_reader_mod
 from .device_reader import device_eval_flag, device_reader_flag, sharded_reader_flag
+from .device_predict import device_predict_flag
 from .text_export import DeviceTextWriter, device_text_flag
 from .trainer import Trainer, make_fully_sharded_engine
 from .vocabularies import VocabType
@@ -160,6 +161,9 @@ class Code2VecModel(Code2VecModelBase):
                              "metrics and loss on the host; unset C2V_DEVICE_EVAL or evaluate with --framework b200")
         # C2V_DEVICE_TEXT=1: `.vectors` and word2vec files are formatted on the GPU (text_export.py, DESIGN.md §6f)
         self._device_text = device_text_flag(os.environ)
+        # C2V_DEVICE_PREDICT=1: `--predict` reads, predicts and formats on the GPU (device_predict.py, DESIGN.md §6i)
+        self._device_predict = device_predict_flag(os.environ)
+        self._dev_predictor = None
         self._device_vocabs = None               # device_reader.DeviceVocabs, shared by the training and evaluation readers
         self._eval_tables = None                 # device_reader.eval_tables of the target vocabulary
         self._dev_eval_reader = None
@@ -261,6 +265,9 @@ class Code2VecModel(Code2VecModelBase):
             self._device_eval))
         self.log("b200 backend text export: `.vectors` and word2vec files formatted %s (C2V_DEVICE_TEXT=%d)" % (
             "on the GPU" if self._device_text else "on the host", self._device_text))
+        self.log("b200 backend predict: %s (C2V_DEVICE_PREDICT=%d)" % (
+            "read, predicted in batches and formatted on the GPU" if self._device_predict else "one method at a time on the host",
+            self._device_predict))
         if self.world > 1:
             # every multi-GPU run, evaluate-only ones too: the row shards and Trainer.predict live in the Trainer.
             # C2V_DETERMINISTIC=1 sends the embedding gradients through the ordered exchange (DESIGN.md §5.1)
@@ -291,6 +298,9 @@ class Code2VecModel(Code2VecModelBase):
         self.log("Done loading model weights")
 
     def close_session(self):
+        if self._dev_predictor is not None:
+            self._dev_predictor.close()
+            self._dev_predictor = None
         if self._dev_eval_reader is not None:
             self._dev_eval_reader.close()
             self._dev_eval_reader = None
@@ -866,6 +876,33 @@ class Code2VecModel(Code2VecModelBase):
                 topk_predicted_words_scores=scores[0], attention_per_context=attention_per_context,
                 code_vector=(code_vectors[0] if self.config.EXPORT_CODE_VECTORS else None)))
         return results
+
+    # ---- `--predict` on the GPU (C2V_DEVICE_PREDICT=1, DESIGN.md §6i) ------------------------------------------------
+    _PREDICT_NORMALIZE = 1                     # softmax over the k scores, as predict() asks the engine for
+
+    @property
+    def device_predict(self) -> bool:
+        return self._device_predict
+
+    def print_predictions_device(self, data: bytes, universal_newlines: bool, out) -> bool:
+        """__main__.print_predictions over the extractor output `data` (a file read in text mode when
+        universal_newlines, else standard input), predicted and formatted on the GPU and written to the binary stream
+        `out`, byte for byte the host route's text.  False, with nothing written, for an input that needs the host route
+        (a byte >= 0x80, or a path the device's key table cannot hold: device_predict.py)."""
+        from .device_predict import DevicePredictor
+        if self.world > 1:
+            raise ValueError("--predict runs on one GPU; this run has %d ranks" % self.world)
+        if self._dev_predictor is None:
+            self._dev_predictor = DevicePredictor(self, self._PREDICT_NORMALIZE)
+        p = self._dev_predictor
+        done = p.run(data, universal_newlines, out, want_code=self.config.EXPORT_CODE_VECTORS)
+        if not done:
+            self.log("Device predict: the input needs the host route (a byte >= 0x80, a numeric path that is not the "
+                     "decimal of an int32, or a path of 1 MB or more); predicting it one method at a time on the host")
+        else:
+            self.log("Device predict: %.1f MB of device memory held, %.1f MB page-locked" % (
+                p.device_bytes() / 1e6, p.pinned_bytes / 1e6))
+        return done
 
     def _get_vocab_embedding_as_np_array(self, vocab_type: VocabType) -> np.ndarray:
         assert vocab_type in VocabType

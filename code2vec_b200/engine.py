@@ -162,6 +162,18 @@ _SIGNATURES = {
     "c2v_knn_queries": (C.c_int, [_P, _P, _P, _P, _I32, _P, _P]),
     "c2v_knn_search": (C.c_int, [_P, _P, _I32, C.c_int64, _I32, _P, _P, _I32, _P, _P, _P]),
     "c2v_knn_profile": (C.c_int, [_P, _I32, C.POINTER(C.c_double), C.POINTER(C.c_double)]),
+    # device predict (device_predict.py)
+    "c2v_pred_create": (C.c_int, [C.c_int, _I32, C.POINTER(c2v_reader_vocab), C.POINTER(c2v_reader_vocab), C.POINTER(_P)]),
+    "c2v_pred_destroy": (None, [_P]),
+    "c2v_pred_device_bytes": (C.c_size_t, [_P]),
+    "c2v_pred_set_targets": (C.c_int, [_P, _I32, _P, _P, _I32, _P]),
+    "c2v_pred_reset_keys": (C.c_int, [_P, _P]),
+    "c2v_pred_chunk": (C.c_int, [_P, _P, C.c_int64, C.c_int64, _I32, _I32, C.POINTER(C.c_int64), _P]),
+    "c2v_pred_seal_keys": (C.c_int, [_P, _P]),
+    "c2v_pred_line_info": (C.c_int, [_P, _P, _P, _P, _P]),
+    "c2v_pred_rows": (C.c_int, [_P, _P, _I32, _P, _P, _P, _P, _P]),
+    "c2v_pred_format": (C.c_int, [_P, _I32, _P, _P, _I32, _P, _P, _I32, _P, C.c_int64, _P, _P, _P]),
+    "c2v_selftest_format_fixed": (C.c_int, [_P, C.c_int64, _P, _P]),
 }
 
 _lib = None

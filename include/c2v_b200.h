@@ -726,6 +726,74 @@ int c2v_knn_search(c2v_knn* h, const float* q, int32_t nq, int64_t ldq, int32_t 
  * each query block), 0 stops. */
 int c2v_knn_profile(c2v_knn* h, int32_t on, double* gemm_ms, double* select_ms);
 
+/* ---- Device predict (DESIGN.md §6i) ---------------------------------------------------------------------------------
+ * `--predict` over extractor output in device memory (device_predict.py): the model input rows of its methods and the
+ * text __main__.print_predictions writes for them, byte for byte.  The input must be ASCII.  A handle is independent of
+ * any engine handle and reads the vocabularies' device tables (c2v_reader_vocab, as c2v_reader_create) while it lives;
+ * failures return a negative c2v_status with the message in c2v_last_error(NULL).  One caller stream, one host thread. */
+typedef struct c2v_pred c2v_pred;
+
+int c2v_pred_create(int device, int32_t max_contexts, const c2v_reader_vocab* tok, const c2v_reader_vocab* path,
+                    c2v_pred** out);
+void c2v_pred_destroy(c2v_pred* h);        /* synchronises the device, then frees the handle's buffers */
+
+/* The most device memory the handle has held at once. */
+size_t c2v_pred_device_bytes(const c2v_pred* h);
+
+/* The predicted-name text of every target word: word i's bytes are repr[repr_off[i], repr_off[i + 1]) (host arrays,
+ * copied; str(word.split("|")) on the host).  Ids outside [0, n_words) and `oov` are not printed. */
+int c2v_pred_set_targets(c2v_pred* h, int32_t n_words, const char* repr, const int64_t* repr_off, int32_t oov, void* stream);
+
+/* The input goes through the handle in chunks of whole lines (each ending at a '\n', or at the end of the input), in
+ * three passes: every chunk with C2V_PRED_KEYS, then c2v_pred_seal_keys, every chunk with C2V_PRED_PATHS, then, for
+ * predicting, each chunk with C2V_PRED_SCAN followed by c2v_pred_rows / c2v_pred_format on its methods.
+ * c2v_pred_reset_keys starts the first pass over.  Only the current chunk is held on the device.
+ *
+ * A chunk's lines end at '\n' and, with universal_newlines != 0 (a file opened in text mode), also at a '\r' not
+ * followed by '\n'.  Each line is rstripped; it is a method when its first ' '-separated field is not empty, and its first
+ * max_contexts non-empty fields after that are its contexts, each of which must have exactly two commas.  Every context's
+ * path has a key: the path itself when it is -?[0-9]+, else the decimal of its Java String.hashCode.  Per key, the handle
+ * keeps the path text of the last context in the input that has it (the largest file_offset + position).
+ *   C2V_PRED_SCAN  : index and scan the chunk's lines (c2v_pred_line_info, c2v_pred_rows read them)
+ *   C2V_PRED_KEYS  : the same, and record every kept context's key (file_offset: the chunk's offset in the input)
+ *   C2V_PRED_PATHS : copy the path texts the table names that lie in this chunk (no line index)
+ * Returns the chunk's number of lines (0 for C2V_PRED_PATHS); synchronises. */
+#define C2V_PRED_SCAN 0
+#define C2V_PRED_KEYS 1
+#define C2V_PRED_PATHS 2
+int c2v_pred_reset_keys(c2v_pred* h, void* stream);
+int c2v_pred_chunk(c2v_pred* h, const char* text, int64_t nbytes, int64_t file_offset, int32_t universal_newlines,
+                   int32_t mode, int64_t* n_lines, void* stream);
+/* After the last C2V_PRED_KEYS chunk: sizes the arena of path texts.  Synchronises. */
+int c2v_pred_seal_keys(c2v_pred* h, void* stream);
+
+/* Per line of the current chunk (host arrays [n_lines]): the rstripped line [lo, hi) in the chunk, its kind (0 skipped,
+ * 1 method, 2 a kept context without exactly three comma-separated parts, 3 a path whose key the table cannot hold: a
+ * numeric path that is not the canonical decimal of an int32, such as "007", or a path of 1 MB or more) and its number of
+ * kept contexts (up to the first bad one).  Synchronous. */
+int c2v_pred_line_info(c2v_pred* h, int64_t* lo, int64_t* hi, int32_t* kind, int32_t* kept);
+
+/* The model input of the n methods on lines lines[0, n) of the current chunk (host; all of kind 1): src / path / tgt [n, max_contexts] int32
+ * and mask [n, max_contexts] float32 (device), as PathContextReader._map_raw_dataset_row_to_input_tensors builds them
+ * from __main__.prepare_extracted_lines' line.  The rows' contexts are kept for the next c2v_pred_format.  Synchronises. */
+int c2v_pred_rows(c2v_pred* h, const int64_t* lines, int32_t n, int32_t* src, int32_t* path, int32_t* tgt, float* mask,
+                  void* stream);
+
+/* The text of the n rows of the last c2v_pred_rows: for each, "Original name:", the predictions idx / val [n, k], the
+ * "Attention:" lines from attn [n, max_contexts] and, when code_vec [n, code_dim] is not NULL, "Code vector:" and its
+ * line (all device), once the C2V_PRED_PATHS pass is done.  Written back to back at out (device) when they fit
+ * out_cap; *total (host) gets their length either way, and *bad_row (host) the lowest row whose distinct contexts have
+ * NaN and non-NaN attention (a value >= n if none; nothing is written then).  Asynchronous: *total and *bad_row are
+ * valid once `stream` has completed, so they should be page-locked. */
+int c2v_pred_format(c2v_pred* h, int32_t n, const int32_t* idx, const float* val, int32_t k, const float* attn,
+                    const float* code_vec, int32_t code_dim, char* out, int64_t out_cap, int64_t* total, int32_t* bad_row,
+                    void* stream);
+
+/* Test hook, on the CPU: Python's '%f' % float(x[i]) as the device formats it, into out[i * C2V_FIXED_BYTES, ...)
+ * padded with NUL bytes, and its length to len[i] (host). */
+#define C2V_FIXED_BYTES 48
+int c2v_selftest_format_fixed(const float* x, int64_t n, char* out, int32_t* len);
+
 #ifdef __cplusplus
 }
 #endif
