@@ -123,6 +123,31 @@ def run_determinism(environ, now=time.time):
     return deterministic, seed
 
 
+MAX_NUM_SAMPLED = 1024              # the sampled-softmax head's limit (c2v_sampled_train_step)
+
+
+def num_sampled_flag(environ) -> int:
+    """C2V_NUM_SAMPLED=<S>: train() runs the sampled softmax with S unique log-uniform negatives per step, drawn on the GPU
+    (DESIGN.md §6j); 0 (the default) runs the full softmax.  ValueError for anything but a non-negative integer."""
+    raw = environ.get("C2V_NUM_SAMPLED", "0") or "0"
+    try:
+        value = int(raw, 10)
+    except ValueError:
+        raise ValueError("C2V_NUM_SAMPLED must be a non-negative integer, got %r" % raw) from None
+    if value < 0 or raw.strip() != raw:
+        raise ValueError("C2V_NUM_SAMPLED must be a non-negative integer, got %r" % raw)
+    return value
+
+
+def check_num_sampled(num_sampled: int, target_vocab: int) -> None:
+    """ValueError unless 1 <= num_sampled <= min(1024, floor(target_vocab / 2)): the unique sampler needs at most half of the
+    target words, which keeps the expected number of draws per step small."""
+    limit = min(MAX_NUM_SAMPLED, target_vocab // 2)
+    if not 1 <= num_sampled <= limit:
+        raise ValueError("C2V_NUM_SAMPLED=%d is outside [1, %d]: the sampled softmax draws at most min(1024, half of the %d "
+                         "target words) negatives; lower it, or set 0 for the full softmax" % (num_sampled, limit, target_vocab))
+
+
 _CKPT_MAGIC = CKPT_MAGIC
 _CKPT_SUFFIX = CKPT_SUFFIX
 
@@ -144,6 +169,15 @@ class Code2VecModel(Code2VecModelBase):
         self.rank = 0
         self._own_group = False
         check_multi_rank_run(config, self.world)
+        # C2V_NUM_SAMPLED=<S>: train() runs the sampled softmax with S negatives drawn on the GPU (DESIGN.md §6j)
+        self._num_sampled = num_sampled_flag(os.environ)
+        if self._num_sampled and self.world > 1:
+            raise ValueError("C2V_NUM_SAMPLED=%d: the sampled softmax trains on one GPU and this run has %d ranks; unset "
+                             "C2V_NUM_SAMPLED to train on several GPUs, or train in a single process" % (
+                                 self._num_sampled, self.world))
+        if self._num_sampled and config.DL_FRAMEWORK == "b200-keras":
+            raise ValueError("C2V_NUM_SAMPLED is not available with --framework b200-keras: its loss is the full-vocabulary "
+                             "crossentropy; unset C2V_NUM_SAMPLED or train with --framework b200")
         # C2V_DEVICE_READER=1: train() reads its batches on the GPU (device_reader.py, DESIGN.md §6d)
         self._device_reader = device_reader_flag(os.environ)
         # C2V_SHARDED_READER=1: on several GPUs each rank reads and parses 1/W of every chunk (DESIGN.md §6d)
@@ -231,6 +265,16 @@ class Code2VecModel(Code2VecModelBase):
         """The engine and, for training or any multi-GPU run, its Trainer.  init: draw the initial parameters (on several
         GPUs before the Trainer moves the embedding tables into row shards)."""
         import torch
+        Y = self.vocabs.target_vocab.size
+        if self._num_sampled:
+            check_num_sampled(self._num_sampled, Y)
+        if self.config.is_training:
+            self.log("b200 backend training loss: %s (C2V_NUM_SAMPLED=%d)" % (
+                "sampled softmax, %d unique log-uniform negatives of the %d target words drawn on the GPU each step" % (
+                    self._num_sampled, Y) if self._num_sampled else "full softmax over the %d target words" % Y,
+                self._num_sampled))
+        elif self._num_sampled:
+            self.log("C2V_NUM_SAMPLED=%d has no effect: this run does not train (no --data)" % self._num_sampled)
         if self.world > 1:
             # this rank's engine: a block of target rows, sized for the global batch (trainer.make_fully_sharded_engine)
             self.engine = make_fully_sharded_engine(self._engine_dims(), self.config.TRAIN_BATCH_SIZE // self.world,
@@ -450,6 +494,7 @@ class Code2VecModel(Code2VecModelBase):
         # synchronous c2v_train_batch_host path.
         # several GPUs: every rank reads the same global batches (same file, same shuffle seed) and steps on its slice
         multi = self.world > 1
+        num_sampled = self._num_sampled        # > 0: every step is Trainer.step_sampled (refused on several ranks)
         dropped_rows = 0
         ring = dev_reader = None
         if self._device_reader:
@@ -491,12 +536,15 @@ class Code2VecModel(Code2VecModelBase):
                         batch.release()
                         continue
                 nxt = None
-                if self._hint_next and not multi and following is not None:
+                if self._hint_next and not multi and following is not None and not num_sampled:
                     following.wait()
                     nxt = following.tensors[:3]
                 batch_num += 1
                 self.engine.set_option("math_mode", self._math_train)
-                loss = self.trainer.step_device(*batch.tensors, next_batch=nxt)
+                if num_sampled:
+                    loss = self.trainer.step_sampled(*batch.tensors, num_sampled)
+                else:
+                    loss = self.trainer.step_device(*batch.tensors, next_batch=nxt)
                 batch.release()                    # the slot is reused once this step has run
                 loss_hist[n_hist:n_hist + 1].copy_(loss, non_blocking=True)
                 n_hist += 1
@@ -520,14 +568,21 @@ class Code2VecModel(Code2VecModelBase):
                     if hi == lo:                       # fewer rows than ranks: the batch is skipped
                         continue
                 nxt = None
-                if self._hint_next and not multi and following is not None:
+                if self._hint_next and not multi and following is not None and not num_sampled:
                     n = former.from_model_input_form(following)
                     nxt = (n.path_source_token_indices, n.path_indices, n.path_target_token_indices)
                 batch_num += 1
                 self.engine.set_option("math_mode", self._math_train)
                 if ring is not None:
                     rows = int(t.target_index.shape[0])
-                    self.trainer.step_ring(ring, rows, loss_hist[n_hist:n_hist + 1])      # upload + step queued; nothing waited for
+                    if num_sampled:                    # upload, draw and step queued; nothing waited for
+                        dev, slot = ring.upload_next(rows)
+                        loss = self.trainer.step_sampled(dev["src"], dev["path"], dev["tgt"], dev["mask"], dev["target"],
+                                                         num_sampled)
+                        ring.mark_compute_done(slot)
+                        loss_hist[n_hist:n_hist + 1].copy_(loss, non_blocking=True)
+                    else:
+                        self.trainer.step_ring(ring, rows, loss_hist[n_hist:n_hist + 1])      # upload + step queued; nothing waited for
                     n_hist += 1
                     self.h2d_bytes += rows * (4 * cfg.MAX_CONTEXTS + 1) * 4
                     flush = (batch_num % cfg.NUM_BATCHES_TO_LOG_PROGRESS == 0) or (batch_num % num_batches_to_save_and_eval == 0) \
@@ -541,11 +596,17 @@ class Code2VecModel(Code2VecModelBase):
                     batch_loss = self.trainer.step_host(*(a[lo:hi] for a in (
                         t.path_source_token_indices, t.path_indices, t.path_target_token_indices, t.context_valid_mask,
                         t.target_index)))
+                elif num_sampled:
+                    batch_loss = self.trainer.step_host_sampled(t.path_source_token_indices, t.path_indices,
+                                                                t.path_target_token_indices, t.context_valid_mask,
+                                                                t.target_index, num_sampled)
                 else:
                     batch_loss = self.trainer.step_host(t.path_source_token_indices, t.path_indices, t.path_target_token_indices,
                                                         t.context_valid_mask, t.target_index, next_batch=nxt)
             sum_loss += batch_loss
             if batch_num % cfg.NUM_BATCHES_TO_LOG_PROGRESS == 0:
+                if num_sampled:
+                    self._check_sampler()
                 self._trace_training(sum_loss, batch_num, multi_batch_start_time)
                 sum_loss = 0.0
                 multi_batch_start_time = time.time()
@@ -578,6 +639,8 @@ class Code2VecModel(Code2VecModelBase):
             self.log("Device reader: %.1f MB of text and draw indices uploaded, %.1f MB of device memory held%s" % (
                 dev_reader.h2d_bytes / 1e6, dev_reader.device_bytes() / 1e6, peers))
             dev_reader.close()
+        if num_sampled:
+            self._check_sampler()
         if multi:
             self.log("%d training rows left out: a short batch trains on a multiple of the %d ranks" % (
                 dropped_rows, self.world))
@@ -587,6 +650,14 @@ class Code2VecModel(Code2VecModelBase):
             self.log("Model saved in file: %s" % cfg.MODEL_SAVE_PATH)
         elapsed = int(time.time() - start_time)
         self.log("Training time: %sH:%sM:%sS\n" % ((elapsed // 60 // 60), (elapsed // 60) % 60, elapsed % 60))
+
+    def _check_sampler(self):
+        """RuntimeError if a sampled step's draw reached the sampler's cap of 2^31 draws without num_sampled distinct
+        classes (engine option "sampler_cap_hits"; the read synchronises, so it is made where train() waits anyway)."""
+        hits = self.engine.get_option("sampler_cap_hits")
+        if hits:
+            raise RuntimeError("the log-uniform sampler reached its cap of 2^31 draws without %d distinct classes in %d "
+                               "step(s)" % (self._num_sampled, hits))
 
     # ---- evaluate (tensorflow_model.py:114-195) ------------------------------------------------------
     def evaluate(self) -> Optional[ModelEvaluationResults]:

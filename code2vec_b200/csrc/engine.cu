@@ -42,6 +42,7 @@ struct Workspace {
   size_t stamp_tgt, last_tgt;                                    // ... of the target table (sampled softmax)
   size_t perm, bkt_count, bkt_cursor, bkt_starts;                            // locality-sorted peer gather / scatter (sharded tables)
   size_t det_keys[2], det_vals[2], det_hist, det_offs, det_starts, det_part;  // deterministic embedding-gradient sort + reduce
+  size_t samp_stamp, samp_status;                                // log-uniform sampler: per-class first-draw stamps, cap counter
   size_t total;
   size_t ldS;
   size_t ldB;     // row pitch of vT: the batch rounded up to 16 bytes, as TMA requires
@@ -142,6 +143,9 @@ Workspace carve(const c2v_dims& d) {
   w.det_offs = take(kDetRadix * tiles * 4);
   w.det_starts = take((kDetRadix * tiles + 1) * 4);
   w.det_part = take(2 * ((M + kDetChunk - 1) / kDetChunk) * (size_t)d.embed_dim * 4);
+  // c2v_sample_log_uniform: one 64-bit (call tag, first draw index) stamp per target class, and its cap-hit counter
+  w.samp_stamp = take((size_t)d.target_vocab * 8);
+  w.samp_status = take(64);
   w.total = off;
   return w;
 }
@@ -152,10 +156,10 @@ Workspace carve(const c2v_dims& d) {
 // the launching stream; c2v_phase_stats() resolves them.
 enum Phase { PH_CTX_FWD = 0, PH_ATTN_FWD, PH_LOGITS, PH_XENT, PH_DV, PH_DY, PH_ATTN_BWD, PH_DW, PH_DX_SCATTER,
              PH_ADAM, PH_TOPK, PH_SAMPLED, PH_GATHER, PH_DX_GEMM, PH_ADAM_CATCHUP, PH_SPLIT, PH_ADAM_SWEEP, PH_PEER_SORT, PH_INBOX_APPLY,
-             PH_COUNT };
+             PH_SAMPLER, PH_COUNT };
 const char* const kPhaseNames[PH_COUNT] = {"ctx_fwd", "attn_fwd", "logits", "xent", "dv", "dY", "attn_bwd", "dW",
                                            "dx_scatter", "adam", "topk", "sampled_softmax", "gather", "dx_gemm",
-                                           "adam_catchup", "split", "adam_sweep", "peer_sort", "inbox_apply"};
+                                           "adam_catchup", "split", "adam_sweep", "peer_sort", "inbox_apply", "sampler"};
 struct PhaseLog {
   std::vector<std::pair<cudaEvent_t, cudaEvent_t>> pending;
   std::vector<std::pair<cudaEvent_t, cudaEvent_t>> free_list;
@@ -269,6 +273,7 @@ struct c2v_engine {
   int64_t early_count = 0;              // how many steps used the hint (option "early_catchup_count", read-only)
   int fuse_tgt = 0;                     // option "fuse_target_adam": c2v_train_batch_host arms itself
   int64_t tgt_fused_t = 0;              // step count whose target update has already been applied (0 = none)
+  uint32_t sample_tag = 0;              // c2v_sample_log_uniform: tag of the last call (counts down; 0 = stamps not initialised)
   int deterministic;
   int64_t launches;
   std::string err;
@@ -1553,6 +1558,10 @@ cudaError_t knn_topk_merge(const int32_t* idx, const float* val, int L, int k, i
   topk_merge_kernel<16><<<rows, kTopkThreads, 0, st>>>(ma);
   return cudaGetLastError();
 }
+cudaError_t launch_log_uniform_sampler(int32_t Y, double log_range, int32_t S, const int32_t* target, int32_t B,
+                                       uint64_t seed, uint64_t step, uint32_t tag, unsigned long long* stamp,
+                                       int32_t* sampled, float* logq_true, float* logq_sampled, int64_t* num_tries,
+                                       int32_t* cap_hits, cudaStream_t st);     // sampler.cu
 cudaError_t knn_topk_slab(const float* S, size_t ldS, int N, int k, int rows, int32_t* idx_out, float* val_out, cudaStream_t st) {
   if (k <= 16)
     topk_kernel<16><<<rows, kTopkThreads, 0, st>>>(S, ldS, N, k, 0, idx_out, val_out);
@@ -1843,6 +1852,17 @@ int c2v_get_option(const c2v_engine* e, const char* key, int64_t* value) {
     }
     return C2V_OK;
   }
+  if (!strcmp(key, "sampler_cap_hits")) {         // c2v_sample_log_uniform calls that reached the draw cap (synchronises)
+    *value = 0;
+    if (e->wbase && e->sample_tag) {
+      int32_t n = 0;
+      if (cudaDeviceSynchronize() != cudaSuccess ||
+          cudaMemcpy(&n, e->wbase + e->ws.samp_status, 4, cudaMemcpyDeviceToHost) != cudaSuccess)
+        return C2V_ERR_CUDA;
+      *value = n;
+    }
+    return C2V_OK;
+  }
   if (!strcmp(key, "recompute_logits")) { *value = e->recompute; return C2V_OK; }
   if (!strcmp(key, "sort_peer_access")) { *value = e->sort_peer; return C2V_OK; }
   if (!strcmp(key, "adam_step_count")) { *value = e->adam_t_done; return C2V_OK; }
@@ -1949,6 +1969,34 @@ int c2v_sampled_train_step(c2v_engine* e, const int32_t* src, const int32_t* pat
   C2V_CUDA(e, cudaSetDevice(e->device));
   return sampled_train_step_impl(e, (cudaStream_t)stream, src, path, tgt, mask, target, B, sampled, S, logq_true,
                                  logq_sampled, keep_prob, seed, step, dropout_mask, loss_out);
+}
+
+int c2v_sample_log_uniform(c2v_engine* e, int32_t S, const int32_t* target, int32_t B, uint64_t seed, uint64_t step,
+                           int32_t* sampled, float* logq_true, float* logq_sampled, int64_t* num_tries, void* stream) {
+  int rc = check_batch(e, B);
+  if (rc) return rc;
+  if (!target || !sampled || !logq_true || !logq_sampled) return fail(e, C2V_ERR_INVALID, "NULL argument");
+  const int32_t Y = e->dims.target_vocab;
+  if (S < 1 || S > kMaxSampled || S > Y / 2)
+    return fail(e, C2V_ERR_INVALID, "number of sampled classes must be in [1, min(1024, target_vocab / 2)]");
+  if (e->table_world > 1)
+    return fail(e, C2V_ERR_UNSUPPORTED, "c2v_sample_log_uniform is single-GPU: the tables are row-sharded over several ranks");
+  C2V_CUDA(e, cudaSetDevice(e->device));
+  cudaStream_t st = (cudaStream_t)stream;
+  unsigned long long* stamp = wsp<unsigned long long>(e, e->ws.samp_stamp);
+  int32_t* cap_hits = wsp<int32_t>(e, e->ws.samp_status);
+  // a call's stamps are (tag << 32 | draw index) with tags counting down, so every earlier call's stamp is larger and the
+  // table never needs clearing -- except once at the start and after the 2^32 - 2 tags are used up
+  if (e->sample_tag <= 1) {
+    C2V_CUDA(e, cudaMemsetAsync(stamp, 0xFF, (size_t)Y * 8, st));
+    if (!e->sample_tag) C2V_CUDA(e, cudaMemsetAsync(cap_hits, 0, 4, st));
+    e->sample_tag = 0xFFFFFFFFu;
+  }
+  e->sample_tag--;
+  PhaseTimer pt(e, PH_SAMPLER, st);
+  C2V_LAUNCH(e, C2V_CUDA(e, launch_log_uniform_sampler(Y, log1p((double)Y), S, target, B, seed, step, e->sample_tag, stamp,
+                                                       sampled, logq_true, logq_sampled, num_tries, cap_hits, st)));
+  return C2V_OK;
 }
 
 int c2v_arm_target_adam(c2v_engine* e, float lr, float beta1, float beta2, float eps, int64_t t) {

@@ -79,6 +79,7 @@ _SIGNATURES = {
     "c2v_train_step": (C.c_int, [_P, _P, _P, _P, _P, _P, _I32, C.c_float, C.c_uint64, C.c_uint64, _P, _P, _P]),
     "c2v_sampled_train_step": (C.c_int, [_P, _P, _P, _P, _P, _P, _I32, _P, _I32, _P, _P, C.c_float,
                                          C.c_uint64, C.c_uint64, _P, _P, _P]),
+    "c2v_sample_log_uniform": (C.c_int, [_P, _I32, _P, _I32, C.c_uint64, C.c_uint64, _P, _P, _P, _P, _P]),
     "c2v_adam_step": (C.c_int, [_P, C.c_float, C.c_float, C.c_float, C.c_float, C.c_int64, _P]),
     "c2v_arm_target_adam": (C.c_int, [_P, C.c_float, C.c_float, C.c_float, C.c_float, C.c_int64]),
     "c2v_hint_next_batch": (C.c_int, [_P, _P, _P, _P, _I32]),
@@ -553,6 +554,22 @@ class PathAttentionEngine:
             src.shape[0], sampled.data_ptr(), sampled.shape[0], logq_true.data_ptr(), logq_sampled.data_ptr(),
             float(keep), int(seed), int(step), _ptr(dropout_mask), out.data_ptr(), self._stream()))
         return out
+
+    def sample_log_uniform(self, target, S: int, seed: int, step: int):
+        """c2v_sample_log_uniform: the S unique log-uniform candidates of (seed, step) and the log expected counts of
+        them and of target [B] (device int32), as device tensors (sampled int32 [S], logq_true [B], logq_sampled [S],
+        num_tries int64 [1]).  The buffers are the engine's own and the next call overwrites them."""
+        torch = self.torch
+        B, S = int(target.shape[0]), int(S)
+        buf = getattr(self, "_sampler_out", None)
+        if buf is None:          # sized once for the largest call the ABI accepts: S <= 1024, B <= max_batch
+            z = lambda n, dt: torch.empty(n, dtype=dt, device=self.dev)
+            buf = self._sampler_out = (z(1024, torch.int32), z(self.dims.max_batch, torch.float32), z(1024, torch.float32),
+                                       z(1, torch.int64))
+        sampled, lq_t, lq_s, tries = buf[0][:S], buf[1][:B], buf[2][:S], buf[3]
+        self._check(self.lib.c2v_sample_log_uniform(self.h, S, target.data_ptr(), B, int(seed), int(step), sampled.data_ptr(),
+                                                    lq_t.data_ptr(), lq_s.data_ptr(), tries.data_ptr(), self._stream()))
+        return sampled, lq_t, lq_s, tries
 
     def adam_step(self, lr=1e-3, beta1=0.9, beta2=0.999, eps=1e-8, t: Optional[int] = None):
         if t is None:

@@ -301,6 +301,36 @@ class Trainer:
         e.adam_step(t=t, **self.adam)
         return loss
 
+    def step_sampled(self, src, path, tgt, mask, target, num_sampled: int):
+        """One sampled-softmax training step whose num_sampled negatives are drawn on the device for (seed, t = adam_t + 1)
+        (c2v_sample_log_uniform, DESIGN.md section 6j), then step_device_sampled.  Single GPU; returns the device loss
+        without a sync.  The draw depends on the step count only, so a run resumed from a checkpoint (which restores
+        adam_t) continues the same negatives."""
+        if self.schedule != "single":
+            raise RuntimeError("the sampled-softmax step is single-GPU")
+        e = self.e
+        sampled, lq_t, lq_s, _ = e.sample_log_uniform(target, num_sampled, self.seed, e.adam_t + 1)
+        return self.step_device_sampled(src, path, tgt, mask, target, sampled, lq_t, lq_s)
+
+    def step_host_sampled(self, src, path, tgt, mask, target, num_sampled: int) -> float:
+        """step_sampled on HOST buffers (numpy / pinned tensors): uploads them, steps and returns the loss (synchronises)."""
+        e = self.e
+        torch = e.torch
+        if self._dev is None:
+            Bm, Cm = e.dims.max_batch, e.dims.max_contexts
+            z = lambda shape, dt: torch.empty(shape, dtype=dt, device=e.dev)
+            self._dev = dict(src=z((Bm, Cm), torch.int32), path=z((Bm, Cm), torch.int32), tgt=z((Bm, Cm), torch.int32),
+                             mask=z((Bm, Cm), torch.float32), target=z((Bm,), torch.int32))
+        B = int(src.shape[0])
+        d = self._dev
+        for name, arr in (("src", src), ("path", path), ("tgt", tgt), ("mask", mask), ("target", target)):
+            t = arr if isinstance(arr, torch.Tensor) else torch.from_numpy(np.ascontiguousarray(arr))
+            d[name][:B].copy_(t, non_blocking=True)
+        loss = self.step_sampled(d["src"][:B], d["path"][:B], d["tgt"][:B], d["mask"][:B], d["target"][:B], num_sampled)
+        self._loss_host.copy_(loss, non_blocking=True)
+        torch.cuda.current_stream(e.dev).synchronize()
+        return float(self._loss_host[0])
+
     def predict(self, src, path, tgt, mask, normalize: int = 0):
         """Top-k prediction of this rank's examples: (idx [B, k], val [B, k], code_vec [B, D]) as device tensors, the
         result of forward + topk on one engine holding the whole model (normalize as c2v_topk).  No training state is

@@ -220,6 +220,27 @@ int c2v_sampled_train_step(c2v_engine* e, const int32_t* src, const int32_t* pat
                            uint64_t step, const float* dropout_mask, float* loss_out,
                            void* stream);
 
+/* The candidates of one sampled-softmax step, drawn on the device: tf.nn.sampled_softmax_loss's default sampler,
+ * tf.random.log_uniform_candidate_sampler(unique=True) (TF's LogUniformSampler with RangeSampler's unique loop), on this
+ * library's own random stream.  NOT IN THE REFERENCE (DESIGN.md section 6j).  With Y = target_vocab:
+ *   draws    draw i = 0, 1, 2, ... of (seed, step) is r = Philox4x32-10 (common.cuh) at counter (i, 0, step_lo, step_hi)
+ *            with key (seed_lo ^ 0x6C6F6775, seed_hi ^ 0x73616D70) -- never the dropout mask's key (seed_lo, seed_hi);
+ *            u = ((r.x >> 5) * 2^26 + (r.y >> 6)) * 2^-53, a double in [0, 1); the drawn class is
+ *            v = ((int64)floor(exp(u * log1p(Y))) - 1) mod Y, in double.
+ *   unique   sampled[0..S) = the first S distinct values in draw order, in the order they first occur; num_tries = the
+ *            1-based index of the draw that supplied the S-th distinct value.
+ *   counts   in double, rounded to float32 once: p(c) = log((c + 2) / (c + 1)) / log1p(Y); count(c) = S p(c) when
+ *            num_tries == S, else -expm1(num_tries * log1p(-p(c))); logq = (float)log(count).  logq_sampled[s] is that of
+ *            c = sampled[s], logq_true[b] that of c = target[b] (same num_tries): c2v_sampled_train_step's logq_*.
+ * 1 <= S <= min(1024, Y / 2), 1 <= B <= max_batch, else C2V_ERR_INVALID; C2V_ERR_UNSUPPORTED on row-sharded tables
+ * (single GPU only).  sampled: device int32 [S]; logq_true: device float [B]; logq_sampled: device float [S]; num_tries:
+ * device int64 [1] or NULL.  Asynchronous on `stream`, writes device memory only, allocates nothing (the workspace holds
+ * 8 bytes per target class of first-draw stamps).  At most 2^31 draws: a call that reaches that cap without S distinct
+ * values fills the missing ids with class 0, reports num_tries = 2^31 and counts itself in the read-only option
+ * "sampler_cap_hits" (the read synchronises). */
+int c2v_sample_log_uniform(c2v_engine* e, int32_t S, const int32_t* target, int32_t B, uint64_t seed, uint64_t step,
+                           int32_t* sampled, float* logq_true, float* logq_sampled, int64_t* num_tries, void* stream);
+
 /* tf.compat.v1.train.AdamOptimizer() update of all five variables from the bound gradients
  * (tensorflow_model.py:232): lr_t = lr*sqrt(1-b2^t)/(1-b1^t); m,v decay on EVERY row (TF1's
  * sparse apply is not lazy); theta -= lr_t*m/(sqrt(v)+eps).  t is the 1-based step count. */

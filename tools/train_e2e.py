@@ -55,8 +55,9 @@ def main(n_lines=131072, C=200, n_tok=200000, n_path=150000, n_tgt=30000, thread
     # C2V_BATCH_RING=0 it calls the synchronous step_host instead.  Either way the host time at which step k was issued is
     # recorded: the ring bounds how far the host can run ahead of the GPU (10 slots), so over hundreds of steps the issue
     # rate is the execution rate.
-    # with C2V_DEVICE_READER=1 the loop feeds device slots to step_device instead
-    for name in ("step_host", "step_ring", "step_device"):
+    # with C2V_DEVICE_READER=1 the loop feeds device slots to step_device instead; with C2V_NUM_SAMPLED=<S> every route
+    # steps through step_sampled
+    for name in ("step_host", "step_ring", "step_device", "step_sampled"):
         inner = getattr(model.trainer, name)
 
         def stamped(*a, _inner=inner, **k):
@@ -77,7 +78,8 @@ def main(n_lines=131072, C=200, n_tok=200000, n_path=150000, n_tgt=30000, thread
                       "path_contexts_per_s": round(n_lines * epochs * C / dt, 1),
                       "steady_state_path_contexts_per_s": round(steady, 1), "batches": len(stamps), "file_MB": round(size_mb, 1),
                       "text_MB_per_s": round(size_mb * epochs / dt, 1), "reader_threads": threads, "host_cores": os.cpu_count(),
-                      "reader": "device" if model._device_reader else "host",
+                      "reader": "device" if model._device_reader else "host", "num_sampled": model._num_sampled,
+                      "target_vocab": model.vocabs.target_vocab.size,
                       "batch_ring": os.environ.get("C2V_BATCH_RING", "1") != "0" and not model._device_reader,
                       "h2d_bytes_total": int(getattr(model, "h2d_bytes", 0)),
                       "dataset_generation_s": round(gen_s, 1)}))
