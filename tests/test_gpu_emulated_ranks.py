@@ -374,23 +374,30 @@ def test_push_grads_survive_a_math_mode_change(monkeypatch):
 # ---- 3. production width ---------------------------------------------------------------------------------------------
 
 PROD_B = 1024
+# the large model's widths (d = 256, D = 768, Y = 261,246; bench.py --workload large) with token / path tables reduced
+# 10x, so that eight engines share one GPU
+LARGE_RED = O.Dims(token_vocab=300001, path_vocab=200001, target_vocab=261246, embed_dim=256, code_dim=768,
+                   max_contexts=200)
+WIDTHS = {"java14m": (PROD, PROD_B), "large": (LARGE_RED, 512)}
 
 
 @pytest.mark.parametrize("math", [1, 2])
-def test_production_width_fully_sharded_world8(monkeypatch, math):
+@pytest.mark.parametrize("shape", ["java14m", "large"])
+def test_production_width_fully_sharded_world8(monkeypatch, shape, math):
     world = 8
-    key = ("prod", world)
-    params = _cache.get(("prod-params",))
-    if params is None:
-        params = _cache[("prod-params",)] = O.init_params(PROD, seed=4321)
-        _cache[("prod-batch",)] = O.synthetic_batch(PROD, PROD_B, seed=1234)
-    batch = _cache[("prod-batch",)]
-    ref = reference(key, PROD, params, batch, world)
-    label = "prod fully_sharded world=8 math=%d" % math
-    out, engines = run_schedule(monkeypatch, PROD, params, batch, world, "fully_sharded", math, steps=1)
+    dims, B = WIDTHS[shape]
+    key = ("prod", shape)
+    if key not in _cache:            # one shape's reference at a time (about 2 GB for java14m, 5 GB for large)
+        for k in [k for k in _cache if k[0] in ("prod", "prod-inputs")]:
+            del _cache[k]
+        _cache[("prod-inputs", shape)] = (O.init_params(dims, seed=4321), O.synthetic_batch(dims, B, seed=1234))
+    params, batch = _cache[("prod-inputs", shape)]
+    ref = reference(key, dims, params, batch, world)
+    label = "%s fully_sharded world=8 math=%d" % (shape, math)
+    out, engines = run_schedule(monkeypatch, dims, params, batch, world, "fully_sharded", math, steps=1)
     print("workspace bytes, 8 engines: %d (%.2f GB)" % (sum(o["workspace"] for o in out),
                                                           sum(o["workspace"] for o in out) / 1e9))
-    worst = check_slots(out, engines, PROD, "fully_sharded", world, ref, math, label)
+    worst = check_slots(out, engines, dims, "fully_sharded", world, ref, math, label)
     worst["loss"] = check_loss(out, "fully_sharded", ref, label)
     worst.update(check_fs_phases(out, ref, params, math, label))
     assert [o["step1"]["fallbacks"] for o in out] == [0] * world

@@ -115,7 +115,7 @@ def test_sampler_refusals():
 
 
 # ---- one step against float64 --------------------------------------------------------------------------------------------
-@pytest.mark.parametrize("math", [0, 2])
+@pytest.mark.parametrize("math", [0, 1, 2])
 def test_step_sampled_against_float64(math):
     import torch
     from code2vec_b200.trainer import Trainer
@@ -139,7 +139,9 @@ def test_step_sampled_against_float64(math):
     assert abs(loss - ref.loss) < LOSS_TOL
     eng.sync_tables()
     label = "step_sampled math=%d" % math
-    report(label, check_adam_slots(eng, ref, math, O.PARAM_NAMES, label))
+    worst = check_adam_slots(eng, ref, math, O.PARAM_NAMES, label)
+    worst["loss"] = abs(loss - ref.loss)
+    report(label, worst)
     eng.close()
 
 
