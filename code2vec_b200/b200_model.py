@@ -148,6 +148,16 @@ def check_num_sampled(num_sampled: int, target_vocab: int) -> None:
                          "target words) negatives; lower it, or set 0 for the full softmax" % (num_sampled, limit, target_vocab))
 
 
+def sharded_sampled_flag(environ) -> bool:
+    """C2V_SHARDED_SAMPLED=1 (with C2V_NUM_SAMPLED=<S>): train() runs the sampled softmax on 2, 4 or 8 GPUs too, on the
+    fully sharded schedule (DESIGN.md §6j, "Several GPUs").  0 (the default) keeps the one-GPU-only refusal.  ValueError
+    for anything but 0 or 1."""
+    flag = environ.get("C2V_SHARDED_SAMPLED", "0") or "0"
+    if flag not in ("0", "1"):
+        raise ValueError("C2V_SHARDED_SAMPLED must be 0 or 1, got %r" % flag)
+    return flag == "1"
+
+
 _CKPT_MAGIC = CKPT_MAGIC
 _CKPT_SUFFIX = CKPT_SUFFIX
 
@@ -171,7 +181,11 @@ class Code2VecModel(Code2VecModelBase):
         check_multi_rank_run(config, self.world)
         # C2V_NUM_SAMPLED=<S>: train() runs the sampled softmax with S negatives drawn on the GPU (DESIGN.md §6j)
         self._num_sampled = num_sampled_flag(os.environ)
-        if self._num_sampled and self.world > 1:
+        # C2V_SHARDED_SAMPLED=1: the sampled softmax on several GPUs too, rows fetched from their owners (§6j)
+        self._sharded_sampled = sharded_sampled_flag(os.environ)
+        if self._sharded_sampled and not self._num_sampled:
+            raise ValueError("C2V_SHARDED_SAMPLED=1 trains the sampled softmax on several GPUs: it needs C2V_NUM_SAMPLED=<S>")
+        if self._num_sampled and self.world > 1 and not self._sharded_sampled:
             raise ValueError("C2V_NUM_SAMPLED=%d: the sampled softmax trains on one GPU and this run has %d ranks; unset "
                              "C2V_NUM_SAMPLED to train on several GPUs, or train in a single process" % (
                                  self._num_sampled, self.world))
@@ -275,6 +289,8 @@ class Code2VecModel(Code2VecModelBase):
                 self._num_sampled))
         elif self._num_sampled:
             self.log("C2V_NUM_SAMPLED=%d has no effect: this run does not train (no --data)" % self._num_sampled)
+        if self._sharded_sampled and self.world == 1:
+            self.log("C2V_SHARDED_SAMPLED=1 has no effect on one GPU: the sampled softmax runs its one-GPU step")
         if self.world > 1:
             # this rank's engine: a block of target rows, sized for the global batch (trainer.make_fully_sharded_engine)
             self.engine = make_fully_sharded_engine(self._engine_dims(), self.config.TRAIN_BATCH_SIZE // self.world,
@@ -298,6 +314,12 @@ class Code2VecModel(Code2VecModelBase):
             {0: "fp32 FFMA", 1: "tf32 tensor cores", 2: "3xTF32 tensor cores (fp32-equivalent)"}[self._math_eval]))
         # C2V_DETERMINISTIC / C2V_SEED: reproducible training runs (run_determinism)
         self._deterministic, self._seed = run_determinism(os.environ)
+        if self.world > 1 and self._num_sampled:
+            # every rank draws the sampled negatives from this seed, and a clock-derived one may differ between ranks
+            import torch.distributed as dist
+            seeds = [None] * self.world
+            dist.all_gather_object(seeds, self._seed)
+            self._seed = seeds[0]
         self.log("b200 backend run: deterministic = %d, seed = %d (C2V_DETERMINISTIC=%d C2V_SEED=%d replays it)" % (
             self._deterministic, self._seed, self._deterministic, self._seed))
         # C2V_HINT_NEXT=1: pass each next batch to the engine (c2v_hint_next_batch); off by default
@@ -494,7 +516,7 @@ class Code2VecModel(Code2VecModelBase):
         # synchronous c2v_train_batch_host path.
         # several GPUs: every rank reads the same global batches (same file, same shuffle seed) and steps on its slice
         multi = self.world > 1
-        num_sampled = self._num_sampled        # > 0: every step is Trainer.step_sampled (refused on several ranks)
+        num_sampled = self._num_sampled        # > 0: every step is Trainer.step_sampled (several ranks: C2V_SHARDED_SAMPLED=1)
         dropped_rows = 0
         ring = dev_reader = None
         if self._device_reader:
@@ -593,9 +615,12 @@ class Code2VecModel(Code2VecModelBase):
                         batch_loss = float(loss_hist[:n_hist].sum())
                         n_hist = 0
                 elif multi:                            # the fully sharded loss is already the mean over the global batch
-                    batch_loss = self.trainer.step_host(*(a[lo:hi] for a in (
-                        t.path_source_token_indices, t.path_indices, t.path_target_token_indices, t.context_valid_mask,
-                        t.target_index)))
+                    rows = tuple(a[lo:hi] for a in (t.path_source_token_indices, t.path_indices, t.path_target_token_indices,
+                                                    t.context_valid_mask, t.target_index))
+                    if num_sampled:
+                        batch_loss = self.trainer.step_host_sampled(*rows, num_sampled)
+                    else:
+                        batch_loss = self.trainer.step_host(*rows)
                 elif num_sampled:
                     batch_loss = self.trainer.step_host_sampled(t.path_source_token_indices, t.path_indices,
                                                                 t.path_target_token_indices, t.context_valid_mask,

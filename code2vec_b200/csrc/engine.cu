@@ -274,6 +274,10 @@ struct c2v_engine {
   int fuse_tgt = 0;                     // option "fuse_target_adam": c2v_train_batch_host arms itself
   int64_t tgt_fused_t = 0;              // step count whose target update has already been applied (0 = none)
   uint32_t sample_tag = 0;              // c2v_sample_log_uniform: tag of the last call (counts down; 0 = stamps not initialised)
+  bool cap_hits_zeroed = false;         // the sampler's cap-hit counter (workspace) has been cleared
+  unsigned long long* vstamp = nullptr; // c2v_sample_log_uniform_vocab: first-draw stamps of vstamp_Y classes (own allocation)
+  int32_t vstamp_Y = 0;
+  uint32_t vsample_tag = 0;             // as sample_tag, for vstamp
   int deterministic;
   int64_t launches;
   std::string err;
@@ -1644,6 +1648,7 @@ void c2v_destroy(c2v_engine* e) {
     if (e->ev_used[i]) cudaEventDestroy(e->ev_used[i]);
   }
   if (e->copy) cudaStreamDestroy(e->copy);
+  if (e->vstamp) cudaFree(e->vstamp);
   for (auto& L : e->phase) {
     for (auto& ev : L.pending) { cudaEventDestroy(ev.first); cudaEventDestroy(ev.second); }
     for (auto& ev : L.free_list) { cudaEventDestroy(ev.first); cudaEventDestroy(ev.second); }
@@ -1852,9 +1857,9 @@ int c2v_get_option(const c2v_engine* e, const char* key, int64_t* value) {
     }
     return C2V_OK;
   }
-  if (!strcmp(key, "sampler_cap_hits")) {         // c2v_sample_log_uniform calls that reached the draw cap (synchronises)
+  if (!strcmp(key, "sampler_cap_hits")) {         // sampler calls (either entry point) that reached the draw cap (synchronises)
     *value = 0;
-    if (e->wbase && e->sample_tag) {
+    if (e->wbase && e->cap_hits_zeroed) {
       int32_t n = 0;
       if (cudaDeviceSynchronize() != cudaSuccess ||
           cudaMemcpy(&n, e->wbase + e->ws.samp_status, 4, cudaMemcpyDeviceToHost) != cudaSuccess)
@@ -1989,12 +1994,53 @@ int c2v_sample_log_uniform(c2v_engine* e, int32_t S, const int32_t* target, int3
   // table never needs clearing -- except once at the start and after the 2^32 - 2 tags are used up
   if (e->sample_tag <= 1) {
     C2V_CUDA(e, cudaMemsetAsync(stamp, 0xFF, (size_t)Y * 8, st));
-    if (!e->sample_tag) C2V_CUDA(e, cudaMemsetAsync(cap_hits, 0, 4, st));
     e->sample_tag = 0xFFFFFFFFu;
+  }
+  if (!e->cap_hits_zeroed) {
+    C2V_CUDA(e, cudaMemsetAsync(cap_hits, 0, 4, st));
+    e->cap_hits_zeroed = true;
   }
   e->sample_tag--;
   PhaseTimer pt(e, PH_SAMPLER, st);
   C2V_LAUNCH(e, C2V_CUDA(e, launch_log_uniform_sampler(Y, log1p((double)Y), S, target, B, seed, step, e->sample_tag, stamp,
+                                                       sampled, logq_true, logq_sampled, num_tries, cap_hits, st)));
+  return C2V_OK;
+}
+
+int c2v_sample_log_uniform_vocab(c2v_engine* e, int32_t S, int32_t Y, const int32_t* target, int32_t B, uint64_t seed,
+                                 uint64_t step, int32_t* sampled, float* logq_true, float* logq_sampled, int64_t* num_tries,
+                                 void* stream) {
+  int rc = check_batch(e, B);
+  if (rc) return rc;
+  if (!target || !sampled || !logq_true || !logq_sampled) return fail(e, C2V_ERR_INVALID, "NULL argument");
+  if (Y < 2) return fail(e, C2V_ERR_INVALID, "the target vocabulary needs at least 2 classes");
+  if (S < 1 || S > kMaxSampled || S > Y / 2)
+    return fail(e, C2V_ERR_INVALID, "number of sampled classes must be in [1, min(1024, Y / 2)]");
+  C2V_CUDA(e, cudaSetDevice(e->device));
+  cudaStream_t st = (cudaStream_t)stream;
+  if (Y > e->vstamp_Y) {            // the first call (or a larger vocabulary): the stamp table is this call's own allocation
+    if (e->vstamp) {
+      C2V_CUDA(e, cudaStreamSynchronize(st));
+      C2V_CUDA(e, cudaFree(e->vstamp));
+      e->vstamp = nullptr;
+      e->vstamp_Y = 0;
+    }
+    C2V_CUDA(e, cudaMalloc((void**)&e->vstamp, (size_t)Y * 8));
+    e->vstamp_Y = Y;
+    e->vsample_tag = 0;
+  }
+  int32_t* cap_hits = wsp<int32_t>(e, e->ws.samp_status);
+  if (e->vsample_tag <= 1) {        // tags count down as in c2v_sample_log_uniform
+    C2V_CUDA(e, cudaMemsetAsync(e->vstamp, 0xFF, (size_t)e->vstamp_Y * 8, st));
+    e->vsample_tag = 0xFFFFFFFFu;
+  }
+  if (!e->cap_hits_zeroed) {
+    C2V_CUDA(e, cudaMemsetAsync(cap_hits, 0, 4, st));
+    e->cap_hits_zeroed = true;
+  }
+  e->vsample_tag--;
+  PhaseTimer pt(e, PH_SAMPLER, st);
+  C2V_LAUNCH(e, C2V_CUDA(e, launch_log_uniform_sampler(Y, log1p((double)Y), S, target, B, seed, step, e->vsample_tag, e->vstamp,
                                                        sampled, logq_true, logq_sampled, num_tries, cap_hits, st)));
   return C2V_OK;
 }
@@ -2250,6 +2296,81 @@ int c2v_context_backward(c2v_engine* e, const int32_t* src, const int32_t* path,
   const Dropout dp = make_dropout(e->dims, keep_prob, seed, step, dropout_mask);
   ContextSource cs = make_source(e, src, path, tgt, B);
   return context_backward(e, (cudaStream_t)stream, cs, mask, B, dp, dv);
+}
+
+// ---- sampled softmax on a row-sharded target table (fully sharded schedule) ------------------------------
+static bool rows_aligned(const void* p) { return ((uintptr_t)p % 16) == 0; }
+
+int c2v_sampled_pack_rows(c2v_engine* e, const int32_t* sampled, int32_t S, const int32_t* target_all, int32_t Bt,
+                          int32_t row_offset, float* neg_rows, float* true_rows, void* stream) {
+  int rc = check_batch(e, Bt);
+  if (rc) return rc;
+  if (!sampled || !target_all || !neg_rows || !true_rows) return fail(e, C2V_ERR_INVALID, "NULL argument");
+  if (S < 1 || S > kMaxSampled) return fail(e, C2V_ERR_INVALID, "number of sampled classes must be in [1, 1024]");
+  if (!e->has_theta) return fail(e, C2V_ERR_STATE, "parameters not bound");
+  if (!rows_aligned(neg_rows) || !rows_aligned(true_rows)) return fail(e, C2V_ERR_INVALID, "row buffers must be 16-byte aligned");
+  C2V_CUDA(e, cudaSetDevice(e->device));
+  cudaStream_t st = (cudaStream_t)stream;
+  const int D = e->dims.code_dim;
+  const size_t n4 = (size_t)(S + Bt) * (D / 4);
+  size_t blocks = (n4 + 255) / 256;
+  if (blocks > (size_t)e->num_sms * 16) blocks = (size_t)e->num_sms * 16;
+  PhaseTimer pt(e, PH_SAMPLED, st);
+  C2V_LAUNCH(e, (sampled_pack_rows_kernel<<<(unsigned)blocks, 256, 0, st>>>(e->theta.tgt, e->dims.target_vocab, row_offset, sampled, S,
+                                                                            target_all, Bt, D, neg_rows, true_rows)));
+  return C2V_OK;
+}
+
+int c2v_sampled_target_step(c2v_engine* e, const float* code_vec, int32_t B, const int32_t* target, const int32_t* sampled,
+                            int32_t S, const float* logq_true, const float* logq_sampled, const float* neg_rows,
+                            const float* true_rows, float inv_batch, float* dv, float* g_true, float* g_neg,
+                            float* loss_partial, void* stream) {
+  int rc = check_batch(e, B);
+  if (rc) return rc;
+  if (!code_vec || !target || !sampled || !logq_true || !logq_sampled || !neg_rows || !true_rows || !dv || !g_true || !g_neg ||
+      !loss_partial)
+    return fail(e, C2V_ERR_INVALID, "NULL argument");
+  if (S < 1 || S > kMaxSampled) return fail(e, C2V_ERR_INVALID, "number of sampled classes must be in [1, 1024]");
+  if (!rows_aligned(code_vec) || !rows_aligned(neg_rows) || !rows_aligned(true_rows))
+    return fail(e, C2V_ERR_INVALID, "code vectors and row buffers must be 16-byte aligned");
+  C2V_CUDA(e, cudaSetDevice(e->device));
+  cudaStream_t st = (cudaStream_t)stream;
+  const int D = e->dims.code_dim;
+  float* loss_b = wsp<float>(e, e->ws.loss_b);
+  float* dl = wsp<float>(e, e->ws.dl);
+  PhaseTimer pt(e, PH_SAMPLED, st);
+  const size_t smem = ((size_t)D + S + 1) * sizeof(float);
+  C2V_LAUNCH(e, (sampled_softmax_rows_fwd_kernel<<<B, kSampledThreads, smem, st>>>(code_vec, true_rows, neg_rows, target, sampled, S,
+                                                                                   logq_true, logq_sampled, D, inv_batch, loss_b, dl,
+                                                                                   dv)));
+  C2V_LAUNCH(e, (loss_reduce_kernel<<<1, 256, 0, st>>>(loss_b, B, inv_batch, loss_partial)));
+  C2V_LAUNCH(e, (sampled_true_grad_kernel<<<B, kSampledThreads, 0, st>>>(code_vec, dl, S, D, g_true)));
+  C2V_LAUNCH(e, (sampled_neg_grad_kernel<<<dim3(S, (D + 31) / 32), kNegGradWarps * 32, 0, st>>>(code_vec, dl, B, S, D, g_neg)));
+  return C2V_OK;
+}
+
+int c2v_sampled_target_fold(c2v_engine* e, const float* g_true_all, const float* g_neg_all, int32_t world,
+                            const int32_t* target_all, int32_t Bt, const int32_t* sampled, int32_t S, int32_t row_offset,
+                            const float* loss_parts, float* loss_out, void* stream) {
+  int rc = check_batch(e, Bt);
+  if (rc) return rc;
+  if (!g_true_all || !g_neg_all || !target_all || !sampled || !loss_parts || !loss_out)
+    return fail(e, C2V_ERR_INVALID, "NULL argument");
+  if (S < 1 || S > kMaxSampled) return fail(e, C2V_ERR_INVALID, "number of sampled classes must be in [1, 1024]");
+  if (world < 1 || world > kMaxShards) return fail(e, C2V_ERR_INVALID, "world out of range");
+  if (!e->has_grad) return fail(e, C2V_ERR_STATE, "gradients not bound (c2v_bind_grads)");
+  const int D = e->dims.code_dim;
+  if (D > kFoldThreads * kFoldCols) return fail(e, C2V_ERR_INVALID, "code_dim too large for the fold");
+  C2V_CUDA(e, cudaSetDevice(e->device));
+  cudaStream_t st = (cudaStream_t)stream;
+  const int Yl = e->dims.target_vocab;
+  PhaseTimer pt(e, PH_SAMPLED, st);
+  // the block may hold a full-softmax step's gradient (or a stale one after a fused Adam): every row is written here
+  C2V_CUDA(e, cudaMemsetAsync(e->grad.tgt, 0, (size_t)Yl * D * 4, st));
+  C2V_LAUNCH(e, (sampled_target_fold_kernel<<<Bt + S, kFoldThreads, 0, st>>>(g_true_all, g_neg_all, world, target_all, Bt, sampled, S,
+                                                                             D, row_offset, Yl, e->grad.tgt)));
+  C2V_LAUNCH(e, (sum_in_order_kernel<<<1, 1, 0, st>>>(loss_parts, world, loss_out)));
+  return C2V_OK;
 }
 
 int c2v_sync_tables(c2v_engine* e, void* stream) {

@@ -1934,4 +1934,195 @@ sampled_softmax_bwd_det_kernel(const float* __restrict__ v, const float* __restr
   }
 }
 
+// ---------------------------------------------------------------------------------------------
+// Sampled softmax on a row-sharded target table (fully sharded schedule, DESIGN.md section 6j): the rows move to the
+// examples.  Every rank draws the same S negatives; the owners pack the negative rows and the rows of the Bt examples'
+// targets into zero-filled buffers that one all-reduce / one reduce-scatter complete (each element has exactly one
+// non-zero contributor); every rank runs the head of sampled_softmax_fwd_kernel on its own Bl examples against the
+// compact rows, writes its partial target gradients, and after an all-gather the owners fold them in a fixed order.
+// ---------------------------------------------------------------------------------------------
+
+// Owner pack: row j of (neg_rows [S, D], true_rows [Bt, D]) = Ytab_local[id - row0] for id = sampled[j] resp. target[j]
+// when this rank holds global row id (row0 <= id < row0 + Yl), else zeros.  D % 4 == 0, rows 16-byte aligned.
+__global__ void __launch_bounds__(256)
+sampled_pack_rows_kernel(const float* __restrict__ Ytab, int Yl, int row0, const int32_t* __restrict__ sampled, int S,
+                         const int32_t* __restrict__ target, int Bt, int D, float* __restrict__ neg_rows,
+                         float* __restrict__ true_rows) {
+  const int D4 = D / 4;
+  const size_t n = (size_t)(S + Bt) * D4;
+  for (size_t k = (size_t)blockIdx.x * 256 + threadIdx.x; k < n; k += (size_t)gridDim.x * 256) {
+    const int j = (int)(k / D4), c = (int)(k % D4);
+    const int local = (j < S ? sampled[j] : target[j - S]) - row0;
+    float4 x = make_float4(0.f, 0.f, 0.f, 0.f);
+    if (local >= 0 && local < Yl) x = reinterpret_cast<const float4*>(Ytab + (size_t)local * D)[c];
+    float* dst = j < S ? neg_rows + (size_t)j * D : true_rows + (size_t)(j - S) * D;
+    reinterpret_cast<float4*>(dst)[c] = x;
+  }
+}
+
+// The head of sampled_softmax_fwd_kernel, operation for operation, with the rows read from the packed buffers: example b
+// (of this rank's B) scores true_rows[b] (its target's row) and neg_rows[s] (sampled[s]'s row) instead of Ytab[target[b]]
+// and Ytab[sampled[s]].  Writes loss_b [B], dl [B, 1+S] and dv [B, D].
+__global__ void __launch_bounds__(kSampledThreads)
+sampled_softmax_rows_fwd_kernel(const float* __restrict__ v, const float* __restrict__ true_rows,
+                                const float* __restrict__ neg_rows, const int32_t* __restrict__ target,
+                                const int32_t* __restrict__ sampled, int S, const float* __restrict__ logq_true,
+                                const float* __restrict__ logq_samp, int D, float inv_batch, float* __restrict__ loss_b,
+                                float* __restrict__ dl, float* __restrict__ dv) {
+  extern __shared__ float sm[];
+  float* vs = sm;                 // [D]
+  float* lg = vs + D;             // [1 + S]
+  __shared__ float red[32];
+  const int b = blockIdx.x, tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
+  const int y = target[b];
+  const float* yrow = true_rows + (size_t)b * D;
+  for (int i = tid; i < D; i += kSampledThreads) vs[i] = v[(size_t)b * D + i];
+  __syncthreads();
+  for (int j = warp; j <= S; j += kSampledThreads / 32) {
+    const float* r = (j == 0) ? yrow : neg_rows + (size_t)(j - 1) * D;
+    float part = 0.f;
+    for (int i = lane * 4; i < D; i += 128) {
+      const float4 a = *reinterpret_cast<const float4*>(r + i);
+      part += a.x * vs[i] + a.y * vs[i + 1] + a.z * vs[i + 2] + a.w * vs[i + 3];
+    }
+    part = warp_sum(part);
+    if (lane == 0) {
+      float l = part - ((j == 0) ? logq_true[b] : logq_samp[j - 1]);
+      if (j > 0 && sampled[j - 1] == y) l = -1e9f;          // accidental hit
+      lg[j] = l;
+    }
+  }
+  __syncthreads();
+  float m = -INFINITY;
+  for (int j = tid; j <= S; j += kSampledThreads) m = fmaxf(m, lg[j]);
+  m = block_max(m, red);
+  float s = 0.f;
+  for (int j = tid; j <= S; j += kSampledThreads) s += expf(lg[j] - m);
+  s = block_sum(s, red);
+  const float lse = m + logf(s);
+  if (tid == 0) loss_b[b] = lse - lg[0];
+  __syncthreads();
+  for (int j = tid; j <= S; j += kSampledThreads) {
+    float g = expf(lg[j] - lse);
+    if (j == 0) g -= 1.f;
+    g *= inv_batch;
+    if (j > 0 && sampled[j - 1] == y) g = 0.f;
+    lg[j] = g;
+    dl[(size_t)b * (S + 1) + j] = g;
+  }
+  __syncthreads();
+  for (int i = tid; i < D; i += kSampledThreads) {
+    float acc = lg[0] * yrow[i];
+    for (int j = 1; j <= S; ++j) acc += lg[j] * neg_rows[(size_t)(j - 1) * D + i];
+    dv[(size_t)b * D + i] = acc;
+  }
+}
+
+// One rank's true-row target gradient terms: g_true[b] = dl[b,0] v_b (one product each), one block per example.
+__global__ void __launch_bounds__(kSampledThreads)
+sampled_true_grad_kernel(const float* __restrict__ v, const float* __restrict__ dl, int S, int D, float* __restrict__ g_true) {
+  const int b = blockIdx.x;
+  const float g = dl[(size_t)b * (S + 1)];
+  for (int i = threadIdx.x; i < D; i += kSampledThreads) g_true[(size_t)b * D + i] = __fmul_rn(g, v[(size_t)b * D + i]);
+}
+
+// One rank's negative-row target gradients: g_neg[s] = the sums over b of dl[b,1+s] v_b in chunks of kSampledChunk
+// examples (each summed from 0 in b order, as sampled_softmax_bwd_det_kernel does), added chunk by chunk from +0.0f.
+// Block (s, column tile of 32): its warps sum different chunks of the same 32 columns into shared memory, and warp 0
+// adds them in chunk order, kNegGradRound chunks at a time -- so the S * D / 32 blocks fill the GPU even at small S and
+// the serial loop per warp is B / kNegGradWarps examples.  No atomics: every element is written once.
+constexpr int kNegGradWarps = 8;
+constexpr int kNegGradRound = 64;
+__global__ void __launch_bounds__(kNegGradWarps * 32)
+sampled_neg_grad_kernel(const float* __restrict__ v, const float* __restrict__ dl, int B, int S, int D,
+                        float* __restrict__ g_neg) {
+  __shared__ float part[kNegGradRound][32];
+  const int s = blockIdx.x, lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+  const int i = blockIdx.y * 32 + lane;
+  const int chunks = (B + kSampledChunk - 1) / kSampledChunk;
+  float acc = 0.f;
+  for (int q0 = 0; q0 < chunks; q0 += kNegGradRound) {
+    const int nq = min(kNegGradRound, chunks - q0);
+    for (int q = warp; q < nq; q += kNegGradWarps) {
+      const int b0 = (q0 + q) * kSampledChunk, b1 = min(B, b0 + kSampledChunk);
+      float c = 0.f;
+      if (i < D)
+        for (int b = b0; b < b1; ++b) c += dl[(size_t)b * (S + 1) + 1 + s] * v[(size_t)b * D + i];
+      part[q][lane] = c;
+    }
+    __syncthreads();
+    if (warp == 0)
+      for (int q = 0; q < nq; ++q) acc = __fadd_rn(acc, part[q][lane]);
+    __syncthreads();                                   // part is rewritten by the next round
+  }
+  if (warp == 0 && i < D) g_neg[(size_t)s * D + i] = acc;
+}
+
+// Owner fold of the partial target gradients.  The Bt + S row ids are read as one list L = (target[0..Bt), sampled[0..S));
+// block j handles row L[j] if this rank holds it and j is its first occurrence in L, and stores into g_tgt (local rows)
+//   from +0.0f, left to right: g_true[b] for every b (global example order) with target[b] == row, then for every s
+//   (in s order) with sampled[s] == row, g_neg[r][s] for r = 0 .. world-1.
+// Rows nobody references are not written (the caller clears the block first).  D <= kFoldThreads * kFoldCols.
+constexpr int kFoldThreads = 256;
+constexpr int kFoldCols = 4;
+__global__ void __launch_bounds__(kFoldThreads)
+sampled_target_fold_kernel(const float* __restrict__ g_true, const float* __restrict__ g_neg, int world,
+                           const int32_t* __restrict__ target, int Bt, const int32_t* __restrict__ sampled, int S, int D,
+                           int row0, int Yl, float* __restrict__ g_tgt) {
+  __shared__ unsigned hits[kFoldThreads / 32];
+  const int j = blockIdx.x, tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
+  const int row = j < Bt ? target[j] : sampled[j - Bt];
+  const int local = row - row0;
+  if (local < 0 || local >= Yl) return;                              // another rank's row
+  int dup = 0;
+  for (int q = tid; q < j; q += kFoldThreads) dup |= (q < Bt ? target[q] : sampled[q - Bt]) == row;
+  if (__syncthreads_or(dup)) return;                                 // not the first occurrence
+  float acc[kFoldCols];
+#pragma unroll
+  for (int k = 0; k < kFoldCols; ++k) acc[k] = 0.f;
+  // the matching entries of each tile of kFoldThreads, taken in index order
+  auto fold_tile = [&](int base, bool hit, auto&& add) {
+    const unsigned m = __ballot_sync(0xffffffffu, hit);
+    if (lane == 0) hits[warp] = m;
+    __syncthreads();
+    for (int w = 0; w < kFoldThreads / 32; ++w)
+      for (unsigned bits = hits[w]; bits; bits &= bits - 1) add(base + w * 32 + __ffs(bits) - 1);
+    __syncthreads();
+  };
+  for (int b0 = 0; b0 < Bt; b0 += kFoldThreads) {
+    const int b = b0 + tid;
+    fold_tile(b0, b < Bt && target[b] == row, [&](int e) {
+#pragma unroll
+      for (int k = 0; k < kFoldCols; ++k) {
+        const int i = tid + k * kFoldThreads;
+        if (i < D) acc[k] = __fadd_rn(acc[k], g_true[(size_t)e * D + i]);
+      }
+    });
+  }
+  for (int s0 = 0; s0 < S; s0 += kFoldThreads) {
+    const int s = s0 + tid;
+    fold_tile(s0, s < S && sampled[s] == row, [&](int e) {
+      for (int r = 0; r < world; ++r) {
+#pragma unroll
+        for (int k = 0; k < kFoldCols; ++k) {
+          const int i = tid + k * kFoldThreads;
+          if (i < D) acc[k] = __fadd_rn(acc[k], g_neg[((size_t)r * S + e) * D + i]);
+        }
+      }
+    });
+  }
+#pragma unroll
+  for (int k = 0; k < kFoldCols; ++k) {
+    const int i = tid + k * kFoldThreads;
+    if (i < D) g_tgt[(size_t)local * D + i] = acc[k];
+  }
+}
+
+// out[0] = parts[0] + parts[1] + ... + parts[n-1], left to right from +0.0f (one thread)
+__global__ void sum_in_order_kernel(const float* __restrict__ parts, int n, float* __restrict__ out) {
+  float acc = 0.f;
+  for (int r = 0; r < n; ++r) acc = __fadd_rn(acc, parts[r]);
+  out[0] = acc;
+}
+
 }  // namespace c2v

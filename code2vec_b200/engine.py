@@ -80,6 +80,7 @@ _SIGNATURES = {
     "c2v_sampled_train_step": (C.c_int, [_P, _P, _P, _P, _P, _P, _I32, _P, _I32, _P, _P, C.c_float,
                                          C.c_uint64, C.c_uint64, _P, _P, _P]),
     "c2v_sample_log_uniform": (C.c_int, [_P, _I32, _P, _I32, C.c_uint64, C.c_uint64, _P, _P, _P, _P, _P]),
+    "c2v_sample_log_uniform_vocab": (C.c_int, [_P, _I32, _I32, _P, _I32, C.c_uint64, C.c_uint64, _P, _P, _P, _P, _P]),
     "c2v_adam_step": (C.c_int, [_P, C.c_float, C.c_float, C.c_float, C.c_float, C.c_int64, _P]),
     "c2v_arm_target_adam": (C.c_int, [_P, C.c_float, C.c_float, C.c_float, C.c_float, C.c_int64]),
     "c2v_hint_next_batch": (C.c_int, [_P, _P, _P, _P, _I32]),
@@ -117,6 +118,9 @@ _SIGNATURES = {
     "c2v_lse_combine": (C.c_int, [_P, _P, _P, _I32, _I32, _P, C.c_float, _P, _P, _P]),
     "c2v_target_backward": (C.c_int, [_P, _P, _I32, _P, _P, _I32, C.c_float, _P, _P]),
     "c2v_context_backward": (C.c_int, [_P, _P, _P, _P, _P, _I32, C.c_float, C.c_uint64, C.c_uint64, _P, _P, _P]),
+    "c2v_sampled_pack_rows": (C.c_int, [_P, _P, _I32, _P, _I32, _I32, _P, _P, _P]),
+    "c2v_sampled_target_step": (C.c_int, [_P, _P, _I32, _P, _P, _I32, _P, _P, _P, _P, C.c_float, _P, _P, _P, _P, _P]),
+    "c2v_sampled_target_fold": (C.c_int, [_P, _P, _P, _I32, _P, _I32, _P, _I32, _I32, _P, _P, _P]),
     "c2v_topk_partial": (C.c_int, [_P, _P, _I32, _I32, _I32, _P, _P, _P, _P, _P]),
     "c2v_topk_merge": (C.c_int, [_P, _P, _P, _P, _P, _I32, _I32, _I32, _I32, _I32, _I32, _P, _P, _P]),
     "c2v_launch_count": (C.c_int64, [_P]),
@@ -559,17 +563,30 @@ class PathAttentionEngine:
         """c2v_sample_log_uniform: the S unique log-uniform candidates of (seed, step) and the log expected counts of
         them and of target [B] (device int32), as device tensors (sampled int32 [S], logq_true [B], logq_sampled [S],
         num_tries int64 [1]).  The buffers are the engine's own and the next call overwrites them."""
-        torch = self.torch
         B, S = int(target.shape[0]), int(S)
+        sampled, lq_t, lq_s, tries = self._sampler_buffers(B, S)
+        self._check(self.lib.c2v_sample_log_uniform(self.h, S, target.data_ptr(), B, int(seed), int(step), sampled.data_ptr(),
+                                                    lq_t.data_ptr(), lq_s.data_ptr(), tries.data_ptr(), self._stream()))
+        return sampled, lq_t, lq_s, tries
+
+    def sample_log_uniform_vocab(self, target, S: int, Y: int, seed: int, step: int):
+        """c2v_sample_log_uniform_vocab: sample_log_uniform over Y classes (a row-sharded engine passes the global target
+        vocabulary, so every rank draws what a one-GPU engine draws for (seed, step)).  Same buffers and results."""
+        B, S = int(target.shape[0]), int(S)
+        sampled, lq_t, lq_s, tries = self._sampler_buffers(B, S)
+        self._check(self.lib.c2v_sample_log_uniform_vocab(self.h, S, int(Y), target.data_ptr(), B, int(seed), int(step),
+                                                          sampled.data_ptr(), lq_t.data_ptr(), lq_s.data_ptr(),
+                                                          tries.data_ptr(), self._stream()))
+        return sampled, lq_t, lq_s, tries
+
+    def _sampler_buffers(self, B: int, S: int):
+        torch = self.torch
         buf = getattr(self, "_sampler_out", None)
         if buf is None:          # sized once for the largest call the ABI accepts: S <= 1024, B <= max_batch
             z = lambda n, dt: torch.empty(n, dtype=dt, device=self.dev)
             buf = self._sampler_out = (z(1024, torch.int32), z(self.dims.max_batch, torch.float32), z(1024, torch.float32),
                                        z(1, torch.int64))
-        sampled, lq_t, lq_s, tries = buf[0][:S], buf[1][:B], buf[2][:S], buf[3]
-        self._check(self.lib.c2v_sample_log_uniform(self.h, S, target.data_ptr(), B, int(seed), int(step), sampled.data_ptr(),
-                                                    lq_t.data_ptr(), lq_s.data_ptr(), tries.data_ptr(), self._stream()))
-        return sampled, lq_t, lq_s, tries
+        return buf[0][:S], buf[1][:B], buf[2][:S], buf[3]
 
     def adam_step(self, lr=1e-3, beta1=0.9, beta2=0.999, eps=1e-8, t: Optional[int] = None):
         if t is None:
@@ -628,6 +645,32 @@ class PathAttentionEngine:
         self._check(self.lib.c2v_context_backward(self.h, src.data_ptr(), path.data_ptr(), tgt.data_ptr(), mask.data_ptr(),
                                                   src.shape[0], float(keep), int(seed), int(step), _ptr(dropout_mask),
                                                   dv.data_ptr(), self._stream()))
+
+    # ---- sampled softmax on a row-sharded target table (fully sharded schedule) -------------------------
+    def sampled_pack_rows(self, sampled, target_all, row_offset, neg_rows, true_rows):
+        """c2v_sampled_pack_rows: the rows of sampled [S] / target_all [Bt] this engine holds into neg_rows [S, D] /
+        true_rows [Bt, D], zeros elsewhere."""
+        self._check(self.lib.c2v_sampled_pack_rows(self.h, sampled.data_ptr(), sampled.shape[0], target_all.data_ptr(),
+                                                   target_all.shape[0], int(row_offset), neg_rows.data_ptr(),
+                                                   true_rows.data_ptr(), self._stream()))
+
+    def sampled_target_step(self, code_vec, target, sampled, logq_true, logq_sampled, neg_rows, true_rows, inv_batch,
+                            dv, g_true, g_neg, loss_partial):
+        """c2v_sampled_target_step: the sampled head of this rank's examples against the packed rows -> dv [B, D], the
+        partial target gradients g_true [B, D] / g_neg [S, D] and loss_partial [1]."""
+        self._check(self.lib.c2v_sampled_target_step(
+            self.h, code_vec.data_ptr(), code_vec.shape[0], target.data_ptr(), sampled.data_ptr(), sampled.shape[0],
+            logq_true.data_ptr(), logq_sampled.data_ptr(), neg_rows.data_ptr(), true_rows.data_ptr(), float(inv_batch),
+            dv.data_ptr(), g_true.data_ptr(), g_neg.data_ptr(), loss_partial.data_ptr(), self._stream()))
+
+    def sampled_target_fold(self, g_true_all, g_neg_all, target_all, sampled, row_offset, loss_parts, loss_out):
+        """c2v_sampled_target_fold: every rank's partial gradients g_true_all [Bt, D] / g_neg_all [world, S, D] -> this
+        engine's target gradient block (cleared first), and loss_out [1] = the sum of loss_parts [world] in rank order."""
+        world, S = g_neg_all.shape[0], sampled.shape[0]
+        self._check(self.lib.c2v_sampled_target_fold(self.h, g_true_all.data_ptr(), g_neg_all.data_ptr(), world,
+                                                     target_all.data_ptr(), target_all.shape[0], sampled.data_ptr(), S,
+                                                     int(row_offset), loss_parts.data_ptr(), loss_out.data_ptr(),
+                                                     self._stream()))
 
     # ---- prediction against a row-sharded target table (fully sharded schedule) ------------------------
     def topk_partial(self, code_all, row_offset, k, idx, val, row_max=None, row_sum=None):

@@ -303,11 +303,15 @@ class Trainer:
 
     def step_sampled(self, src, path, tgt, mask, target, num_sampled: int):
         """One sampled-softmax training step whose num_sampled negatives are drawn on the device for (seed, t = adam_t + 1)
-        (c2v_sample_log_uniform, DESIGN.md section 6j), then step_device_sampled.  Single GPU; returns the device loss
-        without a sync.  The draw depends on the step count only, so a run resumed from a checkpoint (which restores
-        adam_t) continues the same negatives."""
+        (c2v_sample_log_uniform, DESIGN.md section 6j), then step_device_sampled.  Returns the device loss without a sync.
+        The draw depends on the step count only, so a run resumed from a checkpoint (which restores adam_t) continues the
+        same negatives.  One GPU, or the fully sharded schedule (_fully_sharded_sampled_step): there every rank draws
+        the negatives of the one-GPU run with the same seed over the global vocabulary."""
+        if self.schedule == "fully_sharded":
+            return self._fully_sharded_sampled_step(src, path, tgt, mask, target, int(num_sampled))
         if self.schedule != "single":
-            raise RuntimeError("the sampled-softmax step is single-GPU")
+            raise RuntimeError("the sampled-softmax step runs on one GPU or on the fully_sharded schedule, not on %r"
+                               % self.schedule)
         e = self.e
         sampled, lq_t, lq_s, _ = e.sample_log_uniform(target, num_sampled, self.seed, e.adam_t + 1)
         return self.step_device_sampled(src, path, tgt, mask, target, sampled, lq_t, lq_s)
@@ -413,6 +417,70 @@ class Trainer:
         e.target_backward(fs["v_all"], fs["lse"], fs["tgt_all"], e.target_row0, fs["dv_part"])
         dist.reduce_scatter_tensor(fs["dv_local"], fs["dv_part"], op=dist.ReduceOp.SUM, group=self.group)
         e.context_backward(src, path, tgt, mask, fs["dv_local"], keep=self.keep, seed=seed, step=t)
+        self._fully_sharded_update(t)
+        return fs["loss"]
+
+    def _sampled_views(self, B: int, S: int):
+        """The sampled step's buffers for a local batch of B rows and S negatives (allocated for the engine's local batch
+        at the first call with this S): packed rows, partial target gradients and loss partials."""
+        e, torch = self.e, self.e.torch
+        buf = getattr(self, "_fss", None)
+        if buf is None or buf["S"] != S:
+            W, Bl, D = self.world, e.local_batch, e.dims.code_dim
+            z = lambda *shape: torch.zeros(shape, dtype=torch.float32, device=e.dev)
+            buf = self._fss = dict(S=S, neg=z(S, D), true_send=z(W * Bl, D), true=z(Bl, D), g_neg=z(S, D),
+                                   g_neg_all=z(W, S, D), g_true=z(Bl, D), g_true_all=z(W * Bl, D), loss_part=z(1),
+                                   loss_parts=z(W))
+        if B == e.local_batch:
+            return buf
+        v = dict(buf)
+        for name in ("true", "g_true"):
+            v[name] = buf[name][:B]
+        for name in ("true_send", "g_true_all"):
+            v[name] = buf[name][:B * self.world]
+        return v
+
+    def _fully_sharded_sampled_step(self, src, path, tgt, mask, target, S: int):
+        """The sampled-softmax step of the fully sharded schedule (DESIGN.md section 6j): the rows move to the examples.
+        Every rank draws the same S negatives over the global vocabulary for (self.seed, t); the owners pack those rows
+        and their block's rows of the Bt targets (one all-reduce and one reduce-scatter, each element with one non-zero
+        contributor, so both exact); each rank runs the head on its own examples, and the partial target gradients are
+        all-gathered and folded by the owners in a fixed order.  The dY-epilogue Adam is not armed: the target block
+        takes the dense Adam of _fully_sharded_update."""
+        e, dist = self.e, _dist()
+        if not getattr(self, "_seed_agreed", False):
+            # the packed rows are summed over ranks: a rank that drew other negatives would add rows of other ids
+            seeds = [None] * self.world
+            dist.all_gather_object(seeds, self.seed, group=self.group)
+            if len(set(seeds)) > 1:
+                raise ValueError("the sampled-softmax step on the fully_sharded schedule needs the same Trainer seed on "
+                                 "every rank (every rank draws the same negatives from it); got seeds %s" % seeds)
+            self._seed_agreed = True
+        t = e.adam_t + 1
+        Bl = int(src.shape[0])
+        fs, ss = self._fs_views(Bl), self._sampled_views(Bl, S)
+        seed = self.seed + self.rank
+        e.context_forward(src, path, tgt, mask, fs["v_local"], keep=self.keep, seed=seed, step=t)
+        dist.all_gather_into_tensor(fs["tgt_all"], target, group=self.group)
+        sampled, lq_t, lq_s, _ = e.sample_log_uniform_vocab(target, S, e.global_target_vocab, self.seed, t)
+        e.sampled_pack_rows(sampled, fs["tgt_all"], e.target_row0, ss["neg"], ss["true_send"])
+        dist.all_reduce(ss["neg"], op=dist.ReduceOp.SUM, group=self.group)
+        dist.reduce_scatter_tensor(ss["true"], ss["true_send"], op=dist.ReduceOp.SUM, group=self.group)
+        e.sampled_target_step(fs["v_local"], target, sampled, lq_t, lq_s, ss["neg"], ss["true"], 1.0 / (Bl * self.world),
+                              fs["dv_local"], ss["g_true"], ss["g_neg"], ss["loss_part"])
+        dist.all_gather_into_tensor(ss["g_neg_all"], ss["g_neg"], group=self.group)
+        dist.all_gather_into_tensor(ss["g_true_all"], ss["g_true"], group=self.group)
+        dist.all_gather_into_tensor(ss["loss_parts"], ss["loss_part"], group=self.group)
+        e.sampled_target_fold(ss["g_true_all"], ss["g_neg_all"], fs["tgt_all"], sampled, e.target_row0, ss["loss_parts"],
+                              fs["loss"])
+        e.context_backward(src, path, tgt, mask, fs["dv_local"], keep=self.keep, seed=seed, step=t)
+        self._fully_sharded_update(t)
+        return fs["loss"]
+
+    def _fully_sharded_update(self, t: int):
+        """The fully sharded step's tail: the small gradients, the inbox fold and Adam on this rank's shards."""
+        e, dist = self.e, _dist()
+        fs = self._fs
         s0, s1 = self._small
         # sum (not mean): dv already carries 1/global batch.  Completion == every rank's scatter-add has landed.
         dist.all_reduce(e.flat_grads[s0:s1], op=dist.ReduceOp.SUM, group=self.group)
@@ -428,7 +496,6 @@ class Trainer:
         e.adam_step_range(e.flat_params[s0:s1], e.flat_grads[s0:s1], e.flat_m[s0:s1], e.flat_v[s0:s1], t, **self.adam)
         # every shard must be updated before any rank's next gather reads it
         dist.all_reduce(fs["token"], group=self.group)
-        return fs["loss"]
 
     def _table_sharded_update(self, t: int):
         e, torch = self.e, self.e.torch

@@ -237,9 +237,21 @@ int c2v_sampled_train_step(c2v_engine* e, const int32_t* src, const int32_t* pat
  * device int64 [1] or NULL.  Asynchronous on `stream`, writes device memory only, allocates nothing (the workspace holds
  * 8 bytes per target class of first-draw stamps).  At most 2^31 draws: a call that reaches that cap without S distinct
  * values fills the missing ids with class 0, reports num_tries = 2^31 and counts itself in the read-only option
- * "sampler_cap_hits" (the read synchronises). */
+ * "sampler_cap_hits" (the read synchronises; it counts the calls of c2v_sample_log_uniform_vocab too). */
 int c2v_sample_log_uniform(c2v_engine* e, int32_t S, const int32_t* target, int32_t B, uint64_t seed, uint64_t step,
                            int32_t* sampled, float* logq_true, float* logq_sampled, int64_t* num_tries, void* stream);
+
+/* c2v_sample_log_uniform over an explicit vocabulary of Y classes instead of target_vocab: the same draws, uniqueness,
+ * num_tries and log counts, bit for bit, as c2v_sample_log_uniform on an engine whose target_vocab is Y.  Accepted on
+ * row-sharded engines, where target_vocab is this rank's block and Y the global vocabulary: every rank that calls it with
+ * the same (seed, step) draws the same sampled [S] and logq_sampled [S], and logq_true [B] of its own target ids (global
+ * class ids).  NOT IN THE REFERENCE (DESIGN.md section 6j).  2 <= Y, 1 <= S <= min(1024, Y / 2), 1 <= B <= max_batch,
+ * else C2V_ERR_INVALID.  The first-draw stamps (8 bytes per class, 2.09 MB at Y = 261,246) are not in the workspace: the
+ * first call allocates them (cudaMalloc) and c2v_destroy frees them; a later call with a larger Y synchronises `stream`
+ * and allocates again.  A call that reaches the draw cap counts in "sampler_cap_hits" as c2v_sample_log_uniform does. */
+int c2v_sample_log_uniform_vocab(c2v_engine* e, int32_t S, int32_t Y, const int32_t* target, int32_t B, uint64_t seed,
+                                 uint64_t step, int32_t* sampled, float* logq_true, float* logq_sampled, int64_t* num_tries,
+                                 void* stream);
 
 /* tf.compat.v1.train.AdamOptimizer() update of all five variables from the bound gradients
  * (tensorflow_model.py:232): lr_t = lr*sqrt(1-b2^t)/(1-b1^t); m,v decay on EVERY row (TF1's
@@ -305,6 +317,43 @@ int c2v_target_backward(c2v_engine* e, const float* code_all, int32_t Bt, const 
 int c2v_context_backward(c2v_engine* e, const int32_t* src, const int32_t* path, const int32_t* tgt,
                          const float* mask, int32_t B, float keep_prob, uint64_t seed, uint64_t step,
                          const float* dropout_mask, const float* dv, void* stream);
+
+/* ---- Sampled softmax on a row-sharded target table (the fully sharded schedule) -----------------------
+ * NOT IN THE REFERENCE (DESIGN.md section 6j).  The same engine as the phase-split step (target_vocab = LOCAL rows
+ * [row_offset, row_offset + target_vocab), max_batch = GLOBAL batch Bt = world * B).  The rows move to the examples: every
+ * rank draws the same S negatives (c2v_sample_log_uniform_vocab with the global Y and the same seed and step), and a step
+ * runs, after c2v_context_forward and an all-gather of the targets into target_all [Bt]:
+ *   c2v_sampled_pack_rows   : neg_rows [S, D] row s = Ytab[sampled[s]] and true_rows [Bt, D] row b = Ytab[target_all[b]]
+ *                             where this rank holds that row, else zeros.  The caller then all-reduces (sum) neg_rows and
+ *                             reduce-scatters (sum) true_rows into its own [B, D] rows; each element has one non-zero
+ *                             contributor, so both sums are exact in any order (a -0.0 may become +0.0).
+ *   c2v_sampled_target_step : c2v_sampled_train_step's head (fp32 SIMT in every math mode, same operations) on this rank's
+ *                             B examples code_vec [B, D] / target [B] (global ids) against the packed rows: logits over
+ *                             {true row, S negatives} minus logq_true [B] / logq_sampled [S], accidental hits masked,
+ *                             dl = (p - onehot) * inv_batch (pass 1/Bt).  Writes dv [B, D] (c2v_context_backward's input,
+ *                             no reduce-scatter needed), loss_partial [1] = (sum_b loss_b) * inv_batch over these B
+ *                             examples (fixed order), g_true [B, D] = dl[b,0] * v_b (one product each) and g_neg [S, D] =
+ *                             for each s the sums over b of dl[b,1+s] v_b in chunks of 64 examples, added chunk by chunk
+ *                             from +0.0f.  No atomics.
+ *   c2v_sampled_target_fold : after all-gathers of g_true into g_true_all [Bt, D] (global example order), of g_neg into
+ *                             g_neg_all [world, S, D] and of loss_partial into loss_parts [world]: clears the bound target
+ *                             gradient block, then stores for every row this rank holds that target_all or sampled
+ *                             references, from +0.0f and left to right, g_true_all[b] for each b with target_all[b] == row
+ *                             (b order), then for each s with sampled[s] == row (s order) g_neg_all[r][s] for r = 0 ..
+ *                             world-1.  loss_out [1] = loss_parts[0] + ... + loss_parts[world-1], left to right from +0.0f,
+ *                             the same on every rank.  The target block then takes c2v_adam_step_range (dense TF1 Adam).
+ * The whole target side is deterministic by construction.  1 <= S <= 1024, 1 <= B, Bt <= max_batch, 1 <= world <= 8,
+ * code_dim <= 1024; code vectors and row buffers 16-byte aligned; else C2V_ERR_INVALID.  The fold needs bound gradients
+ * (C2V_ERR_STATE).  Asynchronous on `stream`; dl and the per-example losses live in the workspace. */
+int c2v_sampled_pack_rows(c2v_engine* e, const int32_t* sampled, int32_t S, const int32_t* target_all, int32_t Bt,
+                          int32_t row_offset, float* neg_rows, float* true_rows, void* stream);
+int c2v_sampled_target_step(c2v_engine* e, const float* code_vec, int32_t B, const int32_t* target, const int32_t* sampled,
+                            int32_t S, const float* logq_true, const float* logq_sampled, const float* neg_rows,
+                            const float* true_rows, float inv_batch, float* dv, float* g_true, float* g_neg,
+                            float* loss_partial, void* stream);
+int c2v_sampled_target_fold(c2v_engine* e, const float* g_true_all, const float* g_neg_all, int32_t world,
+                            const int32_t* target_all, int32_t Bt, const int32_t* sampled, int32_t S, int32_t row_offset,
+                            const float* loss_parts, float* loss_out, void* stream);
 
 /* ---- Prediction against a row-sharded target table (the fully sharded schedule) -----------------------
  * The same engine as the phase-split step (target_vocab = LOCAL rows, max_batch = GLOBAL batch Bt).
