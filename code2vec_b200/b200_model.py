@@ -26,17 +26,19 @@ import numpy as np
 
 from .common import common
 from .config import Config
-from .engine import PARAM_NAMES, EngineDims, PathAttentionEngine
+from .engine import PARAM_NAMES, EngineDims, PathAttentionEngine, crc32c_combine, crc32c_rows, tensor_crc32c
 from .model_base import Code2VecModelBase, ModelEvaluationResults, ModelPredictionResults
 from .path_context_reader import EstimatorAction, ModelInputTensorsFormer, PathContextReader, ReaderInputTensors
 from .multi_rank import (CKPT_MAGIC, CKPT_SUFFIX, batch_split, check_checkpoint_dims, check_multi_rank_run,
-                         checkpoint_header, create_checkpoint_file, read_checkpoint_header, read_checkpoint_part, run_world,
-                         write_checkpoint, write_checkpoint_part)
+                         checkpoint_header, create_checkpoint_file, read_checkpoint_header, read_checkpoint_part,
+                         read_entries_part, run_world, write_checkpoint, write_checkpoint_part)
+from .tf_bundle import INDEX_SUFFIX, bundle_entries, bundle_layout, crc_view, data_file, save_format_flag, write_index
+from .tf_bundle import crc32c as host_crc32c
 from . import device_reader as _device_reader_mod
 from .device_reader import device_eval_flag, device_reader_flag, sharded_reader_flag
 from .device_predict import device_predict_flag
 from .text_export import DeviceTextWriter, device_text_flag
-from .trainer import Trainer, make_fully_sharded_engine
+from .trainer import ADAM_DEFAULTS, Trainer, make_fully_sharded_engine
 from .vocabularies import VocabType
 
 
@@ -158,6 +160,74 @@ def sharded_sampled_flag(environ) -> bool:
     return flag == "1"
 
 
+class _PinnedStaging:
+    """Two page-locked buffers between files and device tensors, as DeviceTextWriter has (DESIGN.md §6f): the host
+    fills or drains one while the other's copy runs on the current stream."""
+    CHUNK_BYTES = 64 << 20
+
+    def __init__(self, dev, chunk_bytes: int = CHUNK_BYTES):
+        import torch
+        self.torch = torch
+        self.dev = torch.device(dev)
+        self.chunk = int(chunk_bytes)
+        self.buf = [torch.empty(self.chunk, dtype=torch.uint8, pin_memory=True) for _ in range(2)]
+        self.events = [None, None]
+        self.slot = 0
+
+    def __enter__(self):
+        return self
+
+    def __exit__(self, *exc):
+        for ev in self.events:
+            if ev is not None:
+                ev.synchronize()
+        self.buf = self.events = None
+
+    def _take(self) -> int:
+        s = self.slot
+        self.slot ^= 1
+        if self.events[s] is not None:
+            self.events[s].synchronize()
+        return s
+
+    def _mark(self, s: int):
+        ev = self.torch.cuda.Event()
+        ev.record(self.torch.cuda.current_stream(self.dev))
+        self.events[s] = ev
+
+    def upload(self, path: str, offset: int, nbytes: int, t):
+        """Bytes [offset, offset + nbytes) of the file into the contiguous device tensor t."""
+        dst = t.view(-1).view(self.torch.uint8)
+        with open(path, "rb") as f:
+            f.seek(offset)
+            for o in range(0, nbytes, self.chunk):
+                n = min(self.chunk, nbytes - o)
+                s = self._take()
+                if f.readinto(memoryview(self.buf[s].numpy())[:n]) != n:
+                    raise ValueError("`%s` ends inside the tensor at offset %d" % (path, offset))
+                dst[o:o + n].copy_(self.buf[s][:n], non_blocking=True)
+                self._mark(s)
+
+    def download(self, t, f):
+        """The bytes of the contiguous device tensor t appended to the binary file f."""
+        src = t.reshape(-1).view(self.torch.uint8)
+        pending = None
+        for o in range(0, src.numel(), self.chunk):
+            n = min(self.chunk, src.numel() - o)
+            s = self._take()
+            self.buf[s][:n].copy_(src[o:o + n], non_blocking=True)
+            self._mark(s)
+            if pending is not None:
+                self._write(f, *pending)
+            pending = (s, n)
+        if pending is not None:
+            self._write(f, *pending)
+
+    def _write(self, f, s: int, n: int):
+        self.events[s].synchronize()
+        f.write(memoryview(self.buf[s].numpy())[:n])
+
+
 _CKPT_MAGIC = CKPT_MAGIC
 _CKPT_SUFFIX = CKPT_SUFFIX
 
@@ -178,7 +248,9 @@ class Code2VecModel(Code2VecModelBase):
         self.world, self.local_rank = run_world(os.environ)
         self.rank = 0
         self._own_group = False
-        check_multi_rank_run(config, self.world)
+        # C2V_SAVE_FORMAT=tf: save() and --release write TensorFlow V2 checkpoints (tf_bundle.py, DESIGN.md §6k)
+        self._save_format = save_format_flag(os.environ)
+        check_multi_rank_run(config, self.world, self._save_format)
         # C2V_NUM_SAMPLED=<S>: train() runs the sampled softmax with S negatives drawn on the GPU (DESIGN.md §6j)
         self._num_sampled = num_sampled_flag(os.environ)
         # C2V_SHARDED_SAMPLED=1: the sampled softmax on several GPUs too, rows fetched from their owners (§6j)
@@ -357,10 +429,15 @@ class Code2VecModel(Code2VecModelBase):
             self.log("variable name: {} -- shape: {} -- #params: {}".format(name, shape, int(np.prod(shape))))
 
     def _load_inner_model(self):
+        """`X.c2v_b200` when it exists, else the TensorFlow checkpoint `X.index` + `X.data-*` when that exists."""
         self._make_engine()
         path = self.config.MODEL_LOAD_PATH + _CKPT_SUFFIX
-        self.log("Loading model weights from: " + path)
-        self._read_checkpoint(path)
+        if not os.path.isfile(path) and os.path.isfile(self.config.MODEL_LOAD_PATH + INDEX_SUFFIX):
+            self.log("Loading model weights from the TensorFlow checkpoint: " + self.config.MODEL_LOAD_PATH)
+            (self._read_sharded_bundle if self.world > 1 else self._read_bundle)(self.config.MODEL_LOAD_PATH)
+        else:
+            self.log("Loading model weights from: " + path)
+            self._read_checkpoint(path)
         self.log("Done loading model weights")
 
     def close_session(self):
@@ -405,6 +482,8 @@ class Code2VecModel(Code2VecModelBase):
     def _save_inner_model(self, path: str, release: bool = False):
         if self.world > 1:
             return self._save_sharded(path)
+        if self._save_format == "tf":
+            return self._save_bundle(path, release)
         e = self.engine
         e.sync_tables()                                  # lazy Adam: replay deferred row updates before reading the tensors
         tensors = [e.params[k] for k in PARAM_NAMES]
@@ -464,6 +543,112 @@ class Code2VecModel(Code2VecModelBase):
                 e.set_option("adam_step_count", e.adam_t)
             torch.cuda.synchronize(e.dev)
         self._all_ok(read_rows)                          # every shard is loaded before any peer reads it
+
+    # ---- TensorFlow V2 checkpoints (tf_bundle.py, DESIGN.md §6k) -------------------------------------------------
+    def _adam_betas(self):
+        adam = self._ADAM or ADAM_DEFAULTS
+        return adam["beta1"], adam["beta2"]
+
+    def _set_adam_t(self, adam_t: int):
+        e = self.engine
+        e.adam_t = int(adam_t)
+        if e.training:
+            e.set_option("adam_step_count", e.adam_t)
+
+    @staticmethod
+    def _check_crcs(entries, computed) -> None:
+        """ValueError naming the first tensor whose device CRC-32C (computed, device int32 [n]) is not the stored one."""
+        got = computed.cpu().numpy().view(np.uint32)
+        for ent, c in zip(entries, got):
+            if int(c) != ent["crc"]:
+                raise ValueError("checkpoint tensor %s fails its CRC-32C: stored 0x%08x, computed 0x%08x" % (
+                    ent["key"], ent["crc"], int(c)))
+
+    def _read_bundle(self, prefix: str):
+        """The bundle's tensors streamed through page-locked staging into the engine's tensors, each tensor's CRC-32C
+        computed on the device as its rows arrive, then all compared with the stored ones."""
+        import torch
+        e = self.engine
+        entries, adam_t = bundle_entries(prefix, vars(e.dims), e.adam_m is not None, *self._adam_betas())
+        dest = {"theta": e.params, "adam_m": e.adam_m, "adam_v": e.adam_v}
+        computed = torch.empty(len(entries), dtype=torch.int32, device=e.dev)
+        with torch.cuda.device(e.dev), _PinnedStaging(e.dev) as stage:
+            for i, ent in enumerate(entries):
+                group, name = ent["name"].split("/")
+                t = dest[group][name]
+                stage.upload(ent["file"], ent["offset"], ent["nbytes"], t)
+                tensor_crc32c(t, *crc_view(name, ent["shape"]), computed[i:i + 1])
+        self._check_crcs(entries, computed)
+        self._set_adam_t(adam_t)
+
+    def _read_sharded_bundle(self, prefix: str):
+        """_read_sharded for a bundle: every rank reads its own rows, computes their CRC-32Cs on its device, gathers the
+        row CRCs of the sharded tables into global row order and combines them; a failure on any rank (a tensor missing,
+        a wrong shape, a CRC mismatch) raises on every rank."""
+        import torch
+        import torch.distributed as dist
+        e = self.engine
+        W, r = self.world, self.rank
+        state = {}
+
+        def read_rows():
+            entries, adam_t = bundle_entries(prefix, vars(self._engine_dims()), e.training, *self._adam_betas())
+            out = self._sharded_tensors(with_optimizer=e.training)
+            read_entries_part(prefix, 0, entries, r, W, (e.target_row0, e.target_row0 + e.dims.target_vocab), out)
+            torch.cuda.synchronize(e.dev)
+            state.update(entries=entries, out=out, adam_t=adam_t)
+        self._all_ok(read_rows)                          # every shard is loaded before any peer reads it
+        entries, out = state["entries"], state["out"]
+        computed = torch.empty(len(entries), dtype=torch.int32, device=e.dev)
+        with torch.cuda.device(e.dev):
+            for i, ent in enumerate(entries):
+                name = ent["name"].split("/")[1]
+                rows, row_bytes = crc_view(name, ent["shape"])
+                t = out[ent["name"]]
+                if name in ("W", "a"):                   # replicated: every rank checks its own copy
+                    tensor_crc32c(t, rows, row_bytes, computed[i:i + 1])
+                    continue
+                # tok / path: local row i is global row i * W + r (ceil(T / W) rows per rank, padding past the end);
+                # tgt: rank r's block of ceil(Y / W) rows (the last one shorter), padded to that length
+                per = int(t.shape[0]) if name != "tgt" else (rows + W - 1) // W
+                local = torch.zeros(per, dtype=torch.int32, device=e.dev)
+                n_own = min(per, int(t.shape[0]))
+                crc32c_rows(t, n_own, row_bytes, row_bytes, local)
+                gathered = torch.empty(W * per, dtype=torch.int32, device=e.dev)
+                dist.all_gather_into_tensor(gathered, local)
+                order = gathered.view(W, per).t() if name != "tgt" else gathered.view(W, per)
+                crc32c_combine(order.reshape(-1)[:rows].contiguous(), rows, row_bytes, computed[i:i + 1])
+        self._all_ok(lambda: self._check_crcs(entries, computed))
+        self._set_adam_t(state["adam_t"])
+
+    def _save_bundle(self, path: str, release: bool):
+        """<path>.index + <path>.data-00000-of-00001: every tensor's CRC-32C computed on the device, then its bytes
+        downloaded through page-locked staging into the data file, in key order; the Adam beta powers for e.adam_t."""
+        import torch
+        e = self.engine
+        e.sync_tables()                                  # lazy Adam: replay deferred row updates before reading the tensors
+        with_optimizer = (not release) and e.adam_m is not None
+        tensors, scalars = bundle_layout(vars(e.dims), with_optimizer, e.adam_t, *self._adam_betas())
+        src = {"theta": e.params, "adam_m": e.adam_m, "adam_v": e.adam_v}
+        dev = [src[n.split("/")[0]][n.split("/")[1]] for _, n, _, _, _ in tensors]
+        computed = torch.empty(max(len(tensors), 1), dtype=torch.int32, device=e.dev)
+        tmp = data_file(path) + ".tmp"
+        with torch.cuda.device(e.dev):
+            for i, ((_, name, shape, _, _), t) in enumerate(zip(tensors, dev)):
+                tensor_crc32c(t, *crc_view(name.split("/")[1], t.shape), computed[i:i + 1])
+            crcs = computed.cpu().numpy().view(np.uint32)
+            pieces = [(off, t) for (_, _, _, off, _), t in zip(tensors, dev)]
+            pieces += [(off, np.asarray(v, dtype="<f4")) for _, v, off in scalars]
+            with open(tmp, "wb") as f, _PinnedStaging(e.dev) as stage:
+                for off, t in sorted(pieces, key=lambda p: p[0]):
+                    if isinstance(t, np.ndarray):
+                        f.write(t.tobytes())
+                    else:
+                        stage.download(t, f)
+        index = [(key, shape, off, n, int(c)) for (key, _, shape, off, n), c in zip(tensors, crcs)]
+        index += [(key, (), off, 4, host_crc32c(np.asarray(v, dtype="<f4").tobytes())) for key, v, off in scalars]
+        os.replace(tmp, data_file(path))
+        write_index(path, index)
 
     def _read_checkpoint(self, file_path: str):
         import torch

@@ -149,6 +149,9 @@ _SIGNATURES = {
     "c2v_text_format_rows": (C.c_int, [_P, C.c_int64, _I32, C.c_int64, _P, _P, _P, C.c_size_t, _P, C.c_int64, _P, _P,
                                        _P]),
     "c2v_selftest_format_floats": (C.c_int, [_P, C.c_int64, _P, _P]),
+    # CRC-32C of tensor bundle entries (tf_bundle.py)
+    "c2v_crc32c_rows": (C.c_int, [_P, C.c_int64, C.c_int64, C.c_int64, _P, _P]),
+    "c2v_crc32c_combine": (C.c_int, [_P, C.c_int64, C.c_int64, _P, _P]),
     # preprocessing (device_preprocess.py)
     "c2v_prep_create": (C.c_int, [C.c_int, C.POINTER(_P)]),
     "c2v_prep_destroy": (None, [_P]),
@@ -862,3 +865,35 @@ def _host_ptr(a) -> int:
             raise ValueError("host buffer must be a contiguous CPU tensor")
         return a.data_ptr()
     raise TypeError("unsupported host buffer type %r" % type(a))
+
+
+# ---- CRC-32C of device tensors (tf_bundle.py, DESIGN.md §6k) ----------------------------------------------------------
+def crc32c_rows(x, rows: int, row_bytes: int, row_stride: int, out) -> None:
+    """out (device int32 [>= rows], read as uint32) = the CRC-32C of each of the `rows` rows of row_bytes bytes of the
+    device tensor x, row r at byte r * row_stride of it; queued on the current stream."""
+    import torch
+    lib = load_library()
+    rc = lib.c2v_crc32c_rows(x.data_ptr() if rows else None, int(rows), int(row_bytes), int(row_stride), out.data_ptr(),
+                             torch.cuda.current_stream(out.device).cuda_stream)
+    if rc != 0:
+        raise EngineError(rc, lib.c2v_last_error(None).decode())
+
+
+def crc32c_combine(crcs, n: int, seg_bytes: int, out) -> None:
+    """out[0] (device int32, read as uint32) = the CRC-32C of n segments of seg_bytes bytes whose CRCs are crcs[0, n)
+    (device int32); queued on the current stream."""
+    import torch
+    lib = load_library()
+    rc = lib.c2v_crc32c_combine(crcs.data_ptr() if n else None, int(n), int(seg_bytes), out.data_ptr(),
+                                torch.cuda.current_stream(out.device).cuda_stream)
+    if rc != 0:
+        raise EngineError(rc, lib.c2v_last_error(None).decode())
+
+
+def tensor_crc32c(x, rows: int, row_bytes: int, out) -> None:
+    """out[0] = the CRC-32C of the first rows * row_bytes bytes of the contiguous device tensor x, as `rows` rows
+    checked in parallel and combined; queued on the current stream."""
+    import torch
+    row_crc = torch.empty(max(int(rows), 1), dtype=torch.int32, device=x.device)
+    crc32c_rows(x, rows, row_bytes, row_bytes, row_crc)
+    crc32c_combine(row_crc, rows, row_bytes, out)

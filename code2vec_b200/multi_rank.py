@@ -33,8 +33,9 @@ def run_world(environ) -> Tuple[int, int]:
     return int(environ.get("WORLD_SIZE", "1") or "1"), int(environ.get("LOCAL_RANK", "0") or "0")
 
 
-def check_multi_rank_run(config, world: int) -> None:
-    """Raises ValueError if `config` cannot run on `world` ranks.  Host only: it runs before any engine exists."""
+def check_multi_rank_run(config, world: int, save_format: str = "c2v_b200") -> None:
+    """Raises ValueError if `config` (saving in `save_format`, tf_bundle.save_format_flag) cannot run on `world` ranks.
+    Host only: it runs before any engine exists."""
     if world not in WORLD_SIZES:
         raise ValueError("WORLD_SIZE=%d: Code2VecModel runs on 1, 2, 4 or 8 GPUs (the embedding tables are row-sharded "
                          "over the ranks); launch with --nproc-per-node 2, 4 or 8" % world)
@@ -52,6 +53,10 @@ def check_multi_rank_run(config, world: int) -> None:
     if config.DL_FRAMEWORK == "b200-keras":
         raise ValueError("--framework b200-keras runs on one GPU: train on several GPUs with --framework b200, or run "
                          "the Keras backend in a single process")
+    if save_format != "c2v_b200":
+        raise ValueError("C2V_SAVE_FORMAT=%s: TensorFlow checkpoints are written by one GPU; save .c2v_b200 checkpoints "
+                         "on several GPUs (unset C2V_SAVE_FORMAT), then load and save (or --release) in a single process "
+                         "with C2V_SAVE_FORMAT=tf" % save_format)
 
 
 def batch_split(rows: int, world: int, rank: int) -> Tuple[int, int, int]:
@@ -145,18 +150,25 @@ def read_checkpoint_part(path: str, rank: int, world: int, target_rows: Tuple[in
     first rows are filled, padding rows are left as they are).  Tensors the file does not hold are left untouched.
     Returns the header."""
     meta, base = read_checkpoint_header(path)
-    for ent in meta["tensors"]:
+    read_entries_part(path, base, meta["tensors"], rank, world, target_rows, out)
+    return meta
+
+
+def read_entries_part(path: str, base: int, entries: List[dict], rank: int, world: int, target_rows: Tuple[int, int],
+                      out: dict) -> None:
+    """read_checkpoint_part for tensor entries whose bytes start at `base` of `path` (or of ent["file"], when an entry
+    names its own file)."""
+    for ent in entries:
         dest = out.get(ent["name"])
         if dest is None:
             continue
-        src = np.array(_own_rows(ent["name"].split("/")[1], _tensor_map(path, base, ent, "r"), rank, world,
-                                             target_rows))
+        src = np.array(_own_rows(ent["name"].split("/")[1], _tensor_map(ent.get("file", path), base, ent, "r"), rank,
+                                 world, target_rows))
         if isinstance(dest, np.ndarray):
             dest[:src.shape[0]] = src
         else:
             import torch
             dest[:src.shape[0]].copy_(torch.from_numpy(src))
-    return meta
 
 
 def check_checkpoint_dims(meta: dict, dims: dict) -> None:

@@ -690,6 +690,20 @@ int c2v_text_format_rows(const float* x, int64_t rows, int32_t cols, int64_t ld,
  * out[i * C2V_TEXT_VALUE_BYTES, ...) followed by NUL bytes up to the next value, and its length to len[i] (host). */
 int c2v_selftest_format_floats(const float* x, int64_t n, char* out, int32_t* len);
 
+/* ---- CRC-32C of device memory (DESIGN.md §6k) ------------------------------------------------------------------------
+ * The checksum of a TensorFlow tensor bundle entry (tf_bundle.py): CRC-32C, reflected polynomial 0x82F63B78, init and
+ * xorout 0xFFFFFFFF ("123456789" -> 0xE3069283).  No engine handle is needed; any alignment is accepted; failures return
+ * a negative c2v_status with the message in c2v_last_error(NULL).  Asynchronous on `stream`. */
+
+/* crc_out[r] (device, [rows]) = the CRC-32C of the row_bytes bytes at base + r * row_stride (device), r in [0, rows).
+ * A row of no bytes has CRC 0. */
+int c2v_crc32c_rows(const void* base, int64_t rows, int64_t row_bytes, int64_t row_stride, uint32_t* crc_out,
+                    void* stream);
+
+/* *out (device) = the CRC-32C of the concatenation of n segments of seg_bytes bytes each, from their CRCs crcs[0, n)
+ * (device): zlib's crc32_combine as a tree reduction.  n = 0 gives 0. */
+int c2v_crc32c_combine(const uint32_t* crcs, int64_t n, int64_t seg_bytes, uint32_t* out, void* stream);
+
 /* ---- Preprocessing on the device (DESIGN.md §6g) ----------------------------------------------------------------------
  * Raw extractor output (`target ctx ctx ...` lines) in device memory -> what preprocess.py's count_histograms and
  * process_file write, byte for byte (device_preprocess.py).  A chunk is whole lines of a file under universal newlines:
