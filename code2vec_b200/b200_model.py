@@ -26,7 +26,9 @@ import numpy as np
 
 from .common import common
 from .config import Config
-from .engine import PARAM_NAMES, EngineDims, PathAttentionEngine, crc32c_combine, crc32c_rows, tensor_crc32c
+from .engine import (PARAM_NAMES, EngineDims, PathAttentionEngine, cols_to_rows, crc32c_combine, crc32c_rows,
+                     rows_to_cols, tensor_crc32c)
+from .keras_ckpt import keras_entries, keras_layout, latest_checkpoint, record_checkpoint, write_keras_index
 from .model_base import Code2VecModelBase, ModelEvaluationResults, ModelPredictionResults
 from .path_context_reader import EstimatorAction, ModelInputTensorsFormer, PathContextReader, ReaderInputTensors
 from .multi_rank import (CKPT_MAGIC, CKPT_SUFFIX, batch_split, check_checkpoint_dims, check_multi_rank_run,
@@ -248,7 +250,8 @@ class Code2VecModel(Code2VecModelBase):
         self.world, self.local_rank = run_world(os.environ)
         self.rank = 0
         self._own_group = False
-        # C2V_SAVE_FORMAT=tf: save() and --release write TensorFlow V2 checkpoints (tf_bundle.py, DESIGN.md §6k)
+        # C2V_SAVE_FORMAT=tf: save() and --release write TensorFlow V2 checkpoints (tf_bundle.py, DESIGN.md §6k);
+        # C2V_SAVE_FORMAT=keras: the reference Keras backend's checkpoints (keras_ckpt.py, DESIGN.md §6l)
         self._save_format = save_format_flag(os.environ)
         check_multi_rank_run(config, self.world, self._save_format)
         # C2V_NUM_SAMPLED=<S>: train() runs the sampled softmax with S negatives drawn on the GPU (DESIGN.md §6j)
@@ -429,12 +432,17 @@ class Code2VecModel(Code2VecModelBase):
             self.log("variable name: {} -- shape: {} -- #params: {}".format(name, shape, int(np.prod(shape))))
 
     def _load_inner_model(self):
-        """`X.c2v_b200` when it exists, else the TensorFlow checkpoint `X.index` + `X.data-*` when that exists."""
+        """`X.c2v_b200` when it exists, else the TensorFlow checkpoint `X.index` + `X.data-*` when that exists, else the
+        Keras backend's `X__only-weights` or `X__entire-model/` when one exists (_load_keras)."""
         self._make_engine()
-        path = self.config.MODEL_LOAD_PATH + _CKPT_SUFFIX
-        if not os.path.isfile(path) and os.path.isfile(self.config.MODEL_LOAD_PATH + INDEX_SUFFIX):
-            self.log("Loading model weights from the TensorFlow checkpoint: " + self.config.MODEL_LOAD_PATH)
-            (self._read_sharded_bundle if self.world > 1 else self._read_bundle)(self.config.MODEL_LOAD_PATH)
+        load = self.config.MODEL_LOAD_PATH
+        path = load + _CKPT_SUFFIX
+        if not os.path.isfile(path) and os.path.isfile(load + INDEX_SUFFIX):
+            self.log("Loading model weights from the TensorFlow checkpoint: " + load)
+            (self._read_sharded_bundle if self.world > 1 else self._read_bundle)(load)
+        elif not os.path.isfile(path) and (os.path.isfile(Config.get_model_weights_path(load) + INDEX_SUFFIX) or
+                                           os.path.isdir(Config.get_entire_model_path(load))):
+            self._load_keras(load)
         else:
             self.log("Loading model weights from: " + path)
             self._read_checkpoint(path)
@@ -484,6 +492,8 @@ class Code2VecModel(Code2VecModelBase):
             return self._save_sharded(path)
         if self._save_format == "tf":
             return self._save_bundle(path, release)
+        if self._save_format == "keras":
+            return self._save_keras(path, release or self.config.RELEASE)
         e = self.engine
         e.sync_tables()                                  # lazy Adam: replay deferred row updates before reading the tensors
         tensors = [e.params[k] for k in PARAM_NAMES]
@@ -649,6 +659,127 @@ class Code2VecModel(Code2VecModelBase):
         index += [(key, (), off, 4, host_crc32c(np.asarray(v, dtype="<f4").tobytes())) for key, v, off in scalars]
         os.replace(tmp, data_file(path))
         write_index(path, index)
+
+    # ---- the reference Keras backend's checkpoints (keras_ckpt.py, DESIGN.md §6l) --------------------------------
+    def _load_keras(self, load: str):
+        """The rule of the reference's Keras backend (keras_model.py:241-280): training needs the entire model; otherwise
+        the weights file when it exists, else the latest checkpoint of the entire model, whose `ckpt-N` gives the epochs
+        trained."""
+        entire, weights = Config.get_entire_model_path(load), Config.get_model_weights_path(load)
+        must_use_entire_model = self.config.is_training
+        entire_model_exists = os.path.exists(entire)
+        model_weights_exist = os.path.isfile(weights + INDEX_SUFFIX)
+        if must_use_entire_model and not entire_model_exists:
+            raise ValueError(
+                "There is no model at path `{model_file_path}`. When loading the model for further training, "
+                "we must use an entire saved model file (not just weights).".format(model_file_path=entire))
+        if not entire_model_exists and not model_weights_exist:
+            raise ValueError(
+                "There is no entire model to load at path `{entire_model_path}`, "
+                "and there is no model weights file to load at path `{model_weights_path}`.".format(
+                    entire_model_path=entire, model_weights_path=weights))
+        if self.world > 1:
+            raise ValueError("`%s`: Keras checkpoints are read by one GPU; convert it once in a single process (without "
+                             "torch.distributed.run), e.g. `--load %s --save <X>` saves a .c2v_b200 checkpoint that loads on "
+                             "any number of GPUs" % (load, load))
+        if must_use_entire_model or not model_weights_exist:
+            self.log("Loading entire model from path `{}`.".format(entire))
+            latest = latest_checkpoint(entire)
+            if latest is None:
+                raise ValueError("Failed to load model: Model latest checkpoint is not found.")
+            self.log("Loading latest checkpoint `{}`.".format(latest))
+            self._read_keras(latest)
+            if hasattr(self, "nr_epochs_trained"):           # the Keras-schedule backend resumes at this epoch
+                self.nr_epochs_trained = int(latest.split("-")[-1])
+        else:
+            self.log("Loading model weights from path `{}`.".format(weights))
+            self._read_keras(weights)
+
+    def _chunk_rows(self, Y: int) -> int:
+        """File rows of a [D, Y] kernel per device chunk: whole rows, at most _PinnedStaging.CHUNK_BYTES unless one row
+        is larger."""
+        return max(1, _PinnedStaging.CHUNK_BYTES // (4 * Y))
+
+    def _read_keras(self, prefix: str):
+        """As _read_bundle; the [D, Y] output kernel (and its slots) goes through one device chunk of whole file rows:
+        each chunk's row CRCs in file order, then c2v_rows_to_cols into the engine's [Y, D] tensor."""
+        import torch
+        e = self.engine
+        entries, adam_t, self._keras_save_counter = keras_entries(prefix, vars(e.dims), e.adam_m is not None,
+                                                                  self._ADAM or ADAM_DEFAULTS)
+        dest = {"theta": e.params, "adam_m": e.adam_m, "adam_v": e.adam_v}
+        computed = torch.empty(len(entries), dtype=torch.int32, device=e.dev)
+        with torch.cuda.device(e.dev), _PinnedStaging(e.dev) as stage:
+            chunk = row_crc = None
+            for i, ent in enumerate(entries):
+                group, name = ent["name"].split("/")
+                t = dest[group][name]
+                if not ent["transposed"]:
+                    stage.upload(ent["file"], ent["offset"], ent["nbytes"], t)
+                    tensor_crc32c(t, *crc_view(name, ent["shape"]), computed[i:i + 1])
+                    continue
+                Y, D = t.shape
+                rows = min(self._chunk_rows(Y), D)
+                if chunk is None:
+                    chunk = torch.empty(rows * Y, dtype=torch.float32, device=e.dev)
+                    row_crc = torch.empty(D, dtype=torch.int32, device=e.dev)
+                for i0 in range(0, D, rows):
+                    k = min(rows, D - i0)
+                    stage.upload(ent["file"], ent["offset"] + i0 * 4 * Y, k * 4 * Y, chunk[:k * Y])
+                    crc32c_rows(chunk, k, 4 * Y, 4 * Y, row_crc[i0:i0 + k])
+                    rows_to_cols(chunk, k, Y, t, i0)
+                crc32c_combine(row_crc, D, 4 * Y, computed[i:i + 1])
+        self._check_crcs(entries, computed)
+        self._set_adam_t(adam_t)
+
+    def _save_keras(self, path: str, release: bool):
+        """`path__only-weights` (release: the weights alone) or `path__entire-model/ckpt-<epochs trained>` with the
+        optimizer, then the manager's state file and MAX_TO_KEEP rotation.  Each tensor's CRC-32C is computed on the
+        device; the [D, Y] output kernel is gathered into one device chunk of whole file rows at a time
+        (c2v_cols_to_rows), checked and downloaded."""
+        import torch
+        e = self.engine
+        e.sync_tables()                                  # lazy Adam: replay deferred row updates before reading the tensors
+        with_optimizer = (not release) and e.adam_m is not None
+        self._keras_save_counter = getattr(self, "_keras_save_counter", 0) + (0 if release else 1)
+        if release:
+            prefix = Config.get_model_weights_path(path)
+        else:
+            directory = Config.get_entire_model_path(path)
+            os.makedirs(directory, exist_ok=True)
+            prefix = os.path.join(directory, "ckpt-%d" % getattr(self, "nr_epochs_trained", 0))
+        tensors, scalars = keras_layout(vars(e.dims), not release, with_optimizer, e.adam_t, self._keras_save_counter,
+                                        self._ADAM or ADAM_DEFAULTS)
+        src = {"theta": e.params, "adam_m": e.adam_m, "adam_v": e.adam_v}
+        pieces = [(off, src[n.split("/")[0]][n.split("/")[1]], i) for i, (_, n, _, off, _) in enumerate(tensors)]
+        pieces += [(off, raw, None) for _, _, _, raw, off, _ in scalars]
+        computed = torch.empty(max(len(tensors), 1), dtype=torch.int32, device=e.dev)
+        tmp = data_file(prefix) + ".tmp"
+        with torch.cuda.device(e.dev), open(tmp, "wb") as f, _PinnedStaging(e.dev) as stage:
+            chunk = row_crc = None
+            for _, t, i in sorted(pieces, key=lambda p: p[0]):
+                if i is None:
+                    f.write(t)
+                elif tensors[i][1].split("/")[1] != "tgt":
+                    tensor_crc32c(t, *crc_view(tensors[i][1].split("/")[1], t.shape), computed[i:i + 1])
+                    stage.download(t, f)
+                else:
+                    Y, D = t.shape
+                    rows = min(self._chunk_rows(Y), D)
+                    if chunk is None:
+                        chunk = torch.empty(rows * Y, dtype=torch.float32, device=e.dev)
+                        row_crc = torch.empty(D, dtype=torch.int32, device=e.dev)
+                    for i0 in range(0, D, rows):
+                        k = min(rows, D - i0)
+                        cols_to_rows(t, i0, k, Y, chunk)
+                        crc32c_rows(chunk, k, 4 * Y, 4 * Y, row_crc[i0:i0 + k])
+                        stage.download(chunk[:k * Y], f)
+                    crc32c_combine(row_crc, D, 4 * Y, computed[i:i + 1])
+            crcs = computed.cpu().numpy().view(np.uint32)
+        os.replace(tmp, data_file(prefix))
+        write_keras_index(prefix, tensors, scalars, crcs)
+        if not release:
+            record_checkpoint(directory, prefix, self.config.MAX_TO_KEEP, time.time())
 
     def _read_checkpoint(self, file_path: str):
         import torch

@@ -187,6 +187,58 @@ __global__ void __launch_bounds__(kThreads) crc_combine_kernel(const uint32_t* _
   }
 }
 
+// The Keras output kernel's transpose (DESIGN.md §6l): a [k, Y] chunk of file rows <-> columns [col0, col0 + k) of the
+// engine's [Y, ld] table.  32 x 32 tiles through shared memory (one padding word per row, so the column reads do not
+// conflict), 32 x 8 threads, a grid-stride loop over the tiles; the element is moved as a uint32, so every bit survives.
+constexpr int kTile = 32;
+constexpr int kTileRows = 8;
+
+__global__ void __launch_bounds__(kTile * kTileRows) rows_to_cols_kernel(const uint32_t* __restrict__ src, int64_t k,
+                                                                          int64_t Y, uint32_t* __restrict__ dst,
+                                                                          int64_t ld, int64_t col0) {
+  __shared__ uint32_t tile[kTile][kTile + 1];
+  const int64_t tiles_y = (Y + kTile - 1) / kTile, tiles = tiles_y * ((k + kTile - 1) / kTile);
+  const int tx = threadIdx.x, ty = threadIdx.y;
+  for (int64_t t = blockIdx.x; t < tiles; t += gridDim.x) {
+    const int64_t y0 = (t % tiles_y) * kTile, i0 = (t / tiles_y) * kTile;
+#pragma unroll
+    for (int r = 0; r < kTile; r += kTileRows) {              // read along y: src row i0 + ty + r
+      const int64_t i = i0 + ty + r, y = y0 + tx;
+      if (i < k && y < Y) tile[ty + r][tx] = __ldg(src + i * Y + y);
+    }
+    __syncthreads();
+#pragma unroll
+    for (int r = 0; r < kTile; r += kTileRows) {              // write along i: dst row y0 + ty + r
+      const int64_t y = y0 + ty + r, i = i0 + tx;
+      if (i < k && y < Y) dst[y * ld + col0 + i] = tile[tx][ty + r];
+    }
+    __syncthreads();
+  }
+}
+
+__global__ void __launch_bounds__(kTile * kTileRows) cols_to_rows_kernel(const uint32_t* __restrict__ src, int64_t ld,
+                                                                          int64_t col0, int64_t k, int64_t Y,
+                                                                          uint32_t* __restrict__ dst) {
+  __shared__ uint32_t tile[kTile][kTile + 1];
+  const int64_t tiles_y = (Y + kTile - 1) / kTile, tiles = tiles_y * ((k + kTile - 1) / kTile);
+  const int tx = threadIdx.x, ty = threadIdx.y;
+  for (int64_t t = blockIdx.x; t < tiles; t += gridDim.x) {
+    const int64_t y0 = (t % tiles_y) * kTile, i0 = (t / tiles_y) * kTile;
+#pragma unroll
+    for (int r = 0; r < kTile; r += kTileRows) {              // read along i: src row y0 + ty + r
+      const int64_t y = y0 + ty + r, i = i0 + tx;
+      if (i < k && y < Y) tile[ty + r][tx] = __ldg(src + y * ld + col0 + i);
+    }
+    __syncthreads();
+#pragma unroll
+    for (int r = 0; r < kTile; r += kTileRows) {              // write along y: dst row i0 + ty + r
+      const int64_t i = i0 + ty + r, y = y0 + tx;
+      if (i < k && y < Y) dst[i * Y + y] = tile[tx][ty + r];
+    }
+    __syncthreads();
+  }
+}
+
 int cfail(int code, const std::string& msg) {
   c2v::set_global_error(msg);
   return code;
@@ -244,4 +296,39 @@ int c2v_crc32c_combine(const uint32_t* crcs, int64_t n, int64_t seg_bytes, uint3
   if (blocks > 0x7fffffff) return cfail(C2V_ERR_INVALID, "c2v_crc32c_combine: n too large");
   crc_combine_kernel<<<(unsigned)blocks, kThreads, 0, s>>>(crcs, n, blocks * kLeavesPerBlock - n, seg_bytes, out);
   return launch_check("c2v_crc32c_combine");
+}
+
+namespace {
+
+// shared checks of the two transpose entry points; 0 = launch, 1 = nothing to move, < 0 = refused
+int transpose_args(const char* fn, const void* src, int64_t k, int64_t Y, const void* dst, int64_t ld, int64_t col0) {
+  if (k < 0 || Y < 0 || col0 < 0 || (k && Y && ld < col0 + k))
+    return cfail(C2V_ERR_INVALID, std::string(fn) + ": need k >= 0, Y >= 0, col0 >= 0 and ld >= col0 + k");
+  if (!k || !Y) return 1;
+  if (!src || !dst) return cfail(C2V_ERR_INVALID, std::string(fn) + ": NULL argument");
+  if (((uintptr_t)src | (uintptr_t)dst) & 3u)
+    return cfail(C2V_ERR_INVALID, std::string(fn) + ": src and dst must be 4-byte aligned");
+  return 0;
+}
+
+int transpose_grid(int64_t k, int64_t Y) {
+  return grid_for(((Y + kTile - 1) / kTile) * ((k + kTile - 1) / kTile) * kThreads);
+}
+
+}  // namespace
+
+int c2v_rows_to_cols(const float* src, int64_t k, int64_t Y, float* dst, int64_t ld, int64_t col0, void* stream) {
+  const int rc = transpose_args("c2v_rows_to_cols", src, k, Y, dst, ld, col0);
+  if (rc) return rc < 0 ? rc : C2V_OK;
+  rows_to_cols_kernel<<<transpose_grid(k, Y), dim3(kTile, kTileRows), 0, (cudaStream_t)stream>>>(
+      (const uint32_t*)src, k, Y, (uint32_t*)dst, ld, col0);
+  return launch_check("c2v_rows_to_cols");
+}
+
+int c2v_cols_to_rows(const float* src, int64_t ld, int64_t col0, int64_t k, int64_t Y, float* dst, void* stream) {
+  const int rc = transpose_args("c2v_cols_to_rows", src, k, Y, dst, ld, col0);
+  if (rc) return rc < 0 ? rc : C2V_OK;
+  cols_to_rows_kernel<<<transpose_grid(k, Y), dim3(kTile, kTileRows), 0, (cudaStream_t)stream>>>(
+      (const uint32_t*)src, ld, col0, k, Y, (uint32_t*)dst);
+  return launch_check("c2v_cols_to_rows");
 }

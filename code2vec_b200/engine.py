@@ -152,6 +152,9 @@ _SIGNATURES = {
     # CRC-32C of tensor bundle entries (tf_bundle.py)
     "c2v_crc32c_rows": (C.c_int, [_P, C.c_int64, C.c_int64, C.c_int64, _P, _P]),
     "c2v_crc32c_combine": (C.c_int, [_P, C.c_int64, C.c_int64, _P, _P]),
+    # the Keras output kernel's transpose (keras_ckpt.py)
+    "c2v_rows_to_cols": (C.c_int, [_P, C.c_int64, C.c_int64, _P, C.c_int64, C.c_int64, _P]),
+    "c2v_cols_to_rows": (C.c_int, [_P, C.c_int64, C.c_int64, C.c_int64, C.c_int64, _P, _P]),
     # preprocessing (device_preprocess.py)
     "c2v_prep_create": (C.c_int, [C.c_int, C.POINTER(_P)]),
     "c2v_prep_destroy": (None, [_P]),
@@ -897,3 +900,26 @@ def tensor_crc32c(x, rows: int, row_bytes: int, out) -> None:
     row_crc = torch.empty(max(int(rows), 1), dtype=torch.int32, device=x.device)
     crc32c_rows(x, rows, row_bytes, row_bytes, row_crc)
     crc32c_combine(row_crc, rows, row_bytes, out)
+
+
+# ---- the Keras output kernel's transpose (keras_ckpt.py, DESIGN.md §6l) -----------------------------------------------
+def rows_to_cols(src, k: int, Y: int, dst, col0: int) -> None:
+    """dst[y, col0 + i] = src[i * Y + y] for i < k, y < Y, bit for bit: k file rows of a [D, Y] kernel (the contiguous
+    device tensor src) into columns of the contiguous device table dst [Y, ld]; queued on the current stream."""
+    import torch
+    lib = load_library()
+    rc = lib.c2v_rows_to_cols(src.data_ptr(), int(k), int(Y), dst.data_ptr(), int(dst.shape[-1]), int(col0),
+                              torch.cuda.current_stream(dst.device).cuda_stream)
+    if rc != 0:
+        raise EngineError(rc, lib.c2v_last_error(None).decode())
+
+
+def cols_to_rows(src, col0: int, k: int, Y: int, dst) -> None:
+    """dst[i * Y + y] = src[y, col0 + i] for i < k, y < Y, bit for bit: the reverse of rows_to_cols; queued on the current
+    stream."""
+    import torch
+    lib = load_library()
+    rc = lib.c2v_cols_to_rows(src.data_ptr(), int(src.shape[-1]), int(col0), int(k), int(Y), dst.data_ptr(),
+                              torch.cuda.current_stream(dst.device).cuda_stream)
+    if rc != 0:
+        raise EngineError(rc, lib.c2v_last_error(None).decode())

@@ -56,7 +56,7 @@ def check_multi_rank_run(config, world: int, save_format: str = "c2v_b200") -> N
     if save_format != "c2v_b200":
         raise ValueError("C2V_SAVE_FORMAT=%s: TensorFlow checkpoints are written by one GPU; save .c2v_b200 checkpoints "
                          "on several GPUs (unset C2V_SAVE_FORMAT), then load and save (or --release) in a single process "
-                         "with C2V_SAVE_FORMAT=tf" % save_format)
+                         "with C2V_SAVE_FORMAT=%s" % (save_format, save_format))
 
 
 def batch_split(rows: int, world: int, rank: int) -> Tuple[int, int, int]:

@@ -32,17 +32,18 @@ RESTART_INTERVAL = 16
 DT_FLOAT = 1
 BIG_ENDIAN = 1
 MAX_ADAM_T = 10 ** 7
-SAVE_FORMATS = ("c2v_b200", "tf")
+SAVE_FORMATS = ("c2v_b200", "tf", "keras")
 
 _GROUP_SUFFIX = {"theta": "", "adam_m": "/Adam", "adam_v": "/Adam_1"}
 BETA_KEYS = ("model/beta1_power", "model/beta2_power")
 
 
 def save_format_flag(environ) -> str:
-    """C2V_SAVE_FORMAT: "c2v_b200" (the default) or "tf" (a TensorFlow V2 checkpoint: <path>.index + data)."""
+    """C2V_SAVE_FORMAT: "c2v_b200" (the default), "tf" (a TensorFlow V2 checkpoint: <path>.index + data) or "keras" (the
+    reference Keras backend's <path>__entire-model/ckpt-N or <path>__only-weights, keras_ckpt.py)."""
     flag = environ.get("C2V_SAVE_FORMAT", "c2v_b200") or "c2v_b200"
     if flag not in SAVE_FORMATS:
-        raise ValueError("C2V_SAVE_FORMAT must be c2v_b200 or tf, got %r" % flag)
+        raise ValueError("C2V_SAVE_FORMAT must be c2v_b200, tf or keras, got %r" % flag)
     return flag
 
 
@@ -352,8 +353,9 @@ def adam_step_from_powers(p1, p2, beta1: float, beta2: float, max_t: int = MAX_A
 
 
 # ---- bundles --------------------------------------------------------------------------------------------------------
-def read_index(prefix: str) -> Tuple[dict, Dict[str, dict]]:
-    """(header, {tensor key: entry}) of the bundle `prefix`, with the refusals of the format's limits."""
+def read_index(prefix: str, other_dtypes: Optional[Dict[str, int]] = None) -> Tuple[dict, Dict[str, dict]]:
+    """(header, {tensor key: entry}) of the bundle `prefix`, with the refusals of the format's limits.  Every tensor is
+    DT_FLOAT except the keys of `other_dtypes`, which must have the dtype it gives them (keras_ckpt.py)."""
     path = prefix + INDEX_SUFFIX
     with open(path, "rb") as f:
         buf = f.read()
@@ -375,7 +377,10 @@ def read_index(prefix: str) -> Tuple[dict, Dict[str, dict]]:
     for k, e in entries.items():
         if e["slices"]:
             raise ValueError("`%s`: tensor %s is partitioned (slices); only whole tensors are read" % (path, k))
-        if e["dtype"] != DT_FLOAT:
+        if other_dtypes and k in other_dtypes:
+            if e["dtype"] != other_dtypes[k]:
+                raise ValueError("`%s`: tensor %s has dtype %d; it must be %d" % (path, k, e["dtype"], other_dtypes[k]))
+        elif e["dtype"] != DT_FLOAT:
             raise ValueError("`%s`: tensor %s has dtype %d; only DT_FLOAT (1) is read" % (path, k, e["dtype"]))
         if not 0 <= e["shard_id"] < header["num_shards"]:
             raise ValueError("`%s`: tensor %s is in shard %d of %d" % (path, k, e["shard_id"], header["num_shards"]))

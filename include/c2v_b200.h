@@ -704,6 +704,18 @@ int c2v_crc32c_rows(const void* base, int64_t rows, int64_t row_bytes, int64_t r
  * (device): zlib's crc32_combine as a tree reduction.  n = 0 gives 0. */
 int c2v_crc32c_combine(const uint32_t* crcs, int64_t n, int64_t seg_bytes, uint32_t* out, void* stream);
 
+/* ---- The Keras output kernel's transpose (DESIGN.md §6l) ----------------------------------------------------------------
+ * Keras stores the output layer's kernel as [D, Y]; the engine holds it as [Y, ld].  These move a chunk of k file rows
+ * between the two layouts as exact bit copies (NaN payloads and -0.0 included).  Any k >= 0, Y >= 0, col0 >= 0 with
+ * ld >= col0 + k; src and dst are device pointers aligned to 4 bytes.  No engine handle is needed; failures return a
+ * negative c2v_status with the message in c2v_last_error(NULL).  Asynchronous on `stream`. */
+
+/* dst[y * ld + col0 + i] = src[i * Y + y] for i < k, y < Y: k file rows into columns [col0, col0 + k) of dst. */
+int c2v_rows_to_cols(const float* src, int64_t k, int64_t Y, float* dst, int64_t ld, int64_t col0, void* stream);
+
+/* dst[i * Y + y] = src[y * ld + col0 + i] for i < k, y < Y: columns [col0, col0 + k) of src into k file rows. */
+int c2v_cols_to_rows(const float* src, int64_t ld, int64_t col0, int64_t k, int64_t Y, float* dst, void* stream);
+
 /* ---- Preprocessing on the device (DESIGN.md §6g) ----------------------------------------------------------------------
  * Raw extractor output (`target ctx ctx ...` lines) in device memory -> what preprocess.py's count_histograms and
  * process_file write, byte for byte (device_preprocess.py).  A chunk is whole lines of a file under universal newlines:
