@@ -88,6 +88,7 @@ class SubtokenCounts:
 
 class Code2VecModel(_TFNumericsModel):
     _ADAM = KERAS_ADAM
+    _INIT_SCHEME = "keras"
 
     def __init__(self, config):
         self.nr_epochs_trained = 0                              # ModelTrainingStatus (keras_checkpoint_saver_callback.py:14-17)

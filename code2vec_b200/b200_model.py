@@ -162,6 +162,45 @@ def sharded_sampled_flag(environ) -> bool:
     return flag == "1"
 
 
+def extend_vocab_flag(environ) -> bool:
+    """C2V_EXTEND_VOCAB=1: a run that loads (--load) and trains (--data) extends the loaded vocabularies by the dataset's
+    words and continues from the loaded model at the merged sizes (DESIGN.md §6m).  "" and "0" (the default) are off.
+    ValueError for anything but 0 or 1."""
+    flag = environ.get("C2V_EXTEND_VOCAB", "0") or "0"
+    if flag not in ("0", "1"):
+        raise ValueError("C2V_EXTEND_VOCAB must be 0 or 1, got %r" % flag)
+    return flag == "1"
+
+
+def extend_vocab_run(config, extend: bool, log) -> bool:
+    """Whether this run extends its loaded vocabularies (extend: the value of C2V_EXTEND_VOCAB).  A run that does not
+    train or does not load logs that the switch has no effect.  ValueError, before anything is read or written, when
+    --save puts dictionaries.bin in the --load directory: it would replace the file the loaded checkpoints need."""
+    if not extend:
+        return False
+    if not config.is_training:
+        log("C2V_EXTEND_VOCAB=1 has no effect: this run does not train (no --data)")
+        return False
+    if not config.is_loading:
+        log("C2V_EXTEND_VOCAB=1 has no effect: this run does not load a model (no --load), and a model trained from "
+            "scratch already takes the dataset's vocabulary")
+        return False
+    if config.is_saving:
+        where = lambda p: os.path.realpath(os.path.dirname(os.path.abspath(Config.get_vocabularies_path_from_model_path(p))))
+        folder = where(config.MODEL_LOAD_PATH)
+        if where(config.MODEL_SAVE_PATH) == folder:
+            raise ValueError("C2V_EXTEND_VOCAB=1: --save writes the extended vocabularies to `%s`, the directory of --load, "
+                             "and its dictionaries.bin would no longer fit the loaded checkpoints; save to another "
+                             "directory" % os.path.join(folder, "dictionaries.bin"))
+    return True
+
+
+def _lead(t, shape):
+    """The leading rows of the engine tensor t that a stored tensor of `shape` fills: all of t unless C2V_EXTEND_VOCAB=1
+    grew its table."""
+    return t[:int(shape[0])] if len(shape) == 2 else t
+
+
 class _PinnedStaging:
     """Two page-locked buffers between files and device tensors, as DeviceTextWriter has (DESIGN.md §6f): the host
     fills or drains one while the other's copy runs on the current stream."""
@@ -236,6 +275,8 @@ _CKPT_SUFFIX = CKPT_SUFFIX
 
 class Code2VecModel(Code2VecModelBase):
     _ADAM: Optional[dict] = None      # None = tf.compat.v1.train.AdamOptimizer() defaults (tensorflow_model.py:232)
+    _INIT_SCHEME = "tensorflow"       # engine.init_params's initialisers of a model built from scratch
+    _extend_vocab = False             # C2V_EXTEND_VOCAB=1 applies to this run (extend_vocab_run)
 
     def __init__(self, config: Config):
         self.engine: Optional[PathAttentionEngine] = None
@@ -294,7 +335,13 @@ class Code2VecModel(Code2VecModelBase):
             self._join_group()
             if self.rank != 0:
                 config.quiet()                       # rank 0 logs for every rank
+        # C2V_EXTEND_VOCAB=1: --load with --data continues at the loaded vocabularies extended by the dataset's words
+        self._extend_vocab = extend_vocab_run(config, extend_vocab_flag(os.environ), config.log)
         super().__init__(config)
+
+    def _make_vocabs(self):
+        from .vocabularies import Code2VecVocabs
+        return Code2VecVocabs(self.config, extend=self._extend_vocab)
 
     def _join_group(self):
         import torch
@@ -350,6 +397,15 @@ class Code2VecModel(Code2VecModelBase):
                           max_batch=max(c.TRAIN_BATCH_SIZE, c.TEST_BATCH_SIZE, 1),
                           top_k=c.TOP_K_WORDS_CONSIDERED_DURING_PREDICTION)
 
+    def _checkpoint_dims(self, dims: dict) -> dict:
+        """The model's dims `dims` (vars(EngineDims)) as a loaded checkpoint must have them: with C2V_EXTEND_VOCAB=1 the
+        table sizes are the loaded vocabularies', whose rows are the leading rows of the grown tables."""
+        if not self._extend_vocab:
+            return dims
+        sizes = self.vocabs.loaded_sizes
+        return dict(dims, token_vocab=sizes[VocabType.Token], path_vocab=sizes[VocabType.Path],
+                    target_vocab=sizes[VocabType.Target])
+
     def _make_engine(self, init: bool = False):
         """The engine and, for training or any multi-GPU run, its Trainer.  init: draw the initial parameters (on several
         GPUs before the Trainer moves the embedding tables into row shards)."""
@@ -371,7 +427,7 @@ class Code2VecModel(Code2VecModelBase):
             self.engine = make_fully_sharded_engine(self._engine_dims(), self.config.TRAIN_BATCH_SIZE // self.world,
                                                     self.local_rank, training=self.config.is_training)
             if init:
-                self.engine.init_params(whole_target_table=True)
+                self.engine.init_params(scheme=self._INIT_SCHEME, whole_target_table=True)
         else:
             device = int(os.environ.get("LOCAL_RANK", "0")) if torch.cuda.device_count() > 1 else 0
             self.engine = PathAttentionEngine(self._engine_dims(), device=device, training=self.config.is_training)
@@ -421,7 +477,7 @@ class Code2VecModel(Code2VecModelBase):
             self.trainer = Trainer(self.engine, keep_prob=self.config.DROPOUT_KEEP_RATE, seed=self._seed, adam=self._ADAM,
                                    deterministic=self._deterministic)
         if init and self.world == 1:
-            self.engine.init_params()
+            self.engine.init_params(scheme=self._INIT_SCHEME)
 
     def _create_inner_model(self):
         self._make_engine(init=True)
@@ -433,8 +489,13 @@ class Code2VecModel(Code2VecModelBase):
 
     def _load_inner_model(self):
         """`X.c2v_b200` when it exists, else the TensorFlow checkpoint `X.index` + `X.data-*` when that exists, else the
-        Keras backend's `X__only-weights` or `X__entire-model/` when one exists (_load_keras)."""
-        self._make_engine()
+        Keras backend's `X__only-weights` or `X__entire-model/` when one exists (_load_keras).  With C2V_EXTEND_VOCAB=1
+        the engine is built at the merged vocabulary sizes and initialised as a model built from scratch at those sizes;
+        the checkpoint, checked against the loaded sizes (_checkpoint_dims), then fills the leading rows."""
+        if self._extend_vocab:
+            self._make_engine(init=True)
+        else:
+            self._make_engine()
         load = self.config.MODEL_LOAD_PATH
         path = load + _CKPT_SUFFIX
         if not os.path.isfile(path) and os.path.isfile(load + INDEX_SUFFIX):
@@ -545,7 +606,7 @@ class Code2VecModel(Code2VecModelBase):
 
         def read_rows():
             out = self._sharded_tensors(with_optimizer=e.training)
-            check_checkpoint_dims(read_checkpoint_header(file_path)[0], vars(self._engine_dims()))
+            check_checkpoint_dims(read_checkpoint_header(file_path)[0], self._checkpoint_dims(vars(self._engine_dims())))
             meta = read_checkpoint_part(file_path, self.rank, self.world,
                                         (e.target_row0, e.target_row0 + e.dims.target_vocab), out)
             e.adam_t = int(meta.get("adam_t", 0))
@@ -579,13 +640,13 @@ class Code2VecModel(Code2VecModelBase):
         computed on the device as its rows arrive, then all compared with the stored ones."""
         import torch
         e = self.engine
-        entries, adam_t = bundle_entries(prefix, vars(e.dims), e.adam_m is not None, *self._adam_betas())
+        entries, adam_t = bundle_entries(prefix, self._checkpoint_dims(vars(e.dims)), e.adam_m is not None, *self._adam_betas())
         dest = {"theta": e.params, "adam_m": e.adam_m, "adam_v": e.adam_v}
         computed = torch.empty(len(entries), dtype=torch.int32, device=e.dev)
         with torch.cuda.device(e.dev), _PinnedStaging(e.dev) as stage:
             for i, ent in enumerate(entries):
                 group, name = ent["name"].split("/")
-                t = dest[group][name]
+                t = _lead(dest[group][name], ent["shape"])
                 stage.upload(ent["file"], ent["offset"], ent["nbytes"], t)
                 tensor_crc32c(t, *crc_view(name, ent["shape"]), computed[i:i + 1])
         self._check_crcs(entries, computed)
@@ -602,7 +663,7 @@ class Code2VecModel(Code2VecModelBase):
         state = {}
 
         def read_rows():
-            entries, adam_t = bundle_entries(prefix, vars(self._engine_dims()), e.training, *self._adam_betas())
+            entries, adam_t = bundle_entries(prefix, self._checkpoint_dims(vars(self._engine_dims())), e.training, *self._adam_betas())
             out = self._sharded_tensors(with_optimizer=e.training)
             read_entries_part(prefix, 0, entries, r, W, (e.target_row0, e.target_row0 + e.dims.target_vocab), out)
             torch.cuda.synchronize(e.dev)
@@ -619,8 +680,9 @@ class Code2VecModel(Code2VecModelBase):
                     tensor_crc32c(t, rows, row_bytes, computed[i:i + 1])
                     continue
                 # tok / path: local row i is global row i * W + r (ceil(T / W) rows per rank, padding past the end);
-                # tgt: rank r's block of ceil(Y / W) rows (the last one shorter), padded to that length
-                per = int(t.shape[0]) if name != "tgt" else (rows + W - 1) // W
+                # tgt: rank r's block of ceil(Y / W) rows (the last one shorter), padded to that length.  Y is the engine's:
+                # with C2V_EXTEND_VOCAB=1 the stored rows are the first `rows` of the grown table
+                per = int(t.shape[0]) if name != "tgt" else -(-e.global_target_vocab // W)
                 local = torch.zeros(per, dtype=torch.int32, device=e.dev)
                 n_own = min(per, int(t.shape[0]))
                 crc32c_rows(t, n_own, row_bytes, row_bytes, local)
@@ -705,7 +767,7 @@ class Code2VecModel(Code2VecModelBase):
         each chunk's row CRCs in file order, then c2v_rows_to_cols into the engine's [Y, D] tensor."""
         import torch
         e = self.engine
-        entries, adam_t, self._keras_save_counter = keras_entries(prefix, vars(e.dims), e.adam_m is not None,
+        entries, adam_t, self._keras_save_counter = keras_entries(prefix, self._checkpoint_dims(vars(e.dims)), e.adam_m is not None,
                                                                   self._ADAM or ADAM_DEFAULTS)
         dest = {"theta": e.params, "adam_m": e.adam_m, "adam_v": e.adam_v}
         computed = torch.empty(len(entries), dtype=torch.int32, device=e.dev)
@@ -713,7 +775,7 @@ class Code2VecModel(Code2VecModelBase):
             chunk = row_crc = None
             for i, ent in enumerate(entries):
                 group, name = ent["name"].split("/")
-                t = dest[group][name]
+                t = _lead(dest[group][name], ent["shape"])
                 if not ent["transposed"]:
                     stage.upload(ent["file"], ent["offset"], ent["nbytes"], t)
                     tensor_crc32c(t, *crc_view(name, ent["shape"]), computed[i:i + 1])
@@ -794,7 +856,7 @@ class Code2VecModel(Code2VecModelBase):
             (hlen,) = struct.unpack("<Q", f.read(8))
             meta = json.loads(f.read(hlen).decode())
             base = f.tell()
-            want = vars(e.dims)
+            want = self._checkpoint_dims(vars(e.dims))
             for key in ("token_vocab", "path_vocab", "target_vocab", "embed_dim", "code_dim"):
                 if meta["dims"][key] != want[key]:
                     raise ValueError("checkpoint %s=%s does not match the model (%s)" % (key, meta["dims"][key], want[key]))
@@ -805,7 +867,7 @@ class Code2VecModel(Code2VecModelBase):
                     continue
                 f.seek(base + ent["offset"])
                 arr = np.frombuffer(f.read(ent["nbytes"]), dtype="<f4").reshape(ent["shape"])
-                dest[group][name].copy_(torch.from_numpy(arr.copy()))
+                _lead(dest[group][name], ent["shape"]).copy_(torch.from_numpy(arr.copy()))
             e.adam_t = int(meta.get("adam_t", 0))
             if e.training:
                 # resuming: the engine's own step counter (lazy Adam needs consecutive steps and marks every row

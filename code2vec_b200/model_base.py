@@ -79,14 +79,17 @@ class Code2VecModelBase(abc.ABC):
         if not config.RELEASE:                      # a release run has no datasets to size
             self._init_num_of_examples()
         self._log_model_configuration()
-        self.vocabs = Code2VecVocabs(config)
+        self.vocabs = self._make_vocabs()
         self.vocabs.target_vocab.get_index_to_word_lookup_table()
         self._load_or_create_inner_model()
         self._initialize()
 
     def load_or_build(self):
-        self.vocabs = Code2VecVocabs(self.config)
+        self.vocabs = self._make_vocabs()
         self._load_or_create_inner_model()
+
+    def _make_vocabs(self) -> Code2VecVocabs:
+        return Code2VecVocabs(self.config)
 
     def _load_or_create_inner_model(self):
         (self._load_inner_model if self.config.is_loading else self._create_inner_model)()

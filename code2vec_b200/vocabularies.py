@@ -119,6 +119,25 @@ class Vocab:
 WordFreqDictType = Dict[str, int]
 
 
+def extend_vocab(loaded: Vocab, word_to_count: Dict[str, int], max_size: int) -> Vocab:
+    """`loaded` with the words a model trained from scratch on `word_to_count` would hold appended (C2V_EXTEND_VOCAB=1,
+    DESIGN.md §6m): every loaded word, the special words included, keeps its index, and each word of
+    create_from_freq_dict(word_to_count, max_size) that `loaded` does not hold follows, in that function's order.  Old
+    rows never move, so a table grown to the merged size keeps the loaded table as its leading rows."""
+    fresh = Vocab.create_from_freq_dict(loaded.vocab_type, word_to_count, max_size, loaded.special_words)
+    merged = Vocab(loaded.vocab_type, [], loaded.special_words)
+    merged.word_to_index = dict(loaded.word_to_index)
+    merged.index_to_word = dict(loaded.index_to_word)
+    merged.size = loaded.size
+    for i in range(len(fresh.index_to_word)):
+        word = fresh.index_to_word[i]
+        if word not in merged.word_to_index:
+            merged.word_to_index[word] = merged.size
+            merged.index_to_word[merged.size] = word
+            merged.size += 1
+    return merged
+
+
 class Code2VecWordFreqDicts(NamedTuple):
     """The three histograms of `<data>.dict.c2v`, in the order the file stores them (preprocess.py:12-20)."""
     token_to_count: WordFreqDictType
@@ -146,15 +165,19 @@ _DISK_ORDER = (VocabType.Token, VocabType.Target, VocabType.Path)       # dictio
 
 class Code2VecVocabs:
     """The token / path / target vocabularies of a model: built from the training histograms, or read
-    back from the `dictionaries.bin` stored next to a saved model (reference vocabularies.py:142-243)."""
+    back from the `dictionaries.bin` stored next to a saved model (reference vocabularies.py:142-243).
 
-    def __init__(self, config: Config):
+    extend: a run that loads and trains extends the loaded vocabularies by the training histograms' words (extend_vocab);
+    loaded_sizes then holds each vocabulary's size before the extension, else it is None."""
+
+    def __init__(self, config: Config, extend: bool = False):
         self.config = config
         self.token_vocab: Optional[Vocab] = None
         self.path_vocab: Optional[Vocab] = None
         self.target_vocab: Optional[Vocab] = None
+        self.loaded_sizes: Optional[Dict[VocabType, int]] = None
         self._already_saved_in_paths: Set[str] = set()
-        self._load_or_create()
+        self._load_or_create(extend)
 
     # ---- which special words a vocabulary starts with (vocabularies.py:204-209) -----------------
     def _get_special_words_by_vocab_type(self, vocab_type: VocabType) -> SpecialVocabWordsType:
@@ -163,7 +186,7 @@ class Code2VecVocabs:
         return _SpecialVocabWords_JoinedOovPad
 
     # ---- construction --------------------------------------------------------------------------------
-    def _load_or_create(self):
+    def _load_or_create(self, extend: bool = False):
         cfg = self.config
         assert cfg.is_training or cfg.is_loading
         if not cfg.is_loading:
@@ -174,6 +197,9 @@ class Code2VecVocabs:
             raise ValueError("Model dictionaries file is not found in model load dir. "
                              "Expecting file `{vocabularies_load_path}`.".format(vocabularies_load_path=stored))
         self._load_from_path(stored)
+        if extend and cfg.is_training:
+            self._extend_from_word_freq_dict()
+            self._already_saved_in_paths.discard(stored)                # the file holds the loaded vocabularies only
 
     def _load_from_path(self, vocabularies_load_path: str):
         assert os.path.exists(vocabularies_load_path)
@@ -202,6 +228,18 @@ class Code2VecVocabs:
                                                 special_words=self._get_special_words_by_vocab_type(kind))
             setattr(self, slot.attr, vocab)
             self.config.log("Created %s vocab. size: %d" % (slot.label, vocab.size))
+
+    def _extend_from_word_freq_dict(self):
+        histograms = self._load_word_freq_dict()
+        self.loaded_sizes = {}
+        for kind in _BUILD_ORDER:
+            slot = _SLOTS[kind]
+            loaded = getattr(self, slot.attr)
+            merged = extend_vocab(loaded, getattr(histograms, slot.histogram), getattr(self.config, slot.limit))
+            setattr(self, slot.attr, merged)
+            self.loaded_sizes[kind] = loaded.size
+            self.config.log("Extended %s vocab (C2V_EXTEND_VOCAB=1): %d + %d new words = %d" % (
+                slot.label, loaded.size, merged.size - loaded.size, merged.size))
 
     # ---- use -----------------------------------------------------------------------------------------
     def get(self, vocab_type: VocabType) -> Vocab:
