@@ -17,7 +17,7 @@ from typing import Iterable, Optional
 
 import numpy as np
 
-from . import load_model_dynamically, similarity
+from . import load_model_dynamically, name_scores, similarity
 from .common import common
 from .config import Config
 from .multi_rank import run_world
@@ -106,6 +106,22 @@ def write_nearest(model, c2v_path: str, topn: int) -> str:
     return out_path
 
 
+def write_name_scores(model, c2v_path: str) -> str:
+    """`<c2v_path>.name_scores`: one line per example evaluate() scores, in its order (name_scores.format_line); the
+    summary line is logged."""
+    names, target_ids, rank, logp, top1, top1_logp = model.score_names(c2v_path)
+    vocab = model.vocabs.target_vocab
+    in_vocab = target_ids != vocab.word_to_index[vocab.special_words.OOV]
+    top1_names = vocab.lookup_word(top1)
+    out_path = c2v_path + name_scores.SUFFIX
+    with open(out_path, "w") as f:
+        for r, name in enumerate(names):
+            f.write(name_scores.format_line(name, bool(in_vocab[r]), int(rank[r]), float(logp[r]), top1_names[r],
+                                            float(top1_logp[r])))
+    model.config.log(name_scores.summary_line(rank, logp, in_vocab))
+    return out_path
+
+
 def main(argv: Optional[Iterable[str]] = None) -> int:
     argv = list(sys.argv[1:] if argv is None else argv)
     predict_input = None
@@ -114,7 +130,9 @@ def main(argv: Optional[Iterable[str]] = None) -> int:
         predict_input = argv[i + 1]
         del argv[i:i + 2]
     argv, sim = similarity.split_cli_flags(argv)       # --most_similar, --most_similar_input, --nearest, --topn
+    argv, score_path = name_scores.split_cli_flags(argv)
     similarity.check_single_gpu(sim, run_world(os.environ)[0])
+    name_scores.check_single_gpu(score_path, run_world(os.environ)[0])
     config = Config(set_defaults=True)
     config.load_from_args(argv)
     config.verify()
@@ -162,6 +180,8 @@ def main(argv: Optional[Iterable[str]] = None) -> int:
                 print_most_similar(model, vocab_type, sys.stdin, sim.topn)
         if sim.nearest is not None:
             config.log("Nearest code vectors written to: %s" % write_nearest(model, sim.nearest, sim.topn))
+        if score_path is not None:
+            config.log("Name scores written to: %s" % write_name_scores(model, score_path))
     finally:
         model.close_session()
     return 0

@@ -1452,6 +1452,37 @@ class Code2VecModel(Code2VecModelBase):
             vectors.shape[0], nn.device_bytes() / 1e6))
         return names, vectors, idx, val
 
+    # ---- name scores (name_scores.py, DESIGN.md §6n) ------------------------------------------------------------------
+    def score_names(self, c2v_path: str):
+        """The examples of `c2v_path` that evaluate() scores -- in its order and its batches of TEST_BATCH_SIZE -- with each
+        one's own name scored over the whole target vocabulary on the GPU (c2v_name_scores): (names [N], target ids [N],
+        rank [N], logp [N], top1 [N], top1_logp [N]) as host arrays.  A name outside the target vocabulary has the OOV
+        word's id, and its rank and logp are that word's.  The full-softmax quantities are the same for both frameworks."""
+        import copy
+        import torch
+        if self.world > 1:
+            raise ValueError("score_names runs on one GPU; this run has %d ranks" % self.world)
+        cfg = copy.copy(self.config)
+        cfg.TEST_DATA_PATH = c2v_path
+        reader = PathContextReader(vocabs=self.vocabs, model_input_tensors_former=_EvaluateInputFormer(), config=cfg,
+                                   estimator_action=EstimatorAction.Evaluate)
+        e = self.engine
+        e.set_option("math_mode", self._math_eval)
+        names, parts = [], []
+        for batch in reader.get_dataset():
+            t = _EvaluateInputFormer().from_model_input_form(batch)
+            batch_names = [common.binary_to_string(n) for n in t.target_string]
+            ids = self.vocabs.target_vocab.lookup_index(batch_names)
+            code, _ = e.forward(e.to_device(t.path_source_token_indices, torch.int32), e.to_device(t.path_indices, torch.int32),
+                                e.to_device(t.path_target_token_indices, torch.int32),
+                                e.to_device(t.context_valid_mask, torch.float32), want_attention=False)
+            scores = e.name_scores(code, e.to_device(ids, torch.int32))
+            parts.append([ids] + [x.cpu().numpy() for x in scores])
+            names.extend(batch_names)
+        if not parts:
+            return (names, *(np.zeros(0, dt) for dt in (np.int32, np.int32, np.float32, np.int32, np.float32)))
+        return (names, *(np.concatenate(c) for c in zip(*parts)))
+
     def _gather_table(self, name: str):
         """The whole table `name` on every rank (a collective), in device memory: the embedding shards all-gathered and
         interleaved back (global row = local row * world + rank), or the target blocks all-gathered and concatenated."""

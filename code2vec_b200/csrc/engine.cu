@@ -14,6 +14,7 @@
 #include "../../include/c2v_b200.h"
 #include "common.cuh"
 #include "kernels.cuh"
+#include "name_rank.cuh"
 #include "sgemm.cuh"
 #include "umma_gemm.cuh"
 
@@ -156,10 +157,11 @@ Workspace carve(const c2v_dims& d) {
 // the launching stream; c2v_phase_stats() resolves them.
 enum Phase { PH_CTX_FWD = 0, PH_ATTN_FWD, PH_LOGITS, PH_XENT, PH_DV, PH_DY, PH_ATTN_BWD, PH_DW, PH_DX_SCATTER,
              PH_ADAM, PH_TOPK, PH_SAMPLED, PH_GATHER, PH_DX_GEMM, PH_ADAM_CATCHUP, PH_SPLIT, PH_ADAM_SWEEP, PH_PEER_SORT, PH_INBOX_APPLY,
-             PH_SAMPLER, PH_COUNT };
+             PH_SAMPLER, PH_NAME_RANK, PH_COUNT };
 const char* const kPhaseNames[PH_COUNT] = {"ctx_fwd", "attn_fwd", "logits", "xent", "dv", "dY", "attn_bwd", "dW",
                                            "dx_scatter", "adam", "topk", "sampled_softmax", "gather", "dx_gemm",
-                                           "adam_catchup", "split", "adam_sweep", "peer_sort", "inbox_apply", "sampler"};
+                                           "adam_catchup", "split", "adam_sweep", "peer_sort", "inbox_apply", "sampler",
+                                           "name_rank"};
 struct PhaseLog {
   std::vector<std::pair<cudaEvent_t, cudaEvent_t>> pending;
   std::vector<std::pair<cudaEvent_t, cudaEvent_t>> free_list;
@@ -1949,6 +1951,20 @@ int c2v_loss(c2v_engine* e, const float* code_vec, const int32_t* target, int32_
                                                               wsp<float>(e, e->ws.lse), 0)));
     C2V_LAUNCH(e, (loss_reduce_kernel<<<1, 256, 0, st>>>(wsp<float>(e, e->ws.loss_b), B, invB, loss_out)));
   }
+  return C2V_OK;
+}
+
+int c2v_name_scores(c2v_engine* e, const float* code_vec, const int32_t* target, int32_t B, int32_t* rank, float* logp,
+                    int32_t* top1, float* top1_logp, void* stream) {
+  int rc = check_batch(e, B);
+  if (rc) return rc;
+  if (!code_vec || !target || !rank || !logp || !top1 || !top1_logp) return fail(e, C2V_ERR_INVALID, "NULL argument");
+  C2V_CUDA(e, cudaSetDevice(e->device));
+  cudaStream_t st = (cudaStream_t)stream;
+  if ((rc = run_logits(e, st, code_vec, B, LOGITS_STORE))) return rc;       // the slab topk_impl scans, bit for bit
+  PhaseTimer pt(e, PH_NAME_RANK, st);
+  C2V_LAUNCH(e, (name_rank_kernel<<<B, kNameRankThreads, 0, st>>>(wsp<float>(e, e->ws.S), e->ws.ldS, e->dims.target_vocab,
+                                                                     target, rank, logp, top1, top1_logp)));
   return C2V_OK;
 }
 

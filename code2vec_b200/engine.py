@@ -76,6 +76,7 @@ _SIGNATURES = {
     "c2v_forward": (C.c_int, [_P, _P, _P, _P, _P, _I32, _P, _P, _P]),
     "c2v_topk": (C.c_int, [_P, _P, _I32, _P, _P, _I32, _P]),
     "c2v_loss": (C.c_int, [_P, _P, _P, _I32, _P, _P]),
+    "c2v_name_scores": (C.c_int, [_P, _P, _P, _I32, _P, _P, _P, _P, _P]),
     "c2v_train_step": (C.c_int, [_P, _P, _P, _P, _P, _P, _I32, C.c_float, C.c_uint64, C.c_uint64, _P, _P, _P]),
     "c2v_sampled_train_step": (C.c_int, [_P, _P, _P, _P, _P, _P, _I32, _P, _I32, _P, _P, C.c_float,
                                          C.c_uint64, C.c_uint64, _P, _P, _P]),
@@ -547,6 +548,21 @@ class PathAttentionEngine:
         self._check(self.lib.c2v_loss(self.h, code_vec.data_ptr(), target.data_ptr(), code_vec.shape[0],
                                       out.data_ptr(), self._stream()))
         return out
+
+    def name_scores(self, code_vec, target):
+        """c2v_name_scores: (rank [B] int32, logp [B], top1 [B] int32, top1_logp [B]) device tensors -- each example's own
+        name (target [B] int32, device) ranked and scored over the whole target vocabulary, in the current math mode."""
+        torch = self.torch
+        B = code_vec.shape[0]
+        if tuple(target.shape) != (B,) or target.dtype != torch.int32 or target.device != self.dev:
+            raise ValueError("target must be a [%d] int32 tensor on %s" % (B, self.dev))
+        rank = torch.empty(B, dtype=torch.int32, device=self.dev)
+        top1 = torch.empty(B, dtype=torch.int32, device=self.dev)
+        logp = torch.empty(B, dtype=torch.float32, device=self.dev)
+        top1_logp = torch.empty(B, dtype=torch.float32, device=self.dev)
+        self._check(self.lib.c2v_name_scores(self.h, code_vec.data_ptr(), target.data_ptr(), B, rank.data_ptr(),
+                                             logp.data_ptr(), top1.data_ptr(), top1_logp.data_ptr(), self._stream()))
+        return rank, logp, top1, top1_logp
 
     def train_step(self, src, path, tgt, mask, target, keep: float = 1.0, seed: int = 0, step: int = 0,
                    dropout_mask=None, loss_out=None):

@@ -196,6 +196,22 @@ int c2v_topk(c2v_engine* e, const float* code_vec, int32_t B, int32_t* idx, floa
 int c2v_loss(c2v_engine* e, const float* code_vec, const int32_t* target, int32_t B,
              float* loss_out, void* stream);
 
+/* Scores of each example's own name over the whole target vocabulary (NOT IN THE REFERENCE; DESIGN.md §6n): the logits
+ * S_b = code_vec_b . TARGET_WORDS_VOCAB^T in the engine's current math mode -- the slab c2v_topk scans, bit for bit --
+ * then one pass over each row.  With t_b = S_b[y_b], y_b = target[b], m_b = max_j S_b[j] and
+ * lse_b = m_b + log sum_j exp(S_b[j] - m_b):
+ *   rank      : 1 + #{j : S_b[j] > t_b} + #{j < y_b : S_b[j] == t_b}, 1-based in tf.nn.top_k's order (value descending,
+ *               ties to the lower index): a rank r <= k puts y_b at c2v_topk's idx[b, r - 1]
+ *   logp      : t_b - lse_b, the full-softmax log-probability of the target
+ *   top1      : the lowest j with S_b[j] == m_b (c2v_topk's idx[b, 0])
+ *   top1_logp : m_b - lse_b
+ * A row whose logits hold a NaN gets rank 0 and NaN log-probabilities; a target outside [0, target_vocab) rank -1 and
+ * NaN log-probabilities.  code_vec: device [B, D] (as c2v_loss); target: device int32 [B]; rank, top1: device int32 [B];
+ * logp, top1_logp: device float [B].  No memory beyond the bound workspace.  On a row-sharded target table each engine
+ * sees only its rows: the result is its block's, not the model's. */
+int c2v_name_scores(c2v_engine* e, const float* code_vec, const int32_t* target, int32_t B,
+                    int32_t* rank, float* logp, int32_t* top1, float* top1_logp, void* stream);
+
 /* Forward + backward of the training graph (tensorflow_model.py:197-234 without the Adam
  * update): dropout with keep probability `keep_prob` (config.py:69; 1.0 disables it), full
  * softmax loss, gradients of all five variables written to the bound gradient tensors
