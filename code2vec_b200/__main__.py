@@ -95,7 +95,10 @@ def print_most_similar(model, vocab_type: VocabType, lines: Iterable[str], topn:
 
 
 def write_nearest(model, c2v_path: str, topn: int) -> str:
-    """`<c2v_path>.nearest`: line r is example r's name, then `\\t<row>,<name>,<similarity>` per nearest other example."""
+    """`<c2v_path>.nearest`: line r is example r's name, then `\\t<row>,<name>,<similarity>` per nearest other example.
+    With C2V_DEVICE_EVAL=1 the corpus is read, searched and the file written on the GPU (DESIGN.md §6o)."""
+    if getattr(model, "device_eval", False):
+        return model.write_nearest_device(c2v_path, topn)
     names, _vectors, idx, val = model.nearest_code_vectors(c2v_path, topn)
     out_path = c2v_path + ".nearest"
     pad = np.iinfo(np.int32).max
@@ -108,7 +111,9 @@ def write_nearest(model, c2v_path: str, topn: int) -> str:
 
 def write_name_scores(model, c2v_path: str) -> str:
     """`<c2v_path>.name_scores`: one line per example evaluate() scores, in its order (name_scores.format_line); the
-    summary line is logged."""
+    summary line is logged.  With C2V_DEVICE_EVAL=1 the corpus is read, scored and the file written on the GPU (§6o)."""
+    if getattr(model, "device_eval", False):
+        return model.write_name_scores_device(c2v_path)
     names, target_ids, rank, logp, top1, top1_logp = model.score_names(c2v_path)
     vocab = model.vocabs.target_vocab
     in_vocab = target_ids != vocab.word_to_index[vocab.special_words.OOV]

@@ -37,7 +37,7 @@ from .multi_rank import (CKPT_MAGIC, CKPT_SUFFIX, batch_split, check_checkpoint_
 from .tf_bundle import INDEX_SUFFIX, bundle_entries, bundle_layout, crc_view, data_file, save_format_flag, write_index
 from .tf_bundle import crc32c as host_crc32c
 from . import device_reader as _device_reader_mod
-from .device_reader import device_eval_flag, device_reader_flag, sharded_reader_flag
+from .device_reader import device_eval_flag, device_reader_flag, evaluation_route_line, sharded_reader_flag
 from .device_predict import device_predict_flag
 from .text_export import DeviceTextWriter, device_text_flag
 from .trainer import ADAM_DEFAULTS, Trainer, make_fully_sharded_engine
@@ -331,6 +331,8 @@ class Code2VecModel(Code2VecModelBase):
         self._device_vocabs = None               # device_reader.DeviceVocabs, shared by the training and evaluation readers
         self._eval_tables = None                 # device_reader.eval_tables of the target vocabulary
         self._dev_eval_reader = None
+        self._dev_corpus_reader = None           # C2V_DEVICE_EVAL=1: the reader of --score_names / --nearest's corpus
+        self._dev_corpus_path = None
         if self.world > 1:
             self._join_group()
             if self.rank != 0:
@@ -457,9 +459,7 @@ class Code2VecModel(Code2VecModelBase):
         self._hint_next = os.environ.get("C2V_HINT_NEXT", "0") == "1"
         self.log("b200 backend training reader: %s (C2V_DEVICE_READER=%d)" % (
             "on the GPU" if self._device_reader else "on the host", self._device_reader))
-        self.log("b200 backend evaluation: %s (C2V_DEVICE_EVAL=%d)" % (
-            "read, predicted and scored on the GPU" if self._device_eval else "read and scored on the host",
-            self._device_eval))
+        self.log(evaluation_route_line(self._device_eval))
         self.log("b200 backend text export: `.vectors` and word2vec files formatted %s (C2V_DEVICE_TEXT=%d)" % (
             "on the GPU" if self._device_text else "on the host", self._device_text))
         self.log("b200 backend predict: %s (C2V_DEVICE_PREDICT=%d)" % (
@@ -516,6 +516,9 @@ class Code2VecModel(Code2VecModelBase):
         if self._dev_eval_reader is not None:
             self._dev_eval_reader.close()
             self._dev_eval_reader = None
+        if self._dev_corpus_reader is not None:
+            self._dev_corpus_reader.close()
+            self._dev_corpus_reader = None
         self._device_vocabs = None
         if getattr(self, "_knn_handle", None) is not None:
             self._knn_handle.close()
@@ -1428,6 +1431,8 @@ class Code2VecModel(Code2VecModelBase):
         import copy
         import torch
         from . import similarity
+        if self._device_eval:
+            return self._nearest_device(c2v_path, topn)
         nn = self._knn()
         cfg = copy.copy(self.config)
         cfg.TEST_DATA_PATH = c2v_path
@@ -1462,6 +1467,8 @@ class Code2VecModel(Code2VecModelBase):
         import torch
         if self.world > 1:
             raise ValueError("score_names runs on one GPU; this run has %d ranks" % self.world)
+        if self._device_eval:
+            return self._score_names_device(c2v_path)
         cfg = copy.copy(self.config)
         cfg.TEST_DATA_PATH = c2v_path
         reader = PathContextReader(vocabs=self.vocabs, model_input_tensors_former=_EvaluateInputFormer(), config=cfg,
@@ -1482,6 +1489,183 @@ class Code2VecModel(Code2VecModelBase):
         if not parts:
             return (names, *(np.zeros(0, dt) for dt in (np.int32, np.int32, np.float32, np.int32, np.float32)))
         return (names, *(np.concatenate(c) for c in zip(*parts)))
+
+    # ---- --score_names and --nearest on the GPU (C2V_DEVICE_EVAL=1, DESIGN.md §6o) -----------------------------------
+    @property
+    def device_eval(self) -> bool:
+        return self._device_eval
+
+    def _device_corpus_reader(self, c2v_path: str):
+        """The GPU evaluation reader of the corpus `c2v_path` (not TEST_DATA_PATH), sharing the model's device
+        vocabularies; made once per path (and again after a pass that failed).  Its names are checked as UTF-8 chunk by
+        chunk, as the host reader decodes them."""
+        import copy
+        from .device_reader import DeviceBatchReader, eval_tables
+        if self._dev_corpus_reader is not None and self._dev_corpus_path != c2v_path:
+            self._dev_corpus_reader.close()
+            self._dev_corpus_reader = None
+        if self._dev_corpus_reader is None:
+            cfg = copy.copy(self.config)
+            cfg.TEST_DATA_PATH = c2v_path
+            reader = PathContextReader(vocabs=self.vocabs, model_input_tensors_former=_EvaluateInputFormer(), config=cfg,
+                                       estimator_action=EstimatorAction.Evaluate)
+            if self._eval_tables is None:
+                self._eval_tables = eval_tables(self.vocabs.target_vocab)
+            self._dev_corpus_reader = DeviceBatchReader(reader, self.engine.dev, vocabs=self._shared_device_vocabs(reader),
+                                                        tables=self._eval_tables, check_utf8=True)
+            self._dev_corpus_path = c2v_path
+        return self._dev_corpus_reader
+
+    def _device_corpus_pass(self, c2v_path: str, per_batch):
+        """One pass over the examples of `c2v_path` that evaluate() scores, in its order and its batches of
+        TEST_BATCH_SIZE, read and encoded on the GPU: per_batch(batch, n, code) for each batch of n rows, with its code
+        vectors [n, D] (device) in the evaluation math mode.  per_batch queues its device work on the current stream
+        (the batch's slot is handed back after it).  The host reader's exceptions for a malformed corpus are raised."""
+        if self.world > 1:
+            raise ValueError("--score_names and --nearest run on one GPU; this run has %d ranks" % self.world)
+        reader = self._device_corpus_reader(c2v_path)
+        e = self.engine
+        e.set_option("math_mode", self._math_eval)
+        try:
+            for batch in reader:
+                batch.wait()
+                n = batch.hi - batch.lo
+                code, _ = e.forward(*batch.tensors[:4], want_attention=False)
+                per_batch(batch, n, code)
+                batch.release()
+        except BaseException:
+            reader.close()                             # a pass that stopped early leaves rows queued
+            self._dev_corpus_reader = None
+            raise
+
+    @staticmethod
+    def _host_names(names, off, n: int) -> List[str]:
+        """The n names names[off[j], off[j + 1]) (device uint8 / int64) decoded on the host."""
+        off = off[:n + 1].cpu().numpy()
+        blob = names[:int(off[n])].cpu().numpy().tobytes()
+        return [blob[off[j]:off[j + 1]].decode("utf-8") for j in range(n)]
+
+    def _score_names_device(self, c2v_path: str, stage=None):
+        """score_names on the GPU route: the same arrays.  With a corpus_text.LineStage, each batch's lines of
+        `<corpus>.name_scores` are formatted on the GPU into it, and the names stay on the device (None is returned for
+        them)."""
+        import ctypes as C
+        e, lib = self.engine, self.engine.lib
+        vocab = self.vocabs.target_vocab
+        oov = vocab.word_to_index[vocab.special_words.OOV]
+        names, parts = ([] if stage is None else None), []
+
+        def per_batch(batch, n, code):
+            target = batch.tensors[4]
+            rank, logp, top1, top1_logp = e.name_scores(code, target)
+            s = batch._slot
+            if stage is not None:
+                words, word_off, n_words = self._dev_corpus_reader.eval_words()
+                scratch, scratch_bytes = stage.scratch_for(n)
+
+                def fmt(out, cap, total):
+                    e._check(lib.c2v_name_scores_text(
+                        n, s["names"].data_ptr(), s["name_off"].data_ptr(), target.data_ptr(), oov, rank.data_ptr(),
+                        logp.data_ptr(), top1.data_ptr(), top1_logp.data_ptr(), words, word_off, n_words, scratch,
+                        scratch_bytes, out, cap, total, e._stream()))
+                stage.emit(fmt)
+            else:
+                names.extend(self._host_names(s["names"], s["name_off"], n))
+            parts.append([x.cpu().numpy() for x in (target, rank, logp, top1, top1_logp)])
+
+        self._device_corpus_pass(c2v_path, per_batch)
+        if not parts:
+            return (names, *(np.zeros(0, dt) for dt in (np.int32, np.int32, np.float32, np.int32, np.float32)))
+        return (names, *(np.concatenate(c) for c in zip(*parts)))
+
+    def write_name_scores_device(self, c2v_path: str) -> str:
+        """`<c2v_path>.name_scores` read, scored and formatted on the GPU: __main__.write_name_scores' bytes and summary
+        line.  The file appears only once the whole corpus is scored (a corpus the reader rejects leaves none)."""
+        from . import name_scores
+        from .corpus_text import LineStage, atomic_output
+        out_path = c2v_path + name_scores.SUFFIX
+        with atomic_output(out_path) as f:
+            stage = LineStage(f, self.engine.dev)
+            try:
+                _, target, rank, logp, _, _ = self._score_names_device(c2v_path, stage)
+            finally:
+                stage.close()
+        self.corpus_text_stage = stage             # its timings and peak memory (tools/corpus_rate.py)
+        vocab = self.vocabs.target_vocab
+        in_vocab = target != vocab.word_to_index[vocab.special_words.OOV]
+        self.log(name_scores.summary_line(rank, logp, in_vocab))
+        return out_path
+
+    def _nearest_device(self, c2v_path: str, topn: int, stage=None):
+        """nearest_code_vectors on the GPU route: the code vectors [N, D] and the names of the N rows gathered in device
+        memory, then c2v_knn_search.  Without a stage, the host arrays nearest_code_vectors returns; with a
+        corpus_text.LineStage, the lines of `<corpus>.nearest` formatted on the GPU into it, and None."""
+        import torch
+        from . import similarity
+        from .corpus_text import NEAREST_ROWS
+        nn = self._knn()
+        e = self.engine
+        D = self.config.CODE_VECTOR_SIZE
+        acc = {"n": 0, "vec": None, "names": None, "off": None, "name_bytes": 0}
+        nb_host = torch.zeros(1, dtype=torch.int64).pin_memory()
+
+        def grow(t, need, make):
+            if t is not None and t.shape[0] >= need:
+                return t
+            bigger = make(max(need, 2 * (0 if t is None else t.shape[0]), 1024))
+            if t is not None:
+                bigger[:t.shape[0]].copy_(t)
+            return bigger
+
+        def per_batch(batch, n, code):
+            s = batch._slot
+            nb_host.copy_(s["name_off"][n:n + 1])                     # the batch's name bytes
+            N, base = acc["n"], acc["name_bytes"]
+            acc["vec"] = grow(acc["vec"], N + n, lambda m: torch.empty((m, D), dtype=torch.float32, device=e.dev))
+            acc["off"] = grow(acc["off"], N + n + 1, lambda m: torch.zeros(m, dtype=torch.int64, device=e.dev))
+            acc["vec"][N:N + n].copy_(code)
+            acc["off"][N + 1:N + n + 1].copy_(s["name_off"][1:n + 1] + base)
+            nb = int(nb_host[0])
+            acc["names"] = grow(acc["names"], base + nb, lambda m: torch.empty(m, dtype=torch.uint8, device=e.dev))
+            acc["names"][base:base + nb].copy_(s["names"][:nb])
+            acc["n"], acc["name_bytes"] = N + n, base + nb
+
+        self._device_corpus_pass(c2v_path, per_batch)
+        N = acc["n"]
+        if N == 0:
+            empty = (np.zeros((0, D), dtype=np.float32), np.zeros((0, topn), np.int32), np.zeros((0, topn), np.float32))
+            return None if stage is not None else ([], *empty)
+        vectors = acc["vec"][:N]
+        self._knn_bound = None
+        idx, val = similarity.nearest_rows_device(nn, vectors, topn, self._math_eval)
+        self.log("Nearest neighbours: %d code vectors, %.1f MB of device memory held" % (N, nn.device_bytes() / 1e6))
+        if stage is None:
+            names = self._host_names(acc["names"], acc["off"], N)
+            return names, vectors.cpu().numpy(), idx.cpu().numpy(), val.cpu().numpy()
+        for r0 in range(0, N, NEAREST_ROWS):
+            n = min(NEAREST_ROWS, N - r0)
+            scratch, scratch_bytes = stage.scratch_for(n)
+
+            def fmt(out, cap, total, r0=r0, n=n):
+                e._check(e.lib.c2v_nearest_text(r0, n, N, topn, acc["names"].data_ptr(), acc["off"].data_ptr(),
+                                                idx.data_ptr(), val.data_ptr(), scratch, scratch_bytes, out, cap, total,
+                                                e._stream()))
+            stage.emit(fmt)
+        return None
+
+    def write_nearest_device(self, c2v_path: str, topn: int) -> str:
+        """`<c2v_path>.nearest` read, searched and formatted on the GPU: __main__.write_nearest's bytes, without the
+        [N, D] code vectors leaving the device.  The file appears only once the whole corpus is searched."""
+        from .corpus_text import LineStage, atomic_output
+        out_path = c2v_path + ".nearest"
+        with atomic_output(out_path) as f:
+            stage = LineStage(f, self.engine.dev)
+            try:
+                self._nearest_device(c2v_path, topn, stage)
+            finally:
+                stage.close()
+        self.corpus_text_stage = stage             # its timings and peak memory (tools/corpus_rate.py)
+        return out_path
 
     def _gather_table(self, name: str):
         """The whole table `name` on every rank (a collective), in device memory: the embedding shards all-gathered and

@@ -16,7 +16,8 @@ CSRC = os.path.join(PKG_DIR, "csrc")
 LIB_PATH = os.path.join(PKG_DIR, "libc2v_b200.so")
 OBJ_DIR = os.path.join(PKG_DIR, "csrc", "_obj")
 
-SOURCES = ["engine.cu", "reader.cu", "text.cu", "preprocess.cu", "knn.cu", "predict.cu", "sampler.cu", "crc32c.cu"]
+SOURCES = ["engine.cu", "reader.cu", "text.cu", "preprocess.cu", "knn.cu", "predict.cu", "sampler.cu", "crc32c.cu",
+           "corpus_text.cu"]
 NVCC_FLAGS = [
     "-gencode", "arch=compute_90a,code=sm_90a", "-O3", "-lineinfo", "-std=c++17",
     "-Xcompiler", "-fPIC", "--expt-relaxed-constexpr",

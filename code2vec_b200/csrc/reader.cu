@@ -669,6 +669,36 @@ eval_score_kernel(EvalTables T, const int32_t* __restrict__ ids, int n, int k, c
   }
 }
 
+// ---- names Python's strict UTF-8 decoder accepts (c2v_reader_eval_check_utf8) ----------------------------------------
+// Well-formed UTF-8 as str.decode("utf-8") takes it: no overlong forms, no surrogates (ED A0..BF), nothing above U+10FFFF.
+__device__ bool utf8_valid(const unsigned char* s, long long n) {
+  long long p = 0;
+  while (p < n) {
+    const unsigned char c = s[p];
+    if (c < 0x80) { ++p; continue; }
+    int len;
+    unsigned char lo = 0x80, hi = 0xBF;                 // the range of the second byte
+    if (c >= 0xC2 && c <= 0xDF) len = 2;
+    else if (c >= 0xE0 && c <= 0xEF) { len = 3; if (c == 0xE0) lo = 0xA0; if (c == 0xED) hi = 0x9F; }
+    else if (c >= 0xF0 && c <= 0xF4) { len = 4; if (c == 0xF0) lo = 0x90; if (c == 0xF4) hi = 0x8F; }
+    else return false;
+    if (p + len > n || s[p + 1] < lo || s[p + 1] > hi) return false;
+    for (int i = 2; i < len; ++i)
+      if (s[p + i] < 0x80 || s[p + i] > 0xBF) return false;
+    p += len;
+  }
+  return true;
+}
+
+// *bad = the lowest queue row in [q0, q0 + n) whose name is not valid UTF-8 (left as is when there is none); one thread a row
+__global__ void __launch_bounds__(256) eval_utf8_kernel(const long long* __restrict__ noff, const unsigned char* __restrict__ names,
+                                                        long long q0, long long n, unsigned long long* __restrict__ bad) {
+  for (long long j = (long long)blockIdx.x * 256 + threadIdx.x; j < n; j += (long long)gridDim.x * 256) {
+    const long long o = noff[q0 + j];
+    if (!utf8_valid(names + o, noff[q0 + j + 1] - o)) atomicMin(bad, (unsigned long long)(q0 + j));
+  }
+}
+
 }  // namespace
 
 struct c2v_reader {
@@ -1265,6 +1295,42 @@ int c2v_reader_eval_take(c2v_reader* r, int32_t b, int32_t* src, int32_t* path, 
 }
 
 int64_t c2v_reader_eval_queued(const c2v_reader* r) { return r ? r->eq_len - r->eq_head : -1; }
+
+int c2v_reader_eval_check_utf8(c2v_reader* r, int64_t rows, char* name, int64_t name_cap, int64_t* name_len, void* stream) {
+  if (!r || !name_len || rows < 0 || name_cap < 0 || (name_cap && !name))
+    return rfail(C2V_ERR_INVALID, "c2v_reader_eval_check_utf8: NULL argument or negative size");
+  if (rows > r->eq_len - r->eq_head)
+    return rfail(C2V_ERR_INVALID, "c2v_reader_eval_check_utf8: rows must be at most the queued rows");
+  *name_len = -1;
+  if (rows == 0) return C2V_OK;
+  RD_CUDA(cudaSetDevice(r->device));
+  cudaStream_t st = (cudaStream_t)stream;
+  const long long q0 = r->eq_len - rows;
+  RD_CUDA(cudaMemsetAsync(r->bad, 0xff, sizeof(unsigned long long), st));
+  eval_utf8_kernel<<<row_grid(r, rows), 256, 0, st>>>(r->eq_noff, r->eq_names, q0, rows, r->bad);
+  RD_CUDA(cudaGetLastError());
+  RD_CUDA(cudaMemcpyAsync(&r->host->bad, r->bad, sizeof(unsigned long long), cudaMemcpyDeviceToHost, st));
+  RD_CUDA(cudaStreamSynchronize(st));
+  if (r->host->bad == ~0ull) return C2V_OK;
+  long long off[2];
+  RD_CUDA(cudaMemcpyAsync(off, r->eq_noff + r->host->bad, 2 * sizeof(long long), cudaMemcpyDeviceToHost, st));
+  RD_CUDA(cudaStreamSynchronize(st));
+  const long long len = off[1] - off[0];
+  if (len > 0 && name_cap > 0)
+    RD_CUDA(cudaMemcpyAsync(name, r->eq_names + off[0], (size_t)(len < name_cap ? len : name_cap), cudaMemcpyDeviceToHost, st));
+  RD_CUDA(cudaStreamSynchronize(st));
+  *name_len = len;
+  return C2V_OK;
+}
+
+int c2v_reader_eval_words(const c2v_reader* r, const char** words, const int64_t** word_off, int32_t* n_words) {
+  if (!r || !words || !word_off || !n_words) return rfail(C2V_ERR_INVALID, "c2v_reader_eval_words: NULL argument");
+  if (!r->tab_mem) return rfail(C2V_ERR_STATE, "c2v_reader_eval_words: upload the tables first (c2v_reader_eval_tables)");
+  *words = (const char*)r->tab.words;
+  *word_off = (const int64_t*)r->tab.word_off;
+  *n_words = r->tab.Y;
+  return C2V_OK;
+}
 
 int c2v_reader_eval_score(const c2v_reader* r, const int32_t* ids, int32_t n, int32_t k, const int64_t* name_off,
                           const char* names, int32_t* rank, int32_t* first, int32_t* flags, int64_t* acc, void* stream) {

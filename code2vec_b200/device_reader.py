@@ -55,6 +55,16 @@ def device_eval_flag(environ) -> bool:
     return flag == "1"
 
 
+def evaluation_route_line(device_eval: bool) -> str:
+    """The start-up log line of the evaluation route: evaluate(), --score_names and --nearest on the GPU or the host."""
+    if device_eval:
+        route = ("evaluate() read, predicted and scored on the GPU; --score_names and --nearest read, scored or searched "
+                 "and written on the GPU")
+    else:
+        route = "evaluate(), --score_names and --nearest read and scored on the host"
+    return "b200 backend evaluation: %s (C2V_DEVICE_EVAL=%d)" % (route, int(device_eval))
+
+
 def sharded_reader_flag(environ) -> bool:
     """C2V_SHARDED_READER=1 (with C2V_DEVICE_READER=1): on several GPUs each rank reads and parses 1/W of every chunk and
     takes the other rows from its peers; 0 (the default): every rank reads the whole file."""
@@ -245,15 +255,19 @@ class DeviceBatchReader:
     queue (no draws, no RNG), and the reader may be iterated again once a pass has ended."""
 
     def __init__(self, reader: PathContextReader, device, world: int = 1, rank: int = 0, slots: int = 4,
-                 transport: Optional[ShareTransport] = None, vocabs: Optional[DeviceVocabs] = None, tables=None):
+                 transport: Optional[ShareTransport] = None, vocabs: Optional[DeviceVocabs] = None, tables=None,
+                 check_utf8: bool = False):
         """transport: read the chunks sharded across the `world` ranks, meeting through it (ignored on one rank).
         vocabs: the model's DeviceVocabs (uploaded here when None).  tables: eval_tables(target vocabulary), needed by
-        an evaluation reader (an evaluate-mode `reader`); every rank of an evaluation reads the whole file."""
+        an evaluation reader (an evaluate-mode `reader`); every rank of an evaluation reads the whole file.  check_utf8
+        (evaluation): each chunk's names are checked as the host reader decodes them, so a name that is not valid UTF-8
+        raises the host reader's UnicodeDecodeError at the same chunk."""
         import torch
         action = reader.estimator_action
         if not (action.is_train or action.is_evaluate):
             raise ValueError("the device reader reads training and evaluation files only")
         self.evaluate = action.is_evaluate
+        self.check_utf8 = bool(check_utf8)
         if self.evaluate and tables is None:
             raise ValueError("an evaluation reader needs the target-word tables (device_reader.eval_tables)")
         if slots < 3:
@@ -381,7 +395,33 @@ class DeviceBatchReader:
                 _raise_parse_error(-(bad_line.value + 1), bad_kind.value, self.C)
             raise EngineError(rc, self.lib.c2v_last_error(None).decode())
         self._name_bytes = int(name_bytes.value)
+        if self.check_utf8 and kept.value:
+            self._check_utf8(int(kept.value))
         return int(kept.value)
+
+    def _check_utf8(self, rows: int):
+        """The names of the last `rows` queued rows decoded as the host reader decodes them: the first one that is not
+        valid UTF-8 raises the decoder's own UnicodeDecodeError."""
+        buf, n = C.create_string_buffer(1 << 16), C.c_int64()
+        while True:
+            rc = self.lib.c2v_reader_eval_check_utf8(self.h, rows, buf, len(buf), C.byref(n), self.stream.cuda_stream)
+            if rc != 0:
+                raise EngineError(rc, self.lib.c2v_last_error(None).decode())
+            if n.value <= len(buf):
+                break
+            buf = C.create_string_buffer(n.value)          # a name longer than the buffer: again, all of it
+        if n.value >= 0:
+            name = buf.raw[:n.value]
+            name.decode("utf-8")
+            raise RuntimeError("c2v_reader_eval_check_utf8 flagged a name the UTF-8 decoder accepts: %r" % name)
+
+    def eval_words(self):
+        """(words, word_off, n_words): the device pointers of the target words of an evaluation reader's tables."""
+        w, off, n = C.c_void_p(), C.c_void_p(), C.c_int32()
+        rc = self.lib.c2v_reader_eval_words(self.h, C.byref(w), C.byref(off), C.byref(n))
+        if rc != 0:
+            raise EngineError(rc, self.lib.c2v_last_error(None).decode())
+        return w.value, off.value, int(n.value)
 
     def _take(self, b: int, k: int):
         """Batch k: the queue's next b rows and their names; None when the consumer has gone."""

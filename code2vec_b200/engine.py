@@ -146,6 +146,8 @@ _SIGNATURES = {
     "c2v_reader_eval_take": (C.c_int, [_P, _I32, _P, _P, _P, _P, _P, _P, _P, C.c_int64, _P]),
     "c2v_reader_eval_queued": (C.c_int64, [_P]),
     "c2v_reader_eval_score": (C.c_int, [_P, _P, _I32, _I32, _P, _P, _P, _P, _P, _P, _P]),
+    "c2v_reader_eval_check_utf8": (C.c_int, [_P, C.c_int64, _P, C.c_int64, C.POINTER(C.c_int64), _P]),
+    "c2v_reader_eval_words": (C.c_int, [_P, C.POINTER(_P), C.POINTER(_P), C.POINTER(_I32)]),
     # text of float32 matrices (text_export.py)
     "c2v_text_format_rows": (C.c_int, [_P, C.c_int64, _I32, C.c_int64, _P, _P, _P, C.c_size_t, _P, C.c_int64, _P, _P,
                                        _P]),
@@ -186,6 +188,12 @@ _SIGNATURES = {
     "c2v_pred_rows": (C.c_int, [_P, _P, _I32, _P, _P, _P, _P, _P]),
     "c2v_pred_format": (C.c_int, [_P, _I32, _P, _P, _I32, _P, _P, _I32, _P, C.c_int64, _P, _P, _P]),
     "c2v_selftest_format_fixed": (C.c_int, [_P, C.c_int64, _P, _P]),
+    # corpus text (corpus_text.py)
+    "c2v_corpus_text_scratch_bytes": (C.c_size_t, [C.c_int64]),
+    "c2v_name_scores_text": (C.c_int, [_I32, _P, _P, _P, _I32, _P, _P, _P, _P, _P, _P, _I32, _P, C.c_size_t, _P,
+                                       C.c_int64, _P, _P]),
+    "c2v_nearest_text": (C.c_int, [C.c_int64, C.c_int64, C.c_int64, _I32, _P, _P, _P, _P, _P, C.c_size_t, _P, C.c_int64,
+                                   _P, _P]),
 }
 
 _lib = None

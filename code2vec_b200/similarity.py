@@ -211,14 +211,19 @@ def most_similar(nn: NearestNeighbours, word_to_index, index_to_word, positive: 
     return [(index_to_word[int(i)], float(v)) for i, v in zip(idx, val) if i != np.iinfo(np.int32).max]
 
 
-def nearest_rows(nn: NearestNeighbours, vectors, topn: int, math: int):
-    """The topn nearest other rows of every row of vectors [N, D] (device) by cosine: (ids, values) [N, topn] on the
-    host, padded with (INT_MAX, -inf).  Each row's query is its own unit-normalised vector, and only its own row is
+def nearest_rows_device(nn: NearestNeighbours, vectors, topn: int, math: int):
+    """The topn nearest other rows of every row of vectors [N, D] (device) by cosine: (ids, values) [N, topn] as device
+    tensors, padded with (INT_MAX, -inf).  Each row's query is its own unit-normalised vector, and only its own row is
     excluded: two rows with identical vectors are each other's nearest."""
     if topn + 1 > MAX_CANDIDATES:
         raise ValueError("--topn may be at most %d" % (MAX_CANDIDATES - 1))
     nn.bind(vectors, math)
     n = int(vectors.shape[0])
     q = nn.queries(np.arange(n), np.ones(n, dtype=np.float32), np.arange(n + 1))
-    idx, val = nn.search(q, topn, exclude_self=True)
+    return nn.search(q, topn, exclude_self=True)
+
+
+def nearest_rows(nn: NearestNeighbours, vectors, topn: int, math: int):
+    """nearest_rows_device with (ids, values) on the host."""
+    idx, val = nearest_rows_device(nn, vectors, topn, math)
     return idx.cpu().numpy(), val.cpu().numpy()

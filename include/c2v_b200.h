@@ -682,6 +682,16 @@ int64_t c2v_reader_eval_queued(const c2v_reader* r);
 int c2v_reader_eval_score(const c2v_reader* r, const int32_t* ids, int32_t n, int32_t k, const int64_t* name_off,
                           const char* names, int32_t* rank, int32_t* first, int32_t* flags, int64_t* acc, void* stream);
 
+/* Checks the names of the last `rows` queued rows (0 <= rows <= c2v_reader_eval_queued; after an append, the rows it
+ * added) against Python's strict UTF-8 decoder: no overlong forms, no surrogates, nothing above U+10FFFF.  *name_len
+ * (host) = -1 when every name is valid; otherwise the length of the first invalid name in queue order, whose first
+ * min(len, name_cap) bytes go to name (host), so the caller can raise the decoder's own error from them.  Synchronises. */
+int c2v_reader_eval_check_utf8(c2v_reader* r, int64_t rows, char* name, int64_t name_cap, int64_t* name_len, void* stream);
+
+/* The target-word bytes of the tables (device memory of the handle, valid until the tables are replaced or the handle
+ * destroyed): word i is (*words)[(*word_off)[i], (*word_off)[i + 1]) for i < *n_words.  C2V_ERR_STATE before the tables. */
+int c2v_reader_eval_words(const c2v_reader* r, const char** words, const int64_t** word_off, int32_t* n_words);
+
 /* ---- Text of float32 matrices (DESIGN.md §6f) -----------------------------------------------------------------------
  * The lines of `<test file>.vectors` (model_base._write_code_vectors) and of word2vec files (common.save_word2vec_file),
  * formatted on the device.  Every value is written as numpy's str(np.float32(x)) writes it: "nan", "inf", "-inf",
@@ -905,6 +915,34 @@ int c2v_pred_format(c2v_pred* h, int32_t n, const int32_t* idx, const float* val
  * padded with NUL bytes, and its length to len[i] (host). */
 #define C2V_FIXED_BYTES 48
 int c2v_selftest_format_fixed(const float* x, int64_t n, char* out, int32_t* len);
+
+/* ---- Corpus text (DESIGN.md §6o) --------------------------------------------------------------------------------------
+ * The lines of `<corpus>.name_scores` (name_scores.format_line) and `<corpus>.nearest` (similarity.format_nearest_line)
+ * formatted on the device, byte for byte.  Names and words are bytes, copied as they are; floats are Python's '%f' of
+ * the float32 ("nan", "inf", "-inf", "-0.000000" as the host prints them); integers are '%d'.  Lines go back to back
+ * from out[0] (device) when all of them fit out_cap bytes, and *total (host, page-locked: written asynchronously, valid
+ * once `stream` has completed) gets their length either way.  scratch (device) holds at least
+ * c2v_corpus_text_scratch_bytes(rows) bytes for the rows of one call.  No engine handle is needed; failures return a
+ * negative c2v_status with the message in c2v_last_error(NULL).  Asynchronous on `stream`. */
+size_t c2v_corpus_text_scratch_bytes(int64_t rows);
+
+/* n >= 1 rows of name scores, all arrays device memory: row r's name is names[name_off[r], name_off[r + 1]) (as
+ * c2v_reader_eval_take writes them), its line `name\trank\tlogp\ttop1_name\ttop1_logp\n` from target / rank / logp / top1
+ * / top1_logp [n] (c2v_name_scores' outputs for the targets).  A row whose target is `oov` prints '-' for its rank and
+ * logp; rank 0 prints '-'.  top1_name is words[word_off[top1], word_off[top1 + 1]) (c2v_reader_eval_words), the OOV
+ * word for a top1 outside [0, n_words). */
+int c2v_name_scores_text(int32_t n, const char* names, const int64_t* name_off, const int32_t* target, int32_t oov,
+                         const int32_t* rank, const float* logp, const int32_t* top1, const float* top1_logp,
+                         const char* words, const int64_t* word_off, int32_t n_words, void* scratch, size_t scratch_bytes,
+                         char* out, int64_t out_cap, int64_t* total, void* stream);
+
+/* Lines [first, first + n) of a corpus of `rows` rows (rows < 2^31), all arrays device memory: row r's name is
+ * names[name_off[r], name_off[r + 1]) (name_off [rows + 1]), its neighbours idx / val [rows, k] (c2v_knn_search's
+ * outputs).  Line r is the name, then `\t<id>,<name of id>,<val>` for each neighbour in order; the INT_MAX padding
+ * (any id outside [0, rows)) is skipped. */
+int c2v_nearest_text(int64_t first, int64_t n, int64_t rows, int32_t k, const char* names, const int64_t* name_off,
+                     const int32_t* idx, const float* val, void* scratch, size_t scratch_bytes, char* out, int64_t out_cap,
+                     int64_t* total, void* stream);
 
 #ifdef __cplusplus
 }
